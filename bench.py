@@ -231,7 +231,7 @@ def headline_config(seeds_total, world, envs, with_eval=False, env_sharded=False
         return {"workload": f"Breakout-MinAtar pqn_minatar NUM_ENVS={envs} x {seeds_total} seeds, envs sharded "
                             f"{envs // world}/GPU (every rank trains every seed), TEST_DURING_TRAINING=False",
                 "num_steps": NUM_STEPS, "num_minibatches": 32, "num_epochs": 2,
-                "l2": "per-step working set exceeds the 126 MB L2" if seeds_total * envs >= 1 << 16 else
+                "l2": "per-step working set exceeds the 50 MB L2" if seeds_total * envs >= 1 << 16 else
                       "small run: the working set fits the L2; launch/latency bound",
                 "parallelism": f"env-sharded x{world}: one NCCL all-reduce (mean) of the flat [S][P] gradient per "
                                f"minibatch step (64 per update), per-rank minibatch permutation"}
@@ -240,7 +240,7 @@ def headline_config(seeds_total, world, envs, with_eval=False, env_sharded=False
                         + ("True (greedy eval of 128 envs x 1000 steps every 3 updates inside the timed "
                            "region; its env-steps are not counted)" if with_eval else "False"),
             "num_steps": NUM_STEPS, "num_minibatches": 32, "num_epochs": 2,
-            "l2": "per-step working set (obs rows + activations, >2 GB) exceeds the 126 MB L2",
+            "l2": "per-step working set (obs rows + activations, >2 GB) exceeds the 50 MB L2",
             "parallelism": f"seed-sharded x{world}, no data-path collective"}
 
 
@@ -293,24 +293,12 @@ def load_peaks():
         return {}
 
 
-def load_traffic():
-    """dram bytes per launch of each kernel id from the committed `ncu --set full` capture of this round
-    (profiles/r2_traffic.json: {kernel id: bytes}); empty if the file is absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-    except Exception:
-        return {}
-
-
-def roofline_for(dom, prof, S, envs, peaks, traffic, headline_geometry):
+def roofline_for(dom, prof, S, envs, peaks):
     d_ms, d_n = prof[dom]
     k = KERNELS.get(dom)
-    hbm = peaks.get("hbm_gbs", 6650.0)
-    peak_src_h = "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6.65 TB/s (of fallback)"
-    base = {"kernel": dom, "avg_launch_ms": round(d_ms / d_n, 4), "launches": d_n,
-            "traffic": traffic.get(dom) if headline_geometry else None,
-            "traffic_source": "profiles/r2_traffic.json (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum "
-                              "per launch, same workload)" if (headline_geometry and dom in traffic) else None}
+    hbm = peaks.get("hbm_gbs", 3350.0)
+    peak_src_h = "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 3.35 TB/s (H100 SXM data sheet)"
+    base = {"kernel": dom, "avg_launch_ms": round(d_ms / d_n, 4), "launches": d_n}
     if k is None:
         return {"bound": "hbm", "achieved": None, "peak": hbm, "unit": "GB/s", "frac": None, **base}
     mb = NUM_STEPS * envs // 32
@@ -320,14 +308,14 @@ def roofline_for(dom, prof, S, envs, peaks, traffic, headline_geometry):
         return {"bound": "hbm", "achieved": round(gbs, 1), "peak": hbm, "unit": "GB/s", "frac": round(gbs / hbm, 4),
                 "peak_source": peak_src_h, "alg_bytes_per_unit": k["bytes"], "units_per_launch": units,
                 "note": k.get("note", ""), **base}
-    peak = peaks.get("bf16_tflops_sustained") or 1400.0
+    peak = peaks.get("bf16_tflops_sustained") or 989.0
     tf = k["flops"] * units / (d_ms / d_n / 1e3) / 1e12
     gbs = k["bytes"] * units / (d_ms / d_n / 1e3) / 1e9
     return {"bound": "tensor", "achieved": round(tf, 2), "peak": peak, "unit": "TFLOP/s", "frac": round(tf / peak, 4),
             "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks
-                            else "fallback 1.4 PF sustained (of fallback)"),
+                            else "fallback 989 TFLOP/s dense BF16 (H100 SXM data sheet)"),
             "alg_flops_per_unit": k["flops"], "units_per_launch": units,
-            "note": "fp32-accurate split-precision GEMM on tcgen05 (3 tensor-core products per algorithmic one); the "
+            "note": "fp32-accurate split-precision GEMM on wgmma (3 tensor-core products per algorithmic one); the "
                     "fraction is algorithmic fp32 FLOP/s against the dense bf16 peak -- see DESIGN.md section 3 for the "
                     "format-equivalent peak",
             "hbm_gbs": round(gbs, 1), "hbm_frac": round(gbs / hbm, 4), **base}
@@ -340,7 +328,7 @@ def env_step_roofline(dev, local_rank, peaks, names=("Breakout-MinAtar",)):
     import torch
     from purejaxql_b200 import _lib, envs, jaxrandom as jr
     L = _lib.lib()
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)
     out = {}
     for name in names:
         n = (1 << 20) if name.endswith("MinAtar") else (1 << 24)
@@ -380,7 +368,7 @@ def env_step_roofline(dev, local_rank, peaks, names=("Breakout-MinAtar",)):
                      "avg_launch_ms": round(ms, 4), "launches": iters, "alg_bytes_per_env_step": bytes_per,
                      "env_steps_per_s": n / (ms * 1e-3), "achieved": round(gbs, 1), "peak": hbm, "unit": "GB/s",
                      "frac": round(gbs / hbm, 4), "clocks": clocks,
-                     "l2": f"state + outputs of {n} envs ({bytes_per * n / 1e6:.0f} MB per launch) exceed the 126 MB L2"}
+                     "l2": f"state + outputs of {n} envs ({bytes_per * n / 1e6:.0f} MB per launch) exceed the 50 MB L2"}
         del o, r, d, i0, i1, i2, i3, st, keys, act
     return out
 
@@ -437,6 +425,29 @@ def timed_train(module, cfg, rngs_host, warmup, dev, world, local_rank, profile=
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return float(t.item()), int(launches), clocks, out, prof, eng
+
+
+DUMP_PARAMS_MAX = 4 << 20    # parameters written in full up to this many values (16 MB), else a fixed sample of it
+
+
+def dump_outputs(path, out):
+    """What a caller of train() receives from the timed run: every metric ([seeds, updates]) and the final parameters
+    ([seeds, P] flat), float32 (float64 where the engine returns it).  128 seeds of the CNN hold ~17 M parameters, so
+    above DUMP_PARAMS_MAX a seeded sample of DUMP_PARAMS_MAX flat positions is written with its positions
+    (params_index.npy, float64), keeping the directory well under 64 MB."""
+    os.makedirs(path, exist_ok=True)
+
+    def host(t):
+        a = t.detach().cpu().numpy()
+        return a if a.dtype in (np.float32, np.float64) else a.astype(np.float64)
+    for k, v in out["metrics"].items():
+        np.save(os.path.join(path, "metrics_" + k.replace("/", "_") + ".npy"), host(v))
+    params = host(out["runner_state"][0].params_flat).reshape(-1)
+    if params.size > DUMP_PARAMS_MAX:
+        idx = np.sort(np.random.default_rng(0).choice(params.size, DUMP_PARAMS_MAX, replace=False))
+        np.save(os.path.join(path, "params_index.npy"), idx.astype(np.float64))
+        params = params[idx]
+    np.save(os.path.join(path, "params.npy"), params)
 
 
 E2E_PARTS = {}     # wall-clock split of the last e2e_train call (this rank)
@@ -509,6 +520,8 @@ def run_gpu(args, rank, world, local_rank):
     ms_max, launches, clocks, out, _, eng = timed_train(pqn_minatar, cfg, rngs_host, args.warmup, dev, world, local_rank,
                                                         shard=shard)
     graph_used = bool(eng.graph_captured)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     env_steps = seeds_total * args.steps * NUM_STEPS * args.envs
     value = env_steps / (ms_max / 1e3)
 
@@ -525,19 +538,17 @@ def run_gpu(args, rank, world, local_rank):
     if rank != 0:
         return
     peaks = load_peaks()
-    traffic = load_traffic()
-    headline_geometry = (S == 128 and args.envs == NUM_ENVS)
     total_k_ms = sum(v[0] for v in prof.values()) or 1.0
     breakdown = {k: {"ms_per_update": round(v[0] / 2, 3), "launches_per_update": v[1] // 2,
                      "share": round(v[0] / total_k_ms, 4)}
                  for k, v in sorted(prof.items(), key=lambda kv: -kv[1][0])}
     dom = max(prof.items(), key=lambda kv: kv[1][0])[0] if prof else None
-    roof = roofline_for(dom, prof, S, args.envs, peaks, traffic, headline_geometry) if dom else None
+    roof = roofline_for(dom, prof, S, args.envs, peaks) if dom else None
     if roof is not None:
         roof["measured_in"] = ("second pass of the same workload inside this bench.py run (2 eager updates, every "
                                "launch bracketed by CUDA events on the launching stream); profiled step = "
                                f"{p_ms / 2:.1f} ms vs {ms_max / args.steps:.1f} ms unprofiled")
-    rooflines = {k: roofline_for(k, prof, S, args.envs, peaks, traffic, headline_geometry)
+    rooflines = {k: roofline_for(k, prof, S, args.envs, peaks)
                  for k in prof if k in KERNELS and k != dom}
 
     # ---- (4) standalone env.step against the HBM roofline, with its own clock samples
@@ -587,7 +598,7 @@ def run_gpu(args, rank, world, local_rank):
 # the other BASELINE configs (each prints its own line; not the driver's headline)
 # --------------------------------------------------------------------------- #
 def run_acrobot(args, rank, world, local_rank):
-    """BASELINE configs[3]: Acrobot-v1 pqn_gymnax NUM_ENVS=65536 fp32 on one B200 (TOTAL_TIMESTEPS overridden,
+    """BASELINE configs[3]: Acrobot-v1 pqn_gymnax NUM_ENVS=65536 fp32 on one H100 (TOTAL_TIMESTEPS overridden,
     SURVEY 8: the shipped value gives 0 updates)."""
     import torch
     torch.cuda.set_device(local_rank)
@@ -622,7 +633,7 @@ def run_acrobot(args, rank, world, local_rank):
             "config": {"workload": f"Acrobot-v1 pqn_gymnax (pqn_cartpole.yaml) NUM_ENVS={E}, NUM_STEPS={T}, "
                                    f"{c['NUM_MINIBATCHES']} minibatches x {c['NUM_EPOCHS']} epochs, MLP "
                                    f"{c.get('HIDDEN_SIZE')}x{c.get('NUM_LAYERS')}, 1 seed",
-                       "l2": "rollout buffers + activations of 4.2 M samples per update exceed the 126 MB L2"},
+                       "l2": "rollout buffers + activations of 4.2 M samples per update exceed the 50 MB L2"},
             "clocks": clocks,
             "e2e": {"value": env_steps / e2e_s, "unit": UNIT, "h2d_bytes_per_step": h2d / args.steps,
                     "d2h_bytes_per_step": d2h / args.steps},
@@ -632,7 +643,7 @@ def run_acrobot(args, rank, world, local_rank):
 
 
 def run_minatar5(args, rank, world, local_rank):
-    """BASELINE configs[2]: the MinAtar suite at NUM_ENVS=1024 x 16 seeds on one B200 -- one line per game that gymnax
+    """BASELINE configs[2]: the MinAtar suite at NUM_ENVS=1024 x 16 seeds on one H100 -- one line per game that gymnax
     0.0.6 registers (Seaquest-MinAtar is not registered there; DESIGN.md section 8)."""
     import torch
     torch.cuda.set_device(local_rank)
@@ -679,6 +690,9 @@ def main():
     ap.add_argument("--data-parallel", default="auto", choices=["auto", "seeds", "envs"],
                     help="seeds: shard the independent seeds (no collective); envs: shard NUM_ENVS of every seed and "
                          "all-reduce the gradient once per minibatch step; auto: envs when --seeds < #GPUs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed train() returned (metrics of every update, a fixed "
+                         "sample of the final parameters) as DIR/<name>.npy, for output-for-output comparisons of builds")
     ap.add_argument("--with-eval", action="store_true",
                     help="TEST_DURING_TRAINING=True with the reference's cadence (SURVEY 8(d): report both)")
     args = ap.parse_args()

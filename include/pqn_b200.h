@@ -1,4 +1,4 @@
-/* libpqn_b200.so — C ABI of the B200-native PQN rollout-and-update hot path.
+/* libpqn_b200.so — C ABI of the H100-native (sm_90a) PQN rollout-and-update hot path.
  *
  * The reference (mttga/purejaxql) has no FFI boundary of its own: its hot path
  * is traced Python/JAX.  The entry points below are what a binding for that
@@ -258,34 +258,34 @@ int pqn_bn_stats_update(float* batch_stats, float* bn_sums, int32_t S, int32_t F
 
 /* Implementation selectors of the CNN (process-wide; the defaults are the fast paths, the others are kept as A/B
  * references for the parity tests):
- *  tensor-core path of the dense layer (forward, wgrad, dgrad): 2 (default) = tcgen05 kind::f16 on fp16-split (hi, lo')
- *  operand planes; 1 = tcgen05 3xTF32 with the lo operand derived in the kernel; 0 = fp32 FFMA kernels. */
+ *  tensor-core path of the dense layer (forward, wgrad, dgrad): 2 (default) = wgmma on fp16-split (hi, lo') operand
+ *  planes; 1 = 3xTF32 on mma.sync (the lo of the activation operand derived in the kernel); 0 = fp32 FFMA kernels.
+ *  Any other value is rejected (PQN_E_UNSUPPORTED). */
 int pqn_set_tensor_core_path(int on);
 /*  3x3 conv forward: 1 (default) = fp16 mma.sync (exponent-coded im2col bits, fp16-split weights); 3 = the tf32
- *  mma.sync kernel of round 1; 2 = tcgen05 (correct, slower: per-pixel epilogue); 0 = fp32 CUDA cores.  The conv
- *  weight gradient runs on tf32 mma.sync for 1-3. */
+ *  mma.sync kernel; 0 = fp32 CUDA cores; any other value is rejected (PQN_E_UNSUPPORTED).  The conv weight gradient
+ *  runs on mma.sync for 1 and 3. */
 int pqn_set_conv_mma_path(int on);
 
-/* ---- tcgen05 (5th-gen tensor core) path of the dense contractions ----------
+/* ---- tensor-core (sm_90a) paths of the dense contractions ----------
  * lo[i] = x[i] - trunc_tf32(x[i]): the error-compensation operand of 3xTF32. */
 int pqn_tc_split_lo(const float* x, float* lo, int64_t n, void* stream);
-/* Test hook: D[s] = A[s].B[s] through the TMA -> tcgen05.mma(kind::tf32) -> TMEM pipeline.
+/* Test hook: D[s] = A[s].B[s] through TMA -> mma.sync(tf32, fp32 accumulate).
  *  a_mn=0: A is [S][M][K]; a_mn=1: A is [S][K][M].  b_mn=0: B is [S][N][K]; b_mn=1: B is [S][K][N].
- *  split3: 3xTF32 with the *_lo operands from pqn_tc_split_lo; else one TF32 pass.  N % 128 == 0. */
+ *  split3: 1 = 3xTF32 with the *_lo operands from pqn_tc_split_lo; 2 = the same with A's lo derived in the kernel
+ *  (a_lo unused); 0 = one TF32 pass.  N % 128 == 0. */
 int pqn_tc_gemm_test(const float* a, const float* a_lo, const float* b, const float* b_lo, float* d, int32_t S,
                      int32_t M, int32_t N, int32_t K, int a_mn, int b_mn, int split3, void* stream);
 
-/* fp16-split planes for the default tensor-core path: hi = fp16(x*scale), lo = fp16((x*scale - hi) * 2^11), so that
+/* ----
+ * fp16-split planes: hi = fp16(x*scale), lo = fp16((x*scale - hi) * 2^11), so that
  * x*scale = hi + lo * 2^-11 to 22 significant bits (saturating at +-65000).  hi/lo: __half[n]. */
 int pqn_tc_split16(const float* x, void* hi, void* lo, int64_t n, float scale, void* stream);
-/* Test hook: D[s] = (A[s].B[s]) * out_scale through TMA -> tcgen05.mma(kind::f16) -> TMEM with the operands given as
- * (hi, lo) fp16 planes (3 products per k-step: hi.hi into the main accumulator, lo.hi + hi.lo into the 2^-11 one). */
+/* Test hook: D[s] = (A[s].B[s]) * out_scale through TMA -> wgmma(f16, fp32 accumulate) with the operands given as
+ * (hi, lo) fp16 planes (3 products per k-step: hi.hi into the main accumulator, lo.hi + hi.lo into the 2^-11 one).
+ *  a_mn=0: A is [S][M][K]; a_mn=1: A is [S][K][M].  b_mn=0: B is [S][N][K]; b_mn=1: B is [S][K][N].  N % 128 == 0. */
 int pqn_tc_gemm16_test(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, float* d, int32_t S,
                        int32_t M, int32_t N, int32_t K, int a_mn, int b_mn, float out_scale, void* stream);
-
-/* Debug hook: one 128x128x32 tile; dumps the TMA-written smem tiles and the TMEM accumulator. */
-int pqn_tc_debug(const float* a, const float* b, float* dump_a, float* dump_b, float* out_d, uint32_t* info,
-                 int a_mn, int b_mn, int nk, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,4 @@
-"""purejaxql_b200 — a B200-native (sm_100a) PQN rollout-and-update engine.
+"""purejaxql_b200 — an H100-native (sm_90a) PQN rollout-and-update engine.
 
 Host side: Python/PyTorch (device memory, streams, torch.distributed plumbing)
 calling hand-written CUDA through the C ABI of ``libpqn_b200.so``

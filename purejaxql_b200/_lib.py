@@ -88,11 +88,10 @@ _SIGS = {
     "pqn_set_conv_mma_path": (c_int, [c_int]),
     "pqn_tc_split_lo": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "pqn_tc_split16": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_float, c_void_p]),
-    "pqn_tc_gemm16_test": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
-                                   c_int32, c_int, c_int, c_float, c_void_p]),
-    "pqn_tc_debug": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pqn_tc_gemm_test": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                  c_int32, c_int, c_int, c_int, c_void_p]),
+    "pqn_tc_gemm16_test": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
+                                   c_int32, c_int, c_int, c_float, c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

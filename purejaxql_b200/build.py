@@ -1,4 +1,4 @@
-"""Builds libpqn_b200.so in-tree with nvcc for sm_100a.
+"""Builds libpqn_b200.so in-tree with nvcc for sm_90a.
 
     python -m purejaxql_b200.build [--force]
 
@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libpqn_b200.so")
 BUILD = os.path.join(HERE, "csrc", "_build")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 UNITS = [
     ("pqn_api.cu", []),

@@ -31,7 +31,7 @@ int device_sm_count() {
   cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && cache[dev] > 0) return cache[dev];
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   if (dev >= 0 && dev < 64) cache[dev] = n;
   return n;
 }

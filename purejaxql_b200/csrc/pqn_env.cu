@@ -1,4 +1,4 @@
-// Batched environment operator + fused rollout step for sm_100a.
+// Batched environment operator + fused rollout step for sm_90a.
 //
 // Kernels here are HBM-bound integer/byte work: one env per thread, state in
 // registers for the duration of the step, word-major SoA state (128-byte

@@ -1,4 +1,4 @@
-// Q-network forward / loss-gradient kernels for sm_100a, batched over S
+// Q-network forward / loss-gradient kernels for sm_90a, batched over S
 // independent seeds (blockIdx.y or .z = seed; every seed has its own weights).
 //
 // Reference: QNetwork/CNN  purejaxql/pqn_minatar.py:24-69,
@@ -28,11 +28,11 @@ constexpr int CONV_PIX = 64; // 8x8 output pixels
 constexpr int HID_CNN = 128;
 constexpr int FLAT_CNN = CONV_PIX * CONV_O;  // 1024
 
-// tcgen05 path for the CNN dense layer (pqn_set_tensor_core_path); default on
-static int g_use_tc = 2;  // 0 FFMA, 1 tcgen05 3xTF32 (A_lo derived in the kernel), 2 tcgen05 fp16-split planes (default)
+// wgmma path for the CNN dense layer (pqn_set_tensor_core_path); default on
+static int g_use_tc = 2;  // 0 FFMA, 1 3xTF32 on mma.sync (A_lo derived in the kernel), 2 wgmma on fp16-split planes (default)
 // warp-level tensor-core (mma.sync tf32) conv kernels (pqn_set_conv_mma_path); default on
-static int g_conv_mma = 1;   // 0: fp32 CUDA cores, 1: fp16 mma.sync forward (default), 2: tcgen05 forward, 3: tf32 mma.sync forward
-                             // (1-3: tf32 mma.sync backward)
+static int g_conv_mma = 1;   // 0: fp32 CUDA cores, 1: fp16 mma.sync forward (default), 3: tf32 mma.sync forward
+                             // (1, 3: mma.sync backward)
 
 static inline int64_t align4(int64_t x) { return (x + 3) & ~(int64_t)3; }
 
@@ -801,7 +801,7 @@ __global__ void __launch_bounds__(256) conv_fwd_kernel(const uint32_t* __restric
       v.z = fmaxf((acc[4 * o4 + 2] - mean) * rstd * sc[4 * o4 + 2] + bi[4 * o4 + 2], 0.f);
       v.w = fmaxf((acc[4 * o4 + 3] - mean) * rstd * sc[4 * o4 + 3] + bi[4 * o4 + 3], 0.f);
       out[o4] = v;
-      if (H1LO != nullptr) {  // 3xTF32 error-compensation operand for the tcgen05 GEMMs
+      if (H1LO != nullptr) {  // 3xTF32 error-compensation operand
         float4* __restrict__ olo =
             reinterpret_cast<float4*>(H1LO + ((int64_t)seed * rows + row) * FLAT_CNN + pix * CONV_O);
         olo[o4] = make_float4(tc::tf32_lo(v.x), tc::tf32_lo(v.y), tc::tf32_lo(v.z), tc::tf32_lo(v.w));
@@ -1350,7 +1350,7 @@ struct Conv16 {
 // Output channel of column n (0..7) of n-tile h.  NOT the natural 8h + n: with 4 (n / 2) + 2h + (n % 2) the accumulator
 // columns (2t, 2t+1) of the two n-tiles are the four CONSECUTIVE channels 4t .. 4t+3 of a pixel, so a thread stores 16
 // bytes of xhat / 8 bytes of each fp16 plane per pixel with one instruction and no lane exchange (the kernel's time
-// follows its store instructions: same-box A/B in profiles/r2_conv_fwd_sensitivity.json).
+// follows its store instructions).
 __host__ __device__ constexpr int conv16_channel(int h, int n) { return 4 * (n >> 1) + 2 * h + (n & 1); }
 
 // tap of fragment column kk (0..15) of k-step s, see the k order above
@@ -2211,256 +2211,6 @@ __global__ void conv_bwd_final_kernel(const float* __restrict__ part, int nctas,
   else gout[L.conv_b + (i - taps16 - 2 * CONV_O)] = v;
 }
 
-// ---------------------------------------------------------------------------
-// conv forward on tcgen05: per tile of 2 samples (128 output pixels) the 128 producer threads (thread = pixel)
-// write their im2col row ({0,1} floats, taps padded to a multiple of 32) straight into shared memory in the
-// K-major SWIZZLE_128B operand layout, one elected thread issues tcgen05.mma M=128 x N=16 x K=8 per 8 taps
-// against the (hi, lo)-split weights/255 held in shared memory, and the same 128 threads read their pixel's 16
-// channels back from TMEM for LayerNorm + ReLU and the stores.  A tiles and TMEM accumulators are double
-// buffered: tile i+1 is produced while tile i's MMAs run.
-// ---------------------------------------------------------------------------
-template <int C>
-struct ConvTc {
-  static constexpr int TAPS = 9 * C;
-  static constexpr int KB = (TAPS + 31) / 32;           // k-blocks of 32 taps (one 128-byte swizzle row each)
-  static constexpr int KS = (TAPS + 7) / 8;             // MMA k-steps
-  static constexpr int A_TILE = 128 * 128;              // bytes per k-block tile (128 rows x 128 B)
-  static constexpr int A_BUF = KB * A_TILE;
-  static constexpr int B_TILE = 16 * 128;               // 16 output channels x 128 B
-  static constexpr int OFF_A = 0;                       // 2 buffers
-  static constexpr int OFF_BHI = 2 * A_BUF;
-  static constexpr int OFF_BLO = OFF_BHI + KB * B_TILE;
-  static constexpr int OFF_MISC = OFF_BLO + KB * B_TILE;  // barriers, tmem slot, obs words, consts
-  static constexpr int SMEM = OFF_MISC + 1024 + 1024 /*align slack*/;
-};
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void bar_sync_named(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-template <int C, bool TRAIN>
-__global__ void __launch_bounds__(160)
-    conv_fwd_tc_kernel(const uint32_t* __restrict__ obs, int64_t obs_rows_per_seed, const int32_t* __restrict__ gather,
-                       const float* __restrict__ params, int64_t P, pqn_net_layout_t L, float* __restrict__ H1,
-                       float* __restrict__ H1LO, float* __restrict__ XH1, float* __restrict__ RS1,
-                       float* __restrict__ bn_sums, int rows, int tiles_per_seed, int ctas_per_seed) {
-  using Cfg = ConvCfg<C>;
-  using T = ConvTc<C>;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t sbase = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (sbase - tc::smem_u32(smem_raw));
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(sm + T::OFF_MISC);  // [2]
-  uint64_t* d_full = a_full + 2;                                      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_full + 2);
-  float* cb = reinterpret_cast<float*>(sm + T::OFF_MISC + 64);       // [16] conv bias, LN scale, LN bias
-  float* sc = cb + CONV_O;
-  float* bi = sc + CONV_O;
-  float* s_cnt = bi + CONV_O;                                         // [C]
-  uint32_t* sobs = reinterpret_cast<uint32_t*>(sm + T::OFF_MISC + 320);  // [2 buf][2 samples][SW]
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int seed = blockIdx.y;
-  const float* __restrict__ prm = params + (int64_t)seed * P;
-
-  // ---- one-time setup: weights (hi, lo) as K-major SW128 B tiles, constants, barriers, TMEM
-  {
-    const float inv255 = 1.0f / 255.0f;
-    for (int i = tid; i < T::KB * 16 * 32; i += blockDim.x) {
-      const int kb = i / (16 * 32), n = (i / 32) % 16, kk = i % 32;
-      const int tap = kb * 32 + kk;
-      const float w = tap < T::TAPS ? __ldg(prm + L.conv_w + tap * CONV_O + n) * inv255 : 0.f;
-      const float hi = __uint_as_float(__float_as_uint(w) & 0xFFFFE000u);
-      const int off = kb * T::B_TILE + n * 128 + ((((kk >> 2) ^ (n & 7)) << 4) | ((kk & 3) << 2));
-      *reinterpret_cast<float*>(sm + T::OFF_BHI + off) = hi;
-      *reinterpret_cast<float*>(sm + T::OFF_BLO + off) = w - hi;
-    }
-    if (tid < CONV_O) {
-      cb[tid] = __ldg(prm + L.conv_b + tid);
-      sc[tid] = __ldg(prm + L.ln0_scale + tid);
-      bi[tid] = __ldg(prm + L.ln0_bias + tid);
-    }
-    if (tid < C) s_cnt[tid] = 0.f;
-    if (tid == 128) {
-      for (int b = 0; b < 2; ++b) { tc::mbar_init(&a_full[b], 128); tc::mbar_init(&d_full[b], 1); }
-      tc::fence_barrier_init();
-    }
-    if (warp == 4) { tc::tmem_alloc(tmem_slot, 32); tc::tmem_relinquish(); }
-    fence_proxy_async_smem();
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    tc::tcgen05_fence_after();
-  }
-  const uint32_t tmem_base = *tmem_slot;
-  const int n_iters = (tiles_per_seed - (int)blockIdx.x + ctas_per_seed - 1) / ctas_per_seed;  // tiles of this CTA
-
-  if (warp == 4) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = tc::make_idesc_tf32(128, 16, 0, 0);
-      for (int it = 0; it < n_iters; ++it) {
-        const int b = it & 1;
-        tc::mbar_wait(&a_full[b], (it >> 1) & 1);
-        tc::tcgen05_fence_after();
-        const uint32_t d = tmem_base + b * 16;
-        const uint32_t abase = sbase + T::OFF_A + b * T::A_BUF;
-#pragma unroll
-        for (int ks = 0; ks < T::KS; ++ks) {
-          const int kb = ks >> 2, kq = ks & 3;
-          const uint64_t da = tc::make_sdesc<0>(abase + kb * T::A_TILE, kq);
-          const uint64_t dlo = tc::make_sdesc<0>(sbase + T::OFF_BLO + kb * T::B_TILE, kq);
-          const uint64_t dhi = tc::make_sdesc<0>(sbase + T::OFF_BHI + kb * T::B_TILE, kq);
-          tc::umma_tf32(d, da, dlo, idesc, ks > 0 ? 1u : 0u);
-          tc::umma_tf32(d, da, dhi, idesc, 1u);
-        }
-        tc::umma_commit(&d_full[b]);
-      }
-    }
-  } else {
-    // ===================== producers / epilogue: thread = output pixel of the 2-sample tile =====================
-    const int sl = tid >> 6, pix = tid & 63, y = pix >> 3, x = pix & 7;
-    int cnt[C];
-#pragma unroll
-    for (int c = 0; c < C; ++c) cnt[c] = 0;
-
-    // observation word of this thread for tile `it` (issued one iteration ahead to hide the HBM latency)
-    auto fetch_word = [&](int it) -> uint32_t {
-      const int row = (blockIdx.x + it * ctas_per_seed) * 2 + sl;
-      if (it < n_iters && row < rows && pix < Cfg::PW) {
-        const int64_t src = gather ? gather[(int64_t)seed * rows + row] : row;
-        return __ldg(obs + ((int64_t)seed * obs_rows_per_seed + src) * Cfg::PW + pix);
-      }
-      return 0u;
-    };
-    uint32_t w_next = fetch_word(0);
-
-    auto produce = [&](int it) {
-      const int b = it & 1;
-      const int tile = blockIdx.x + it * ctas_per_seed;
-      const int row = tile * 2 + sl;
-      uint32_t* so = sobs + (b * 2 + sl) * Cfg::SW;
-      if (pix < Cfg::SW) so[pix] = w_next;
-      w_next = fetch_word(it + 1);
-      bar_sync_named(1, 128);
-      // im2col row of this pixel: taps (di,dj,c) -> {0,1}
-      float f[T::KB * 32];
-#pragma unroll
-      for (int k = 0; k < T::KB * 32; ++k) f[k] = 0.f;
-#pragma unroll
-      for (int r = 0; r < 9; ++r) {
-        const uint32_t nib = pixel_bits<C>(so, (y + r / 3) * 10 + x + r % 3);
-#pragma unroll
-        for (int c = 0; c < C; ++c) f[r * C + c] = ((nib >> c) & 1u) ? 1.0f : 0.0f;
-      }
-      uint8_t* arow = sm + T::OFF_A + b * T::A_BUF + tid * 128;
-#pragma unroll
-      for (int kb = 0; kb < T::KB; ++kb)
-#pragma unroll
-        for (int c16 = 0; c16 < 8; ++c16)
-          *reinterpret_cast<float4*>(arow + kb * T::A_TILE + ((c16 ^ (tid & 7)) << 4)) =
-              make_float4(f[kb * 32 + 4 * c16], f[kb * 32 + 4 * c16 + 1], f[kb * 32 + 4 * c16 + 2], f[kb * 32 + 4 * c16 + 3]);
-      if (TRAIN && bn_sums != nullptr && row < rows) {
-        const uint32_t b0 = pixel_bits<C>(so, pix);
-        const uint32_t b1 = (pix + 64 < 100) ? pixel_bits<C>(so, pix + 64) : 0u;
-#pragma unroll
-        for (int c = 0; c < C; ++c) cnt[c] += (int)((b0 >> c) & 1u) + (int)((b1 >> c) & 1u);
-      }
-      fence_proxy_async_smem();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc::mbar_arrive(&a_full[b]);
-    };
-
-    auto epilogue = [&](int it) {
-      const int b = it & 1;
-      const int tile = blockIdx.x + it * ctas_per_seed;
-      const int row = tile * 2 + sl;
-      tc::mbar_wait(&d_full[b], (it >> 1) & 1);
-      tc::tcgen05_fence_after();
-      uint32_t v[16];
-      tmem_ld_32x32b_x16(tmem_base + b * 16 + ((uint32_t)(warp * 32) << 16), v);
-      tc::tmem_ld_wait();
-      tc::tcgen05_fence_before();
-      float z[CONV_O];
-#pragma unroll
-      for (int o = 0; o < CONV_O; ++o) z[o] = __uint_as_float(v[o]) + cb[o];
-      float mean, rstd;
-      ln16(z, mean, rstd);
-      if (row < rows) {
-        const int64_t base = ((int64_t)seed * rows + row) * FLAT_CNN + pix * CONV_O;
-#pragma unroll
-        for (int o4 = 0; o4 < CONV_O / 4; ++o4) {
-          float xh[4], hv[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            xh[j] = (z[4 * o4 + j] - mean) * rstd;
-            hv[j] = fmaxf(xh[j] * sc[4 * o4 + j] + bi[4 * o4 + j], 0.f);
-          }
-          *reinterpret_cast<float4*>(H1 + base + 4 * o4) = make_float4(hv[0], hv[1], hv[2], hv[3]);
-          if (H1LO)
-            *reinterpret_cast<float4*>(H1LO + base + 4 * o4) =
-                make_float4(tc::tf32_lo(hv[0]), tc::tf32_lo(hv[1]), tc::tf32_lo(hv[2]), tc::tf32_lo(hv[3]));
-          if (TRAIN && XH1) *reinterpret_cast<float4*>(XH1 + base + 4 * o4) = make_float4(xh[0], xh[1], xh[2], xh[3]);
-        }
-        if (TRAIN && RS1) RS1[((int64_t)seed * rows + row) * CONV_PIX + pix] = rstd;
-      }
-    };
-
-    if (n_iters > 0) produce(0);
-    for (int it = 1; it < n_iters; ++it) {
-      produce(it);
-      epilogue(it - 1);
-    }
-    if (n_iters > 0) epilogue(n_iters - 1);
-
-    if (TRAIN && bn_sums != nullptr) {
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        int vsum = cnt[c];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) vsum += __shfl_xor_sync(0xffffffffu, vsum, o);
-        if (lane == 0 && vsum) atomicAdd(&s_cnt[c], (float)vsum);
-      }
-    }
-  }
-  tc::tcgen05_fence_before();
-  __syncthreads();
-  if (TRAIN && bn_sums != nullptr && tid < C && s_cnt[tid] != 0.f) {
-    atomicAdd(bn_sums + (int64_t)seed * 2 * C + tid, s_cnt[tid]);
-    atomicAdd(bn_sums + (int64_t)seed * 2 * C + C + tid, s_cnt[tid]);
-  }
-  if (warp == 4) {
-    tc::tcgen05_fence_after();
-    tc::tmem_dealloc(tmem_base, 32);
-  }
-}
-
-template <int C, bool TRAIN>
-static int launch_conv_fwd_tc_t(int S, cudaStream_t st, const uint32_t* obs, int64_t orps, const int32_t* gather,
-                                const float* params, int64_t P, const pqn_net_layout_t& L, float* h1, float* h1lo,
-                                float* xh1, float* rs1, float* bn, int rows) {
-  auto kfn = conv_fwd_tc_kernel<C, TRAIN>;
-  if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, ConvTc<C>::SMEM) != cudaSuccess)
-    return check_launch("conv_fwd_tc(cudaFuncSetAttribute)");
-  const int tiles = (rows + 1) / 2;
-  // all CTAs co-resident (3 per SM by shared memory): a second partial wave would double the time
-  int per_seed = (148 * 3) / S;
-  if (per_seed > tiles) per_seed = tiles;
-  if (per_seed < 1) per_seed = 1;
-  {
-    LaunchScope _ls(TRAIN ? K_CONV_FWD : K_CONV_FWD_INFER, st);
-    kfn<<<dim3(per_seed, S), 160, ConvTc<C>::SMEM, st>>>(obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, bn, rows,
-                                                         tiles, per_seed);
-  }
-  return 0;
-}
-
 // MLP input gather (minibatch rows of float obs); the input BatchNorm sums come from nrm::colsum2 of the result.
 __global__ void gather_rows_kernel(const float* __restrict__ obs, int64_t obs_rows_per_seed,
                                    const int32_t* __restrict__ gather, float* __restrict__ out, int rows, int D) {
@@ -2479,9 +2229,9 @@ __global__ void gather_rows_kernel(const float* __restrict__ obs, int64_t obs_ro
 struct Workspace {
   // CNN
   float *h1, *h2, *xhat2, *rstd2, *dz2;
-  float *h1_lo, *dz2_lo, *w1_lo;  // 3xTF32 "lo" operands of the tcgen05 path
+  float *h1_lo, *dz2_lo, *w1_lo;  // 3xTF32 "lo" operands of the TF32 path; regions of the fp16-split planes (Planes16)
   float *cxhat, *crstd;           // conv LayerNorm xhat / rstd saved by the training forward (MMA conv path)
-  uint32_t* relu_bits;            // packed (h1 > 0) mask, 1024 bits per row (MMA conv path -> tcgen05 dgrad epilogue)
+  uint32_t* relu_bits;            // packed (h1 > 0) mask, 1024 bits per row (MMA conv path -> tensor-core dgrad epilogue)
   float *rb_part, *cb_part;       // per-CTA partial vectors of the deterministic row_bwd / conv_bwd reductions
   float* wg_part;                 // split-K partial outputs of the tensor-core weight gradient (small S: few output tiles)
   // MLP
@@ -2491,8 +2241,9 @@ struct Workspace {
 
 // split-K of the tensor-core weight gradient: when S * m_tiles * n_tiles output tiles cannot fill the SMs (one seed of
 // the MLP has 4 tiles, of the CNN 8), the K = rows range is divided so that one CTA per SM runs; the partial tiles
-// (at most WGRAD_SPLIT_TILES of them) are added in split order by wgrad_split_reduce_kernel (deterministic)
-constexpr int64_t WGRAD_SPLIT_TILES = 4 * 148 + 16;   // tensor-core split-K: <= SMs; FFMA row splits: tiles * S * splits < 4 * 148
+// (at most wgrad_split_tiles() of them) are added in split order by wgrad_split_reduce_kernel (deterministic)
+// tensor-core split-K: <= SMs tiles; FFMA row splits: tiles * S * splits < 4 * SMs
+static int64_t wgrad_split_tiles() { return 4 * (int64_t)device_sm_count() + 16; }
 static int wgrad_ksplit(int tiles_total, int k_blocks) {
   const int sms = device_sm_count();                 // persistent kernel, one CTA per SM: one wave of split tiles
   if (tiles_total >= sms) return 1;
@@ -2521,7 +2272,7 @@ static void launch_split_reduce(const float* part, int ksplit, int64_t split_str
 }
 
 // The register-tiled FFMA weight gradient + (splits > 1) its ordered reduction.  `part` needs splits * S * Kin * N floats
-// (<= WGRAD_SPLIT_TILES tiles of 128 x 128: wgrad_splits keeps tiles * S * splits below 4 * 148).
+// (<= wgrad_split_tiles() tiles of 128 x 128: wgrad_splits keeps tiles * S * splits below 4 * SMs).
 static void run_wgrad_ffma(const float* X, int64_t x_seed_stride, int ldx, const float* DZ, int64_t dz_seed_stride, int N,
                            float* grads, int64_t P, int64_t off_w, int rows, int Kin, int S, int splits, float* part,
                            cudaStream_t st) {
@@ -2647,7 +2398,7 @@ static int64_t carve(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* bas
     ww->relu_bits = reinterpret_cast<uint32_t*>(take(R * (FLAT_CNN / 32)));
     ww->rb_part = take(part_ctas(S) * row_bwd_part_floats(HID_CNN, d->num_actions));
     ww->cb_part = take(part_ctas(S) * (int64_t)(9 * d->in_c * CONV_O + 3 * CONV_O));
-    ww->wg_part = take(WGRAD_SPLIT_TILES * 128 * 128);
+    ww->wg_part = take(wgrad_split_tiles() * 128 * 128);
   } else {
     const int H = d->hidden;
     ww->xg = take(R * d->in_c);
@@ -2661,7 +2412,7 @@ static int64_t carve(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* bas
     ww->dh0 = take(R * H);
     ww->rb_part = take(part_ctas(S) * row_bwd_part_floats(H, d->num_actions));
     ww->cb_part = nullptr;
-    ww->wg_part = take(WGRAD_SPLIT_TILES * 128 * 128);
+    ww->wg_part = take(wgrad_split_tiles() * 128 * 128);
     ww->m16_h0 = take(R * H);                       // 2 planes x 2 bytes = 4 bytes per element
     ww->m16_w = take((int64_t)S * H * H);
     ww->m16_dz = take(R * H);
@@ -2793,16 +2544,6 @@ static int launch_conv_fwd(int C, dim3 grid, cudaStream_t st, const uint32_t* ob
                            const float* params, int64_t P, const pqn_net_layout_t& L, float* h1, float* h1lo, float* bn,
                            int rows, float* xh1 = nullptr, float* rs1 = nullptr, uint32_t* rb = nullptr,
                            bool h16 = false) {
-  if (g_conv_mma == 2) {
-    const int S = (int)grid.y;
-    switch (C) {
-      case 4: return launch_conv_fwd_tc_t<4, TRAIN>(S, st, obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, bn, rows);
-      case 6: return launch_conv_fwd_tc_t<6, TRAIN>(S, st, obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, bn, rows);
-      case 7: return launch_conv_fwd_tc_t<7, TRAIN>(S, st, obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, bn, rows);
-      case 10: return launch_conv_fwd_tc_t<10, TRAIN>(S, st, obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, bn, rows);
-      default: return -1;
-    }
-  }
   if (g_conv_mma == 1) {  // fp16 mma.sync conv (default); h16: h1 / h1lo are the fp16 (hi, lo') planes
     const dim3 mg(conv_mma_ctas((int)grid.y, rows, CONV16_CTAS_PER_SM), grid.y);
     LaunchScope _ls(TRAIN ? K_CONV_FWD : K_CONV_FWD_INFER, st);
@@ -2843,7 +2584,7 @@ static int launch_conv_fwd(int C, dim3 grid, cudaStream_t st, const uint32_t* ob
 
 // CTAs per seed for conv_bwd: ~4 waves of 2 CTAs/SM over all seeds, at most one sample-group per CTA
 static unsigned conv_bwd_ctas(int S, int rows) {
-  int per_seed = (148 * 2 * 4 + S - 1) / S;
+  int per_seed = (device_sm_count() * 2 * 4 + S - 1) / S;
   const int maxc = (rows + CONV_BWD_WARPS - 1) / CONV_BWD_WARPS;
   if (per_seed > maxc) per_seed = maxc;
   if (per_seed < 1) per_seed = 1;
@@ -2851,7 +2592,7 @@ static unsigned conv_bwd_ctas(int S, int rows) {
 }
 
 static int wgrad_splits(int tiles, int S, int rows) {
-  int s = (2 * 148 + tiles * S - 1) / (tiles * S);
+  int s = (2 * device_sm_count() + tiles * S - 1) / (tiles * S);
   const int maxs = (rows + 255) / 256;
   if (s > maxs) s = maxs;
   if (s < 1) s = 1;
@@ -2932,7 +2673,7 @@ static int tc16_dense_fwd(int epi, const float* params, int64_t P, const pqn_net
   if ((rc = tc::make_tmap16(&t[2], pl.w1_hi, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 64))) return rc;
   if ((rc = tc::make_tmap16(&t[3], pl.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 64))) return rc;
   tc::GemmShape gs = {};
-  gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = 1; gs.k_blocks = FLAT_CNN / tc::TC_BK16; gs.split3 = 1;
+  gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = 1; gs.k_blocks = FLAT_CNN / tc::TC_BK16;
   tc::EpiParams ep = {};
   ep.params = params; ep.P = P; ep.off_b = L.d0_b; ep.off_scale = L.ln1_scale; ep.off_bias = L.ln1_bias;
   ep.off_hw = L.head_w; ep.off_hb = L.head_b; ep.A = A; ep.rows = rows;
@@ -2950,7 +2691,7 @@ static int tc16_wgrad(float* grads, int64_t P, const pqn_net_layout_t& L, const 
   if ((rc = tc::make_tmap16(&t[3], pl.dz_lo, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 64))) return rc;
   tc::GemmShape gs = {};
   gs.S = S; gs.M = FLAT_CNN; gs.m_tiles = FLAT_CNN / 128; gs.n_tiles = 1;
-  gs.k_blocks = (rows + tc::TC_BK16 - 1) / tc::TC_BK16; gs.split3 = 1;
+  gs.k_blocks = (rows + tc::TC_BK16 - 1) / tc::TC_BK16;
   gs.k_split = wgrad_ksplit(S * gs.m_tiles * gs.n_tiles, gs.k_blocks);
   tc::EpiParams ep = {};
   ep.ld_out = HID_CNN; ep.out_scale = 1.0f / gscale;
@@ -2976,7 +2717,7 @@ static int tc16_dgrad(const Workspace& w, const Planes16& pl, int S, int rows, b
   if ((rc = tc::make_tmap16(&t[3], pl.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 128))) return rc;
   tc::GemmShape gs = {};
   gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = FLAT_CNN / 128; gs.k_blocks = HID_CNN / tc::TC_BK16;
-  gs.split3 = 1;
+ 
   tc::EpiParams ep = {};
   ep.out = w.h1; ep.mask = w.h1; ep.ld_out = FLAT_CNN; ep.out_seed_stride = (int64_t)rows * FLAT_CNN;
   ep.relu_bits = w.relu_bits; ep.rows = rows; ep.out_scale = 1.0f / gscale;
@@ -2995,7 +2736,7 @@ static int tc16_mm_store(const __half* a, int64_t a_plane, const __half* b, int6
   if ((rc = tc::make_tmap16(&t[3], b + b_plane, N, K, S, N, (uint64_t)K * N, 64))) return rc;
   tc::GemmShape gs = {};
   gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = N / 128; gs.k_blocks = (K + tc::TC_BK16 - 1) / tc::TC_BK16;
-  gs.split3 = 1;
+ 
   tc::EpiParams ep = {};
   ep.out = out; ep.ld_out = N; ep.out_seed_stride = (int64_t)rows * N;
   return tc::launch_gemm16(0, 1, tc::EPI_STORE, t, gs, ep, st, kid);
@@ -3010,7 +2751,7 @@ static int tc16_mm_wgrad(const __half* a, int64_t a_plane, const __half* dz, int
   if ((rc = tc::make_tmap16(&t[2], dz, N, rows, S, N, (uint64_t)rows * N, 64))) return rc;
   if ((rc = tc::make_tmap16(&t[3], dz + dz_plane, N, rows, S, N, (uint64_t)rows * N, 64))) return rc;
   tc::GemmShape gs = {};
-  gs.S = S; gs.M = M; gs.m_tiles = M / 128; gs.n_tiles = N / 128; gs.k_blocks = (rows + tc::TC_BK16 - 1) / tc::TC_BK16; gs.split3 = 1;
+  gs.S = S; gs.M = M; gs.m_tiles = M / 128; gs.n_tiles = N / 128; gs.k_blocks = (rows + tc::TC_BK16 - 1) / tc::TC_BK16;
   gs.k_split = wgrad_ksplit(S * gs.m_tiles * gs.n_tiles, gs.k_blocks);
   tc::EpiParams ep = {};
   ep.ld_out = N; ep.out_scale = out_scale;
@@ -3034,7 +2775,7 @@ static int tc16_mm_dgrad(const __half* dz, int64_t dz_plane, const __half* wgt, 
   if ((rc = tc::make_tmap16(&t[3], wgt + w_plane, N, Kp, S, N, (uint64_t)Kp * N, 128))) return rc;
   tc::GemmShape gs = {};
   gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = Kp / 128; gs.k_blocks = (N + tc::TC_BK16 - 1) / tc::TC_BK16;
-  gs.split3 = 1;
+ 
   tc::EpiParams ep = {};
   ep.out = out; ep.mask = mask; ep.ld_out = Kp; ep.out_seed_stride = (int64_t)rows * Kp; ep.rows = rows; ep.out_scale = out_scale;
   return tc::launch_gemm16(0, 0, tc::EPI_RELU_MASK, t, gs, ep, st, K_TC_DGRAD);
@@ -3045,18 +2786,18 @@ static void split16_rows(const float* src, int64_t src_seed_stride, int64_t n_pe
   split16_strided_kernel<<<dim3(cdiv(n_per_seed / 4, 256), S), 256, 0, st>>>(src, src_seed_stride, hi, lo, n_per_seed);
 }
 
-// Z = H1 . W1 on the tcgen05 path with the LayerNorm/ReLU(/head) epilogue.  epi = EPI_LN_TRAIN or EPI_LN_HEAD.
+// ---- 3xTF32 tensor-core path (g_use_tc == 1): mma.sync.tf32 on the TMA ring of the GEMM kernel -------------------
+// Z = H1 . W1 with the LayerNorm/ReLU(/head) epilogue.  epi = EPI_LN_TRAIN or EPI_LN_HEAD.
 static int tc_dense_fwd(int epi, const float* params, int64_t P, const pqn_net_layout_t& L, const Workspace& w, int A,
                         float* q, int S, int rows, cudaStream_t st) {
   CUtensorMap t[4];
   int rc;
-  if ((rc = tc::make_tmap(&t[0], w.h1, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 128, 0))) return rc;
-  if ((rc = tc::make_tmap(&t[1], w.h1_lo, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 128, 0))) return rc;
-  if ((rc = tc::make_tmap(&t[2], params + L.d0_w, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)P, 32, 1))) return rc;
-  if ((rc = tc::make_tmap(&t[3], w.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 32, 1))) return rc;
+  if ((rc = tc::make_tmap(&t[0], w.h1, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 128))) return rc;
+  if ((rc = tc::make_tmap(&t[1], w.h1_lo, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 128))) return rc;
+  if ((rc = tc::make_tmap(&t[2], params + L.d0_w, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)P, 32))) return rc;
+  if ((rc = tc::make_tmap(&t[3], w.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 32))) return rc;
   tc::GemmShape gs = {};
-  gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = 1; gs.k_blocks = FLAT_CNN / tc::TC_BK; gs.split3 = 1;
-  gs.a_lo_inline = 1;
+  gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = 1; gs.k_blocks = FLAT_CNN / tc::TC_BK; gs.split3 = 2;
   tc::EpiParams ep = {};
   ep.params = params; ep.P = P; ep.off_b = L.d0_b; ep.off_scale = L.ln1_scale; ep.off_bias = L.ln1_bias;
   ep.off_hw = L.head_w; ep.off_hb = L.head_b; ep.A = A; ep.rows = rows;
@@ -3069,14 +2810,13 @@ static int tc_wgrad(float* grads, int64_t P, const pqn_net_layout_t& L, const Wo
                     cudaStream_t st) {
   CUtensorMap t[4];
   int rc;
-  if ((rc = tc::make_tmap(&t[0], w.h1, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 32, 1))) return rc;
-  if ((rc = tc::make_tmap(&t[1], w.h1_lo, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 32, 1))) return rc;
-  if ((rc = tc::make_tmap(&t[2], w.dz2, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 32, 1))) return rc;
-  if ((rc = tc::make_tmap(&t[3], w.dz2_lo, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 32, 1))) return rc;
+  if ((rc = tc::make_tmap(&t[0], w.h1, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 32))) return rc;
+  if ((rc = tc::make_tmap(&t[1], w.h1_lo, FLAT_CNN, rows, S, FLAT_CNN, (uint64_t)rows * FLAT_CNN, 32))) return rc;
+  if ((rc = tc::make_tmap(&t[2], w.dz2, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 32))) return rc;
+  if ((rc = tc::make_tmap(&t[3], w.dz2_lo, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 32))) return rc;
   tc::GemmShape gs = {};
   gs.S = S; gs.M = FLAT_CNN; gs.m_tiles = FLAT_CNN / 128; gs.n_tiles = 1; gs.k_blocks = (rows + tc::TC_BK - 1) / tc::TC_BK;
-  gs.split3 = 1;
-  gs.a_lo_inline = 1;
+  gs.split3 = 2;
   tc::EpiParams ep = {};
   ep.out = grads + L.d0_w; ep.ld_out = HID_CNN; ep.out_seed_stride = P;
   return tc::launch_gemm(1, 1, tc::EPI_STORE, t, gs, ep, st, K_TC_WGRAD);
@@ -3087,13 +2827,13 @@ static int tc_dgrad(const float* params, int64_t P, const pqn_net_layout_t& L, c
                     bool have_bits, cudaStream_t st) {
   CUtensorMap t[4];
   int rc;
-  if ((rc = tc::make_tmap(&t[0], w.dz2, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 128, 0))) return rc;
-  if ((rc = tc::make_tmap(&t[1], w.dz2_lo, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 128, 0))) return rc;
-  if ((rc = tc::make_tmap(&t[2], params + L.d0_w, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)P, 128, 0))) return rc;
-  if ((rc = tc::make_tmap(&t[3], w.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 128, 0))) return rc;
+  if ((rc = tc::make_tmap(&t[0], w.dz2, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 128))) return rc;
+  if ((rc = tc::make_tmap(&t[1], w.dz2_lo, HID_CNN, rows, S, HID_CNN, (uint64_t)rows * HID_CNN, 128))) return rc;
+  if ((rc = tc::make_tmap(&t[2], params + L.d0_w, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)P, 128))) return rc;
+  if ((rc = tc::make_tmap(&t[3], w.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 128))) return rc;
   tc::GemmShape gs = {};
   gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = FLAT_CNN / 128; gs.k_blocks = HID_CNN / tc::TC_BK;
-  gs.split3 = 1;
+  gs.split3 = 1;   // A_lo = dz2_lo, written by row_bwd
   tc::EpiParams ep = {};
   ep.out = w.h1; ep.mask = w.h1; ep.ld_out = FLAT_CNN; ep.out_seed_stride = (int64_t)rows * FLAT_CNN;
   ep.relu_bits = w.relu_bits; ep.rows = rows;
@@ -3226,12 +2966,14 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
 }
 
 int pqn_set_conv_mma_path(int on) {
-  g_conv_mma = on < 0 ? 0 : (on > 3 ? 3 : on);
+  if (on != 0 && on != 1 && on != 3) return set_error(PQN_E_UNSUPPORTED, "pqn_set_conv_mma_path: no conv path %d", on);
+  g_conv_mma = on;
   return PQN_OK;
 }
 
 int pqn_set_tensor_core_path(int on) {
-  g_use_tc = on < 0 ? 0 : (on > 2 ? 2 : on);
+  if (on < 0 || on > 2) return set_error(PQN_E_UNSUPPORTED, "pqn_set_tensor_core_path: no tensor-core path %d", on);
+  g_use_tc = on;
   return PQN_OK;
 }
 
@@ -3307,7 +3049,7 @@ int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* 
       launch_dense<0>(H, dim3(cdiv(rows, BM), S), st, x, xss, D, params, L.total, L.d0_w, L.d0_b, L.ln0_scale,
                       L.ln0_bias, 0, 0, A, w.h0, nullptr, nullptr, nullptr, (int)rows, D);
       if (g_use_tc == 2) {
-        // hidden layer (K = N = H) on tcgen05: fp16-split planes of h0 and of the Dense_1 kernel, raw product, then
+        // hidden layer (K = N = H) on wgmma: fp16-split planes of h0 and of the Dense_1 kernel, raw product, then
         // bias + LayerNorm + ReLU and the Q head in row kernels
         const int64_t R = (int64_t)S * rows;
         __half* hp = reinterpret_cast<__half*>(w.m16_h0);
@@ -3438,7 +3180,7 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
                     L.ln0_bias, 0, 0, A, w.h0, w.xhat0, w.rstd0, nullptr, R, D);
     const dim3 rbg(conv_mma_ctas(S, R, 4), S);
     if (d->layers == 2 && g_use_tc == 2) {
-      // hidden layer on tcgen05 (fp16-split planes): forward product, weight gradient and input gradient
+      // hidden layer on wgmma (fp16-split planes): forward product, weight gradient and input gradient
       const int64_t RR = (int64_t)S * rows;
       __half* hp = reinterpret_cast<__half*>(w.m16_h0);
       __half* wp = reinterpret_cast<__half*>(w.m16_w);

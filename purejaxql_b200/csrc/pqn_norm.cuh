@@ -687,7 +687,7 @@ static int64_t carve_norm(const pqn_net_desc_t* d, int32_t S, int64_t rows, char
   const int64_t R = (int64_t)S * rows;
   const int A = d->num_actions;
   ww->part = take((int64_t)S * part_floats(d));
-  ww->wgp = take(WGRAD_SPLIT_TILES * 128 * 128);
+  ww->wgp = take(wgrad_split_tiles() * 128 * 128);
   ww->sums = take((int64_t)S * 2 * 256);
   ww->dg = take((int64_t)S * 2 * 256);
   for (int i = 0; i < 3; ++i) ww->mr[i] = take((int64_t)S * 2 * 256);

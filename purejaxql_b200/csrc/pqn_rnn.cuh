@@ -321,7 +321,7 @@ static int64_t carve_rnn(const pqn_net_desc_t* d, int32_t S, int64_t rows, char*
   ww->wt = take(3 * (int64_t)S * H * H);
   ww->part = take((int64_t)S * nrm::RED_BLOCKS * (2 * 256 > A + H * A ? 2 * 256 : A + H * A));
   ww->sums = take((int64_t)S * 2 * 256);
-  ww->wgp = take(WGRAD_SPLIT_TILES * 128 * 128);   // per-split partials of the FFMA weight gradient
+  ww->wgp = take(wgrad_split_tiles() * 128 * 128);   // per-split partials of the FFMA weight gradient
   ww->rbp = take(part_ctas(S) * row_bwd_part_floats(H, A));
   return off;
 }

@@ -1,23 +1,20 @@
-// tcgen05 / TMEM / TMA path for the dense contractions of the Q-network
-// (sm_100a only): one warp-specialised, persistent GEMM kernel used for
+// wgmma / TMA path for the dense contractions of the Q-network (sm_90a): one
+// warp-specialised, persistent GEMM kernel used for
 //   forward   Z  = H1 [rows,1024] . W1 [1024,128]        (A K-major,  B MN-major)
 //   wgrad     dW = H1^T [1024,rows] . dZ [rows,128]      (A MN-major, B MN-major)
 //   dgrad     dX = dZ [rows,128] . W1^T [128,1024]       (A K-major,  B K-major)
-// with fp32 accuracy from 3xTF32 error compensation: every operand x is fed as
-// hi = x (the tensor core reads the top 19 bits) and lo = x - trunc_tf32(x),
-// and D += A_lo.B_hi + A_hi.B_lo + A_hi.B_hi accumulates in fp32 in TMEM.
+// with fp32 accuracy from fp16-split operands: every operand x is fed as the
+// planes hi = fp16(x), lo' = fp16((x - hi) * 2^11) (pqn_tc_split16), and
+// D = A_hi.B_hi + (A_lo'.B_hi + A_hi.B_lo') * 2^-11 accumulates in fp32.
 //
 // Reference arithmetic: nn.Dense(128) of CNN (purejaxql/pqn_minatar.py:48) and
 // its autodiff; XLA itself runs these as TF32 tensor-core GEMMs on GPU.
 //
-// Pipeline (per CTA, 192 threads):
-//   warp 0   TMA producer   cp.async.bulk.tensor (SWIZZLE_128B boxes) -> smem ring
-//   warp 1   MMA issuer     tcgen05.mma.cta_group::1.kind::tf32 (one thread), TMEM accumulators
-//   warps 2-5 epilogue      tcgen05.ld 32x32b -> registers -> fused epilogue -> global
-//   warps 6-7 converters    (a_lo_inline) A_lo tile = A tile - trunc_tf32(A tile), smem -> smem, so that the
-//                           big activation operand is read from HBM once instead of as a (hi, lo) pair
-// Barriers: full[stage]/empty[stage] (TMA <-> MMA), lo_full[stage] (converters -> MMA),
-//           main_full/main_empty[2], corr_full/corr_empty[2] (MMA <-> epilogue).
+// Pipeline (per CTA, 288 threads, one CTA per SM, 128 x 128 output tiles):
+//   warp 8      TMA producer   cp.async.bulk.tensor (SWIZZLE_128B boxes) -> 2-stage smem ring
+//   warps 0-7   consumers      two warpgroups, rows 0-63 / 64-127 of the tile: wgmma m64n128k16 into register
+//                              accumulators, promotion into an fp32 tile in shared memory, then the epilogue
+// Barriers: full[stage] (TMA -> consumers, tx bytes), empty[stage] (8 consumer warps -> TMA).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,18 +27,16 @@ namespace pqn {
 namespace tc {
 
 // ---------------------------------------------------------------------------
-// epilogues: each epilogue thread owns one row of the 128x128 tile, already
-// promoted to fp32 registers (acc[128], fully unrolled static indexing)
+// LayerNorm epilogues: each of the 128 threads of warps 0-3 owns one row of the 128x128 tile, read from the fp32
+// tile into registers (acc[128], fully unrolled static indexing)
 // ---------------------------------------------------------------------------
 // Coalesced tile-row-block store: the warp's 32 rows x 32 columns chunk goes through a padded shared-memory
 // stage so that 8 lanes write one 128-byte row segment (4 rows per store instruction) instead of 32 lanes
-// writing 32 different rows.  `vals` = this lane's row, columns [0,32) of the chunk.  MASKED: multiply by
-// (mask > 0) read with the same coalesced addressing (dgrad's fused ReLU mask; may alias dst).
+// writing 32 different rows.  `vals` = this lane's row, columns [0,32) of the chunk.
 constexpr int STG_LD = 36;  // floats per staged row (16-byte aligned, conflict-free for 128-bit accesses)
 
-template <bool MASKED>
 __device__ __forceinline__ void store_chunk_coalesced(float* stage, const float (&vals)[32], int lane, float* dst,
-                                                      uint32_t mask_bits, int64_t ld, int m_base, int M) {
+                                                      int64_t ld, int m_base, int M) {
 #pragma unroll
   for (int j = 0; j < 8; ++j)
     *reinterpret_cast<float4*>(stage + lane * STG_LD + 4 * j) =
@@ -51,291 +46,257 @@ __device__ __forceinline__ void store_chunk_coalesced(float* stage, const float 
 #pragma unroll
   for (int it = 0; it < 8; ++it) {
     const int r = it * 4 + r_in;
-    if (m_base + r < M) {
-      float4 o = *reinterpret_cast<const float4*>(stage + r * STG_LD + 4 * c4);
-      const int64_t off = (int64_t)r * ld + 4 * c4;
-      if (MASKED) {
-        const uint32_t b = mask_bits >> (it * 4);
-        o.x = (b & 1u) ? o.x : 0.f; o.y = (b & 2u) ? o.y : 0.f;
-        o.z = (b & 4u) ? o.z : 0.f; o.w = (b & 8u) ? o.w : 0.f;
-      }
-      *reinterpret_cast<float4*>(dst + off) = o;
-    }
+    if (m_base + r < M)
+      *reinterpret_cast<float4*>(dst + (int64_t)r * ld + 4 * c4) = *reinterpret_cast<const float4*>(stage + r * STG_LD + 4 * c4);
   }
   __syncwarp();
 }
 
-// ReLU mask of dgrad, fetched BEFORE the tile's MMAs are awaited (it does not depend on them) so the HBM latency
-// overlaps the tensor-core work: bit (it*4 + j) of bits[c] = (mask[row it*4 + lane/8][c*32 + 4*(lane%8) + j] > 0),
-// i.e. exactly the elements this lane stores in store_chunk_coalesced.
-__device__ __forceinline__ void prefetch_mask_bits(const EpiParams& ep, int seed, int m_base, int n0, int lane, int M,
-                                                   uint32_t (&bits)[4]) {
-  const float* msk = ep.mask + (int64_t)seed * ep.out_seed_stride + (int64_t)m_base * ep.ld_out + n0;
-  const int r_in = lane >> 3, c4 = lane & 7;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    float4 h[8];
-#pragma unroll
-    for (int it = 0; it < 8; ++it) {
-      const int r = it * 4 + r_in;
-      h[it] = (m_base + r < M) ? *reinterpret_cast<const float4*>(msk + (int64_t)r * ep.ld_out + c * 32 + 4 * c4)
-                               : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    uint32_t b = 0u;
-#pragma unroll
-    for (int it = 0; it < 8; ++it)
-      b |= ((h[it].x > 0.f ? 1u : 0u) | (h[it].y > 0.f ? 2u : 0u) | (h[it].z > 0.f ? 4u : 0u) | (h[it].w > 0.f ? 8u : 0u))
-           << (it * 4);
-    bits[c] = b;
-  }
-}
-
-// `m_base` = first row of this warp's 32-row block; the lane's own row is m_base + lane.
 // Shared-memory copy of the per-seed epilogue parameters (LN epilogues), staged once per tile by the 128 epilogue
 // threads: every thread needs all of them, and 128-bit broadcast reads cost a quarter of the per-element loads.
 constexpr int SP_B = 0, SP_SC = 128, SP_BI = 256, SP_HW = 384 /* [PQN_TC_MAX_A][128] */,
               SP_HB = SP_HW + PQN_TC_MAX_A * 128, SP_FLOATS = SP_HB + PQN_TC_MAX_A;
-static_assert(SP_FLOATS == 384 + 8 * 128 + 8, "matches the TC_SMEM_BYTES budget in tc_common.cuh");
+static_assert(SP_FLOATS == TC_SP_FLOATS, "matches the TC_SMEM_BYTES budget in tc_common.cuh");
 
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
 
 template <int EPI>
 __device__ __forceinline__ void stage_epi_params(const EpiParams& ep, float* sp, int seed, int et /*0..127*/) {
-  if constexpr (EPI == EPI_LN_TRAIN || EPI == EPI_LN_HEAD) {
-    const float* __restrict__ prm = ep.params + (int64_t)seed * ep.P;
-    epi_bar_sync();  // everyone is done with the previous tile's parameters
-    sp[SP_B + et] = __ldg(prm + ep.off_b + et);
-    sp[SP_SC + et] = __ldg(prm + ep.off_scale + et);
-    sp[SP_BI + et] = __ldg(prm + ep.off_bias + et);
-    if constexpr (EPI == EPI_LN_HEAD) {
-      for (int a = 0; a < ep.A; ++a) sp[SP_HW + a * 128 + et] = __ldg(prm + ep.off_hw + (int64_t)et * ep.A + a);
-      if (et < ep.A) sp[SP_HB + et] = __ldg(prm + ep.off_hb + et);
-    }
-    epi_bar_sync();
+  const float* __restrict__ prm = ep.params + (int64_t)seed * ep.P;
+  epi_bar_sync();  // everyone is done with the previous tile's parameters
+  sp[SP_B + et] = __ldg(prm + ep.off_b + et);
+  sp[SP_SC + et] = __ldg(prm + ep.off_scale + et);
+  sp[SP_BI + et] = __ldg(prm + ep.off_bias + et);
+  if constexpr (EPI == EPI_LN_HEAD) {
+    for (int a = 0; a < ep.A; ++a) sp[SP_HW + a * 128 + et] = __ldg(prm + ep.off_hw + (int64_t)et * ep.A + a);
+    if (et < ep.A) sp[SP_HB + et] = __ldg(prm + ep.off_hb + et);
   }
+  epi_bar_sync();
 }
 
+// bias + LayerNorm(128) + ReLU, then either (h, xhat, rstd) or the fused Q-head.  `m_base` = first row of this warp's
+// 32-row block; the lane's own row is m_base + lane.
 template <int EPI>
-__device__ __forceinline__ void epilogue_row(const EpiParams& ep, float (&acc)[128], float* stage, const float* sp,
-                                             int lane, int seed, int m_base, int n0, int M,
-                                             const uint32_t (&mask_bits)[4]) {
+__device__ __forceinline__ void epilogue_ln_row(const EpiParams& ep, float (&acc)[128], float* stage, const float* sp,
+                                                int lane, int seed, int m_base, int M) {
   const int m = m_base + lane;
   const bool row_ok = m < M;
-  if constexpr (EPI == EPI_STORE || EPI == EPI_RELU_MASK || EPI == EPI_RELU_BITS) {
-    // no __restrict__: dgrad runs in place (out == mask)
-    float* out = ep.out + (int64_t)seed * ep.out_seed_stride + (int64_t)m_base * ep.ld_out + n0;
+  float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+  for (int j4 = 0; j4 < 32; ++j4) {
+    const float4 b = *reinterpret_cast<const float4*>(sp + SP_B + 4 * j4);
+    const float bb[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = 4 * j4 + e;
+      acc[j] += bb[e];
+      s1 += acc[j];
+      s2 = fmaf(acc[j], acc[j], s2);
+    }
+  }
+  const float mean = s1 * (1.0f / 128.f);
+  const float var = fmaxf(s2 * (1.0f / 128.f) - mean * mean, 0.f);
+  const float rstd = 1.0f / sqrtf(var + 1e-6f);
+  const int64_t grow = (int64_t)seed * ep.rows + m;
+  if constexpr (EPI == EPI_LN_TRAIN) {
+    float* hbase = ep.H + ((int64_t)seed * ep.rows + m_base) * 128;
+    float* xbase = ep.XHAT + ((int64_t)seed * ep.rows + m_base) * 128;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      float v[32];
+      float xh[32], h[32];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        v[j] = acc[c * 32 + j];
-        // EPI_RELU_BITS: mask_bits = this lane's own row, one word per 32-column chunk
-        if (EPI == EPI_RELU_BITS) v[j] = ((mask_bits[c] >> j) & 1u) ? v[j] : 0.f;
+      for (int j4 = 0; j4 < 8; ++j4) {
+        const float4 s4 = *reinterpret_cast<const float4*>(sp + SP_SC + c * 32 + 4 * j4);
+        const float4 b4 = *reinterpret_cast<const float4*>(sp + SP_BI + c * 32 + 4 * j4);
+        const float ss[4] = {s4.x, s4.y, s4.z, s4.w}, bb[4] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int j = 4 * j4 + e;
+          xh[j] = (acc[c * 32 + j] - mean) * rstd;
+          h[j] = fmaxf(xh[j] * ss[e] + bb[e], 0.f);
+        }
       }
-      store_chunk_coalesced<EPI == EPI_RELU_MASK>(stage, v, lane, out + c * 32, mask_bits[c], ep.ld_out, m_base, M);
+      store_chunk_coalesced(stage, h, lane, hbase + c * 32, 128, m_base, M);
+      store_chunk_coalesced(stage, xh, lane, xbase + c * 32, 128, m_base, M);
     }
-  } else {
-    // bias + LayerNorm(128) + ReLU, then either (h, xhat, rstd) or the fused Q-head
-    float s1 = 0.f, s2 = 0.f;
+    if (row_ok) ep.RSTD[grow] = rstd;
+  } else {  // EPI_LN_HEAD
+    float q[PQN_TC_MAX_A];
+#pragma unroll
+    for (int a = 0; a < PQN_TC_MAX_A; ++a) q[a] = 0.f;
 #pragma unroll
     for (int j4 = 0; j4 < 32; ++j4) {
-      const float4 b = *reinterpret_cast<const float4*>(sp + SP_B + 4 * j4);
-      const float bb[4] = {b.x, b.y, b.z, b.w};
+      const float4 s4 = *reinterpret_cast<const float4*>(sp + SP_SC + 4 * j4);
+      const float4 b4 = *reinterpret_cast<const float4*>(sp + SP_BI + 4 * j4);
+      float h[4];
+      h[0] = fmaxf((acc[4 * j4 + 0] - mean) * rstd * s4.x + b4.x, 0.f);
+      h[1] = fmaxf((acc[4 * j4 + 1] - mean) * rstd * s4.y + b4.y, 0.f);
+      h[2] = fmaxf((acc[4 * j4 + 2] - mean) * rstd * s4.z + b4.z, 0.f);
+      h[3] = fmaxf((acc[4 * j4 + 3] - mean) * rstd * s4.w + b4.w, 0.f);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int j = 4 * j4 + e;
-        acc[j] += bb[e];
-        s1 += acc[j];
-        s2 = fmaf(acc[j], acc[j], s2);
-      }
-    }
-    const float mean = s1 * (1.0f / 128.f);
-    const float var = fmaxf(s2 * (1.0f / 128.f) - mean * mean, 0.f);
-    const float rstd = 1.0f / sqrtf(var + 1e-6f);
-    const int64_t grow = (int64_t)seed * ep.rows + m;
-    if constexpr (EPI == EPI_LN_TRAIN) {
-      float* hbase = ep.H + ((int64_t)seed * ep.rows + m_base) * 128;
-      float* xbase = ep.XHAT + ((int64_t)seed * ep.rows + m_base) * 128;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float xh[32], h[32];
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const float4 s4 = *reinterpret_cast<const float4*>(sp + SP_SC + c * 32 + 4 * j4);
-          const float4 b4 = *reinterpret_cast<const float4*>(sp + SP_BI + c * 32 + 4 * j4);
-          const float ss[4] = {s4.x, s4.y, s4.z, s4.w}, bb[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int j = 4 * j4 + e;
-            xh[j] = (acc[c * 32 + j] - mean) * rstd;
-            h[j] = fmaxf(xh[j] * ss[e] + bb[e], 0.f);
-          }
+      for (int a = 0; a < PQN_TC_MAX_A; ++a)
+        if (a < ep.A) {
+          const float4 w4 = *reinterpret_cast<const float4*>(sp + SP_HW + a * 128 + 4 * j4);
+          q[a] = fmaf(h[0], w4.x, q[a]); q[a] = fmaf(h[1], w4.y, q[a]);
+          q[a] = fmaf(h[2], w4.z, q[a]); q[a] = fmaf(h[3], w4.w, q[a]);
         }
-        store_chunk_coalesced<false>(stage, h, lane, hbase + c * 32, 0u, 128, m_base, M);
-        store_chunk_coalesced<false>(stage, xh, lane, xbase + c * 32, 0u, 128, m_base, M);
-      }
-      if (row_ok) ep.RSTD[grow] = rstd;
-    } else {  // EPI_LN_HEAD
-      float q[PQN_TC_MAX_A];
+    }
+    if (row_ok) {
 #pragma unroll
-      for (int a = 0; a < PQN_TC_MAX_A; ++a) q[a] = 0.f;
-#pragma unroll
-      for (int j4 = 0; j4 < 32; ++j4) {
-        const float4 s4 = *reinterpret_cast<const float4*>(sp + SP_SC + 4 * j4);
-        const float4 b4 = *reinterpret_cast<const float4*>(sp + SP_BI + 4 * j4);
-        float h[4];
-        h[0] = fmaxf((acc[4 * j4 + 0] - mean) * rstd * s4.x + b4.x, 0.f);
-        h[1] = fmaxf((acc[4 * j4 + 1] - mean) * rstd * s4.y + b4.y, 0.f);
-        h[2] = fmaxf((acc[4 * j4 + 2] - mean) * rstd * s4.z + b4.z, 0.f);
-        h[3] = fmaxf((acc[4 * j4 + 3] - mean) * rstd * s4.w + b4.w, 0.f);
-#pragma unroll
-        for (int a = 0; a < PQN_TC_MAX_A; ++a)
-          if (a < ep.A) {
-            const float4 w4 = *reinterpret_cast<const float4*>(sp + SP_HW + a * 128 + 4 * j4);
-            q[a] = fmaf(h[0], w4.x, q[a]); q[a] = fmaf(h[1], w4.y, q[a]);
-            q[a] = fmaf(h[2], w4.z, q[a]); q[a] = fmaf(h[3], w4.w, q[a]);
-          }
-      }
-      if (row_ok) {
-#pragma unroll
-        for (int a = 0; a < PQN_TC_MAX_A; ++a)
-          if (a < ep.A) ep.Q[grow * ep.A + a] = q[a] + sp[SP_HB + a];
-      }
+      for (int a = 0; a < PQN_TC_MAX_A; ++a)
+        if (a < ep.A) ep.Q[grow * ep.A + a] = q[a] + sp[SP_HB + a];
     }
   }
 }
 
-// acc[0..128) (+)= the 128 fp32 columns of this thread's TMEM lane at `row_addr`.  The loads are issued back to
-// back and awaited once (FIRST: all four 32-column loads straight into acc; otherwise two at a time, 64 staging
-// registers) -- the per-load round trip to TMEM was the longest part of the epilogue's dependent chain.
-template <bool FIRST, int NC = 128>
-__device__ __forceinline__ void tmem_accumulate_row(uint32_t row_addr, float (&acc)[NC], float scale = 1.0f) {
-  if constexpr (FIRST && NC == 128) {
-    uint32_t v0[32], v1[32], v2[32], v3[32];
-    tmem_ld_32x32b_x32(row_addr, v0);
-    tmem_ld_32x32b_x32(row_addr + 32, v1);
-    tmem_ld_32x32b_x32(row_addr + 64, v2);
-    tmem_ld_32x32b_x32(row_addr + 96, v3);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      acc[j] = __uint_as_float(v0[j]); acc[32 + j] = __uint_as_float(v1[j]);
-      acc[64 + j] = __uint_as_float(v2[j]); acc[96 + j] = __uint_as_float(v3[j]);
-    }
-  } else {
-#pragma unroll
-    for (int c = 0; c < NC / 64; ++c) {
-      uint32_t v0[32], v1[32];
-      tmem_ld_32x32b_x32(row_addr + c * 64, v0);
-      tmem_ld_32x32b_x32(row_addr + c * 64 + 32, v1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        if (FIRST) {
-          acc[c * 64 + j] = __uint_as_float(v0[j]);
-          acc[c * 64 + 32 + j] = __uint_as_float(v1[j]);
-        } else {
-          acc[c * 64 + j] = fmaf(__uint_as_float(v0[j]), scale, acc[c * 64 + j]);   // scale == 1: exact add
-          acc[c * 64 + 32 + j] = fmaf(__uint_as_float(v1[j]), scale, acc[c * 64 + 32 + j]);
-        }
-      }
-    }
-  }
+// ---------------------------------------------------------------------------
+// TF32 consumers (3xTF32 / single-pass).  Hopper's wgmma reads 32-bit operands only K-major, and the forward and
+// weight-gradient products have MN-major operands, so this variant runs warp-level mma.sync.m16n8k8.tf32 on fragments
+// read from the same TMA ring (SWIZZLE_128B tiles of 128 rows x 32 fp32).  Warp w owns tile rows 32 (w % 4) .. +31 and
+// columns 64 (w / 4) .. +63: 2 x 8 MMAs per k-step and product.
+// ---------------------------------------------------------------------------
+// fp32 element (r = M or N index, k) of a 128 x 32 operand tile as TMA writes it with SWIZZLE_128B:
+//   K-major : 128-byte rows r, 16-byte chunk (k / 4) ^ (r % 8)
+//   MN-major: 4 boxes of [32 k rows][32 mn] at 4096 B, 128-byte rows k, chunk ((r % 32) / 4) ^ (k % 8)
+template <int MN>
+__device__ __forceinline__ float lds_tf32(const uint8_t* tile, int r, int k) {
+  const int off = MN ? ((r >> 5) * 4096 + k * 128 + ((((r & 31) >> 2) ^ (k & 7)) << 4) + ((r & 3) << 2))
+                     : (r * 128 + (((k >> 2) ^ (r & 7)) << 4) + ((k & 3) << 2));
+  return *reinterpret_cast<const float*>(tile + off);
+}
+__device__ __forceinline__ uint32_t tf32_trunc_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
+__device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// SPLIT epilogue (fp16 kernels with a store epilogue: wgrad, dgrad): EIGHT epilogue warps instead of four -- warps 2-5
-// take columns 0..63 of the tile, warps 6-9 columns 64..127 (a warp may only touch the TMEM lane quadrant warp % 4, and
-// both sets cover the four quadrants).  Half the registers per thread and twice the warps in flight: the dgrad
-// epilogue (K = 128, one tile every ~2500 MMA clocks) was latency-bound with one warp per scheduler (ncu r2c: issue
-// active 20 %, 4468 warp-instructions per tile).  The 32 x 32 staging tile of a warp is XOR-swizzled instead of padded
-// (8 x 4 KB fit next to the three operand stages).
-__device__ __forceinline__ void store_chunk_swz(float* stage, const float (&vals)[32], int lane, float* dst, int64_t ld,
-                                                int m_base, int M) {
+// One output tile into tile_s (promotion as in the fp16 path; the cross products are in the units of the result).
+// split3: 0 single TF32 pass; 1 3xTF32 with A_lo from memory; 2 3xTF32 with A_lo = A - trunc_tf32(A) in registers.
+template <int A_MN, int B_MN>
+__device__ __forceinline__ void tf32_tile(const uint8_t* smem_al, float* tile_s, uint64_t* full, uint64_t* empty,
+                                          int& stage, uint32_t& phase, int kbn, int split3, float osc, int warp,
+                                          int lane) {
+  const int g = lane >> 2, tq = lane & 3;
+  const int wr = (warp & 3) * 32, wc = (warp >> 2) * 64;
+  float mainacc[2][8][4], corr[2][8][4];
 #pragma unroll
-  for (int j = 0; j < 8; ++j)   // row = lane, 16-byte chunk j -> physical chunk j ^ (lane & 7)
-    *reinterpret_cast<float4*>(stage + lane * 32 + 4 * (j ^ (lane & 7))) =
-        make_float4(vals[4 * j], vals[4 * j + 1], vals[4 * j + 2], vals[4 * j + 3]);
-  __syncwarp();
-  const int r_in = lane >> 3, c4 = lane & 7;
+  for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const int r = it * 4 + r_in;
-    if (m_base + r < M) {
-      const float4 o = *reinterpret_cast<const float4*>(stage + r * 32 + 4 * (c4 ^ (r & 7)));
-      *reinterpret_cast<float4*>(dst + (int64_t)r * ld + 4 * c4) = o;
+    for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) { mainacc[mi][ni][e] = 0.f; corr[mi][ni][e] = 0.f; }
+  for (int kb = 0; kb < kbn; ++kb) {
+    mbar_wait(&full[stage], phase);
+    const uint8_t* sb = smem_al + stage * TC_STAGE_BYTES;
+    if (kb % TC_PROMOTE == 0) {
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) mainacc[mi][ni][e] = 0.f;
+    }
+#pragma unroll
+    for (int ks = 0; ks < TC_BK / 8; ++ks) {
+      const int k = ks * 8 + tq;
+      uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi) {
+        const int r0 = wr + mi * 16 + g;
+        const int rr[4] = {r0, r0 + 8, r0, r0 + 8}, kk[4] = {k, k, k + 4, k + 4};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float x = lds_tf32<A_MN>(sb + TC_A_HI, rr[e], kk[e]);
+          ahi[mi][e] = tf32_trunc_bits(x);
+          const float lo = split3 == 1 ? lds_tf32<A_MN>(sb + TC_A_LO, rr[e], kk[e]) : x - __uint_as_float(ahi[mi][e]);
+          alo[mi][e] = tf32_trunc_bits(lo);
+        }
+      }
+#pragma unroll
+      for (int ni = 0; ni < 8; ++ni) {
+        const int n = wc + ni * 8 + g;
+        const uint32_t bh0 = tf32_trunc_bits(lds_tf32<B_MN>(sb + TC_B_HI, n, k));
+        const uint32_t bh1 = tf32_trunc_bits(lds_tf32<B_MN>(sb + TC_B_HI, n, k + 4));
+        if (split3) {
+          const uint32_t bl0 = tf32_trunc_bits(lds_tf32<B_MN>(sb + TC_B_LO, n, k));
+          const uint32_t bl1 = tf32_trunc_bits(lds_tf32<B_MN>(sb + TC_B_LO, n, k + 4));
+#pragma unroll
+          for (int mi = 0; mi < 2; ++mi) {
+            mma_tf32_16x8x8(corr[mi][ni], alo[mi], bh0, bh1);
+            mma_tf32_16x8x8(corr[mi][ni], ahi[mi], bl0, bl1);
+          }
+        }
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi) mma_tf32_16x8x8(mainacc[mi][ni], ahi[mi], bh0, bh1);
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);   // this warp's fragment reads of the slot are done
+    if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
+    if ((kb + 1) % TC_PROMOTE == 0 || kb == kbn - 1) {
+      const bool first = kb < TC_PROMOTE;
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float2* p = reinterpret_cast<float2*>(tile_s + (wr + mi * 16 + g + 8 * h) * TC_ACC_LD + wc + ni * 8 + 2 * tq);
+            const float2 v = make_float2(mainacc[mi][ni][2 * h], mainacc[mi][ni][2 * h + 1]);
+            if (first) *p = v;
+            else { const float2 o = *p; *p = make_float2(o.x + v.x, o.y + v.y); }
+          }
     }
   }
-  __syncwarp();
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2* p = reinterpret_cast<float2*>(tile_s + (wr + mi * 16 + g + 8 * h) * TC_ACC_LD + wc + ni * 8 + 2 * tq);
+        float2 o = kbn > 0 ? *p : make_float2(0.f, 0.f);
+        o.x += corr[mi][ni][2 * h];
+        o.y += corr[mi][ni][2 * h + 1];
+        *p = make_float2(o.x * osc, o.y * osc);
+      }
 }
 
 // ---------------------------------------------------------------------------
 // the kernel
 //
-// Accuracy: the tensor core truncates (round-toward-zero) when it accumulates into TMEM, so a long in-TMEM
-// chain drifts (measured: 3e-5 relative at K=1024).  Two-level accumulation fixes it:
-//   * the correction terms A_lo.B_hi + A_hi.B_lo (2^-11 of the result) get their own TMEM accumulator for the
-//     whole K — their truncation error is negligible at that magnitude;
-//   * the main A_hi.B_hi chain is cut every TC_PROMOTE k-blocks (16 MMAs): the partial is added to fp32
-//     registers by the epilogue warps (round-to-nearest FADD) and the MMA warp continues into the other TMEM
-//     buffer with accumulate=0.
-// TMEM columns: main[2] at 0/128, corr[2] at 256/384.
+// Accuracy: the tensor core's fp32 accumulation is not round-to-nearest, so a long chain of MMAs into one
+// accumulator drifts.  Two-level accumulation keeps fp32 accuracy:
+//   * the correction terms A_lo'.B_hi + A_hi.B_lo' (2^-11 of the result) get their own register accumulator for the
+//     whole K -- their accumulation error is negligible at that magnitude;
+//   * the main A_hi.B_hi chain is cut every TC_PROMOTE k-blocks (16 k-steps): the partial is added to the fp32 tile in
+//     shared memory (round-to-nearest FADD) and the chain restarts with scale-d = 0.
 // ---------------------------------------------------------------------------
-template <int EPI, bool F16>
-struct TcSplit {
-  static constexpr bool value = F16 && (EPI == EPI_STORE || EPI == EPI_RELU_BITS);
-  static constexpr int threads = value ? TC_THREADS + 64 : TC_THREADS;
-  // operand ring + align slack + barriers + staging (split: 8 x [32][32]; else 4 x [32][36] + epilogue parameters)
-  static constexpr int smem = TC_STAGES * TC_STAGE_BYTES + 1024 + 256 +
-                              (value ? 8 * 32 * 32 * 4 : 4 * 32 * 36 * 4 + (384 + 8 * 128 + 8) * 4);
-};
-
-template <int A_MN, int B_MN, int EPI, bool F16 = false>
-__global__ void __launch_bounds__((TcSplit<EPI, F16>::threads), 1)
+template <int A_MN, int B_MN, int EPI, bool F16 = true>
+__global__ void __launch_bounds__(TC_THREADS, 1)
     tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                    const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
                    const GemmShape gs, const EpiParams ep) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte aligned operand ring (swizzle atoms), then barriers
+  // 1024-byte aligned operand ring (swizzle atoms), then the fp32 tile, the epilogue parameters and the barriers
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_al + TC_STAGES * TC_STAGE_BYTES);
-  uint64_t* full = bars;                        // [TC_STAGES]   TMA -> MMA
-  uint64_t* empty = bars + TC_STAGES;           // [TC_STAGES]   MMA -> TMA
-  uint64_t* main_full = bars + 2 * TC_STAGES;   // [2]           MMA -> epilogue (main partial ready)
-  uint64_t* main_empty = main_full + 2;         // [2]           epilogue -> MMA
-  uint64_t* corr_full = main_empty + 2;         // [2]
-  uint64_t* corr_empty = corr_full + 2;         // [2]
-  uint64_t* lo_full = corr_empty + 2;           // [TC_STAGES]   converters -> MMA (A_lo tile written)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(lo_full + TC_STAGES);
-  float* stage_all = reinterpret_cast<float*>(smem_al + TC_STAGES * TC_STAGE_BYTES + 256);  // 4 x [32][STG_LD]
-  float* sp_all = stage_all + 4 * 32 * STG_LD;                                              // [SP_FLOATS]
+  float* tile_s = reinterpret_cast<float*>(smem_al + TC_STAGES * TC_STAGE_BYTES);   // [128][TC_ACC_LD]
+  float* sp_all = tile_s + 128 * TC_ACC_LD;                                            // [SP_FLOATS]
+  uint64_t* full = reinterpret_cast<uint64_t*>(sp_all + TC_SP_FLOATS);                // [TC_STAGES]  TMA -> MMA
+  uint64_t* empty = full + TC_STAGES;                                                 // [TC_STAGES]  MMA -> TMA
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_b_hi);
-    if (gs.split3) { if (!gs.a_lo_inline) prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_lo); }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < TC_STAGES; ++i) {
-      mbar_init(&full[i], 1); mbar_init(&empty[i], 1); mbar_init(&lo_full[i], TC_CONV_THREADS);
-    }
-    constexpr int EPI_WARPS = TcSplit<EPI, F16>::value ? 8 : 4;
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&main_full[i], 1); mbar_init(&main_empty[i], EPI_WARPS);
-      mbar_init(&corr_full[i], 1); mbar_init(&corr_empty[i], EPI_WARPS);
-    }
+  if (warp == 8 && lane == 0) {
+    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
+    for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TC_CONSUMERS / 32); }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // split-K: tile index -> (seed, m/n tile, k range).  k_split == 1 is the plain case.
   const int ksplit = gs.k_split > 1 ? gs.k_split : 1;
@@ -353,13 +314,12 @@ __global__ void __launch_bounds__((TcSplit<EPI, F16>::threads), 1)
     return ks;
   };
 
-  // F16: fp16 operand planes (hi, lo'), 64-element k-blocks, A_lo' always comes from memory (no converter warps)
-  const bool a_lo_tma = gs.split3 && (F16 || !gs.a_lo_inline);
-  const bool a_lo_conv = !F16 && gs.split3 && gs.a_lo_inline;
-  constexpr int BKE = F16 ? TC_BK16 : TC_BK;              // elements per k-block
+  // F16: 64-element k-blocks, 2 MN-major boxes of 64; TF32: 32-element k-blocks, 4 MN-major boxes of 32
+  constexpr int BKE = F16 ? TC_BK16 : TC_BK;
   constexpr int MNB = F16 ? 2 : 4;                        // MN-major TMA boxes per 128-wide tile
   constexpr int MNB_ELEMS = F16 ? 64 : 32, MNB_BYTES = F16 ? 8192 : 4096;
-  if (warp == 0) {
+  const bool a_lo_tma = F16 || gs.split3 == 1, b_lo_tma = F16 || gs.split3 != 0;
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
@@ -370,7 +330,7 @@ __global__ void __launch_bounds__((TcSplit<EPI, F16>::threads), 1)
         for (int kb = kb0; kb < kb0 + kbn; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1u);
           const uint32_t sb = smem_base + stage * TC_STAGE_BYTES;
-          mbar_expect_tx(&full[stage], gs.split3 ? (a_lo_tma ? TC_STAGE_BYTES : 3 * TC_TILE_BYTES) : TC_STAGE_BYTES / 2);
+          mbar_expect_tx(&full[stage], (2 + (a_lo_tma ? 1 : 0) + (b_lo_tma ? 1 : 0)) * TC_TILE_BYTES);
           const int k0 = kb * BKE;
           if (A_MN) {
 #pragma unroll
@@ -386,239 +346,127 @@ __global__ void __launch_bounds__((TcSplit<EPI, F16>::threads), 1)
 #pragma unroll
             for (int j = 0; j < MNB; ++j) {
               tma_load_3d(sb + TC_B_HI + j * MNB_BYTES, &tm_b_hi, &full[stage], n0 + MNB_ELEMS * j, k0, seed);
-              if (gs.split3) tma_load_3d(sb + TC_B_LO + j * MNB_BYTES, &tm_b_lo, &full[stage], n0 + MNB_ELEMS * j, k0, seed);
+              if (b_lo_tma) tma_load_3d(sb + TC_B_LO + j * MNB_BYTES, &tm_b_lo, &full[stage], n0 + MNB_ELEMS * j, k0, seed);
             }
           } else {
             tma_load_3d(sb + TC_B_HI, &tm_b_hi, &full[stage], k0, n0, seed);
-            if (gs.split3) tma_load_3d(sb + TC_B_LO, &tm_b_lo, &full[stage], k0, n0, seed);
+            if (b_lo_tma) tma_load_3d(sb + TC_B_LO, &tm_b_lo, &full[stage], k0, n0, seed);
           }
           if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = F16 ? make_idesc_f16(128, 128, A_MN, B_MN) : make_idesc_tf32(128, 128, A_MN, B_MN);
-      auto sdesc_a = [](uint32_t tile, int ks) { return F16 ? make_sdesc16<A_MN>(tile, ks) : make_sdesc<A_MN>(tile, ks); };
-      auto sdesc_b = [](uint32_t tile, int ks) { return F16 ? make_sdesc16<B_MN>(tile, ks) : make_sdesc<B_MN>(tile, ks); };
-      auto umma = [](uint32_t d, uint64_t da, uint64_t db, uint32_t id, uint32_t acc) {
-        if (F16) umma_f16(d, da, db, id, acc); else umma_tf32(d, da, db, id, acc);
-      };
-      int stage = 0;
-      uint32_t phase = 0;
-      int mb = 0, cb = 0;
-      uint32_t mb_phase = 0, cb_phase = 0;
-      // Short-K mode (k_blocks <= TC_PROMOTE, e.g. dgrad with K = 128): the whole tile is one promotion chunk, so the
-      // correction terms share the main accumulator (a chain of <= 48 MMAs keeps the truncation drift ~1e-6) and the
-      // four 128-column TMEM regions form one ring of accumulators: the epilogue reads each tile once.
-      // (tf32 only: the f16 path keeps the cross products in units of 2^-11, so they need their own accumulator)
-      const bool single_acc = !F16 && gs.split3 && gs.k_blocks <= TC_PROMOTE;
-      if (single_acc) {
-        int ab = 0;
-        uint32_t ab_phase = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          uint64_t* e_bar = ab < 2 ? &main_empty[ab] : &corr_empty[ab - 2];
-          uint64_t* f_bar = ab < 2 ? &main_full[ab] : &corr_full[ab - 2];
-          mbar_wait(e_bar, ab_phase ^ 1u);
-          tcgen05_fence_after();
-          const uint32_t d_acc = tmem_base + ab * 128;
-          bool first = true;
-          int seed_, m0_, n0_, kb0_, kbn_;
-          decode(tile, seed_, m0_, n0_, kb0_, kbn_);
-          for (int kb = 0; kb < kbn_; ++kb) {
-            mbar_wait(&full[stage], phase);
-            if (a_lo_conv) mbar_wait(&lo_full[stage], phase);
-            tcgen05_fence_after();
-            const uint32_t sb = smem_base + stage * TC_STAGE_BYTES;
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint64_t a_hi = sdesc_a(sb + TC_A_HI, ks), a_lo = sdesc_a(sb + TC_A_LO, ks);
-              const uint64_t b_hi = sdesc_b(sb + TC_B_HI, ks), b_lo = sdesc_b(sb + TC_B_LO, ks);
-              umma(d_acc, a_lo, b_hi, idesc, first ? 0u : 1u);
-              umma(d_acc, a_hi, b_lo, idesc, 1u);
-              umma(d_acc, a_hi, b_hi, idesc, 1u);
-              first = false;
-            }
-            umma_commit(&empty[stage]);
-            if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
-          }
-          umma_commit(f_bar);
-          if (++ab == 4) { ab = 0; ab_phase ^= 1u; }
-        }
-      } else
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const uint32_t d_corr = tmem_base + 256 + cb * 128;
-        if (gs.split3) {
-          mbar_wait(&corr_empty[cb], cb_phase ^ 1u);
-          tcgen05_fence_after();
-        }
-        bool first_corr = true, first_main = true;
-        int seed_, m0_, n0_, kb0_, kbn_;
-        decode(tile, seed_, m0_, n0_, kb0_, kbn_);
-        for (int kb = 0; kb < kbn_; ++kb) {
-          if (kb % TC_PROMOTE == 0) {
-            mbar_wait(&main_empty[mb], mb_phase ^ 1u);
-            tcgen05_fence_after();
-            first_main = true;
-          }
-          const uint32_t d_main = tmem_base + mb * 128;
-          mbar_wait(&full[stage], phase);
-          if (a_lo_conv) mbar_wait(&lo_full[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t sb = smem_base + stage * TC_STAGE_BYTES;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t a_hi = sdesc_a(sb + TC_A_HI, ks);
-            const uint64_t b_hi = sdesc_b(sb + TC_B_HI, ks);
-            if (gs.split3) {
-              const uint64_t a_lo = sdesc_a(sb + TC_A_LO, ks);
-              const uint64_t b_lo = sdesc_b(sb + TC_B_LO, ks);
-              umma(d_corr, a_lo, b_hi, idesc, first_corr ? 0u : 1u);
-              umma(d_corr, a_hi, b_lo, idesc, 1u);
-              first_corr = false;
-            }
-            umma(d_main, a_hi, b_hi, idesc, first_main ? 0u : 1u);
-            first_main = false;
-          }
-          umma_commit(&empty[stage]);  // smem slot free once these MMAs retire
-          if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
-          if ((kb + 1) % TC_PROMOTE == 0 || kb == kbn_ - 1) {
-            umma_commit(&main_full[mb]);  // main partial ready for promotion
-            if (++mb == 2) { mb = 0; mb_phase ^= 1u; }
-          }
-        }
-        if (gs.split3) {
-          umma_commit(&corr_full[cb]);
-          if (++cb == 2) { cb = 0; cb_phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp >= 6 && !TcSplit<EPI, F16>::value) {
-    // ===================== converter warps (6..7) =====================
-    // The split is elementwise, so it is independent of the (swizzled) tile layout: byte i of the A_hi tile maps
-    // to byte i of the A_lo tile.  TMA zero-fills out-of-range rows, whose lo is 0 as well.
-    if (a_lo_conv) {
-      const int ct = threadIdx.x - 6 * 32;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int seed_, m0_, n0_, kb0_, kbn_;
-        decode(tile, seed_, m0_, n0_, kb0_, kbn_);
-        for (int kb = 0; kb < kbn_; ++kb) {
-          mbar_wait(&full[stage], phase);
-          const float4* src = reinterpret_cast<const float4*>(smem_al + stage * TC_STAGE_BYTES + TC_A_HI);
-          float4* dst = reinterpret_cast<float4*>(smem_al + stage * TC_STAGE_BYTES + TC_A_LO);
-          constexpr int PER = TC_TILE_BYTES / 16 / TC_CONV_THREADS;  // 16 float4 per thread
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            float4 v[PER / 2];
-#pragma unroll
-            for (int i = 0; i < PER / 2; ++i) v[i] = src[(half * (PER / 2) + i) * TC_CONV_THREADS + ct];
-#pragma unroll
-            for (int i = 0; i < PER / 2; ++i)
-              dst[(half * (PER / 2) + i) * TC_CONV_THREADS + ct] =
-                  make_float4(tf32_lo(v[i].x), tf32_lo(v[i].y), tf32_lo(v[i].z), tf32_lo(v[i].w));
-          }
-          fence_proxy_async_smem();
-          mbar_arrive(&lo_full[stage]);
-          if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue warps (2..5; split mode: 2..9) =====================
-    constexpr bool SPLIT = TcSplit<EPI, F16>::value;
-    constexpr int NC = SPLIT ? 64 : 128;   // accumulator columns per thread
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access (warp id % 4)
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const int col_off = SPLIT ? (warp >= 6 ? 64 : 0) : 0;
-    int mb = 0, cb = 0, ab = 0;
-    uint32_t mb_phase = 0, cb_phase = 0, ab_phase = 0;
-    const bool single_acc = !F16 && gs.split3 && gs.k_blocks <= TC_PROMOTE;  // see the MMA issuer
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int seed, m0, n0, kb0, kbn;
-      const int ks = decode(tile, seed, m0, n0, kb0, kbn);
-      const int partials = (kbn + TC_PROMOTE - 1) / TC_PROMOTE;
-      uint32_t mask_bits[4] = {0u, 0u, 0u, 0u};
-      if constexpr (EPI == EPI_RELU_MASK) prefetch_mask_bits(ep, seed, m0 + quad * 32, n0, lane, gs.M, mask_bits);
-      if constexpr (EPI == EPI_RELU_BITS) {
-        // packed ReLU mask written by the conv forward: 16 bytes per (row, 128-column tile)
-        const int m = m0 + quad * 32 + lane;
-        if (m < gs.M) {
-          const uint32_t* bp = ep.relu_bits + ((int64_t)seed * ep.rows + m) * (ep.ld_out >> 5) + (n0 >> 5);
-          if constexpr (SPLIT) {
-            const uint2 b = __ldg(reinterpret_cast<const uint2*>(bp + (col_off >> 5)));
-            mask_bits[0] = b.x; mask_bits[1] = b.y;
-          } else {
-            const uint4 b = __ldg(reinterpret_cast<const uint4*>(bp));
-            mask_bits[0] = b.x; mask_bits[1] = b.y; mask_bits[2] = b.z; mask_bits[3] = b.w;
-          }
-        }
-      }
-      if constexpr (!SPLIT) stage_epi_params<EPI>(ep, sp_all, seed, threadIdx.x - 64);
-      float acc[NC];
-      if (single_acc) {
-        uint64_t* e_bar = ab < 2 ? &main_empty[ab] : &corr_empty[ab - 2];
-        uint64_t* f_bar = ab < 2 ? &main_full[ab] : &corr_full[ab - 2];
-        mbar_wait(f_bar, ab_phase);
-        tcgen05_fence_after();
-        tmem_accumulate_row<true, NC>(tmem_base + ab * 128 + col_off + lane_off, acc);
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(e_bar);
-        if (++ab == 4) { ab = 0; ab_phase ^= 1u; }
-      } else {
-      for (int pi = 0; pi < partials; ++pi) {
-        mbar_wait(&main_full[mb], mb_phase);
-        tcgen05_fence_after();
-        if (pi == 0) tmem_accumulate_row<true, NC>(tmem_base + mb * 128 + col_off + lane_off, acc);
-        else tmem_accumulate_row<false, NC>(tmem_base + mb * 128 + col_off + lane_off, acc);
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&main_empty[mb]);
-        if (++mb == 2) { mb = 0; mb_phase ^= 1u; }
-      }
-      if (gs.split3) {
-        mbar_wait(&corr_full[cb], cb_phase);
-        tcgen05_fence_after();
-        tmem_accumulate_row<false, NC>(tmem_base + 256 + cb * 128 + col_off + lane_off, acc, F16 ? TC_LO_INV : 1.0f);
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&corr_empty[cb]);
-        if (++cb == 2) { cb = 0; cb_phase ^= 1u; }
-      }
-      }
-      if (F16 && ep.out_scale != 0.f) {   // undo the power-of-two pre-scaling of an operand (exact)
-#pragma unroll
-        for (int j = 0; j < NC; ++j) acc[j] *= ep.out_scale;
-      }
-      if constexpr (SPLIT) {
-        const int m_base = m0 + quad * 32;
-        float* out = ep.out + (int64_t)ks * ep.split_stride + (int64_t)seed * ep.out_seed_stride +
-                     (int64_t)m_base * ep.ld_out + n0 + col_off;
-        float* stg = stage_all + (warp - 2) * 32 * 32;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v[j] = acc[c * 32 + j];
-            if (EPI == EPI_RELU_BITS) v[j] = ((mask_bits[c] >> j) & 1u) ? v[j] : 0.f;
-          }
-          store_chunk_swz(stg, v, lane, out + c * 32, ep.ld_out, m_base, gs.M);
-        }
-      } else {
-        epilogue_row<EPI>(ep, acc, stage_all + (warp - 2) * 32 * STG_LD, sp_all, lane, seed, m0 + quad * 32, n0, gs.M,
-                          mask_bits);
-      }
-    }
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  // ===================== consumers (warps 0-7) =====================
+  const int t = threadIdx.x;                 // 0..255
+  const int wg = t >> 7;                     // warpgroup: tile rows 64 * wg ..
+  // A operand of this warpgroup: rows 64 * wg.. of a K-major tile (64 rows x 128 B) or the second 64-wide MN box
+  const uint32_t a_off = wg * 8192;
+  // fragment coordinates (see wgmma_f16_m64n128): rows fr, fr + 8; columns 8 j + fc, 8 j + fc + 1
+  const int fr = 64 * wg + 16 * ((t & 127) >> 5) + (lane >> 2), fc = 2 * (lane & 3);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int seed, m0, n0, kb0, kbn;
+    const int ks_idx = decode(tile, seed, m0, n0, kb0, kbn);
+    consumer_bar_sync();   // the previous tile's epilogue is done with tile_s
+    if constexpr (!F16) {
+      tf32_tile<A_MN, B_MN>(smem_al, tile_s, full, empty, stage, phase, kbn, gs.split3,
+                            ep.out_scale != 0.f ? ep.out_scale : 1.0f, warp, lane);
+    } else {
+    float mainacc[64], corr[64];   // scoped to the k loop: dead (no registers) during the epilogue
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { mainacc[i] = 0.f; corr[i] = 0.f; }
+    for (int kb = 0; kb < kbn; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sb = smem_base + stage * TC_STAGE_BYTES;
+      const uint32_t first_corr = kb == 0 ? 0u : 1u, first_main = kb % TC_PROMOTE == 0 ? 0u : 1u;
+      fence_operands(mainacc); fence_operands(corr);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t a_hi = make_gdesc16<A_MN>(sb + TC_A_HI + a_off, ks), a_lo = make_gdesc16<A_MN>(sb + TC_A_LO + a_off, ks);
+        const uint64_t b_hi = make_gdesc16<B_MN>(sb + TC_B_HI, ks), b_lo = make_gdesc16<B_MN>(sb + TC_B_LO, ks);
+        wgmma_f16_m64n128<A_MN, B_MN>(corr, a_lo, b_hi, ks == 0 ? first_corr : 1u);
+        wgmma_f16_m64n128<A_MN, B_MN>(corr, a_hi, b_lo, 1u);
+        wgmma_f16_m64n128<A_MN, B_MN>(mainacc, a_hi, b_hi, ks == 0 ? first_main : 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(mainacc); fence_operands(corr);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);   // smem slot free: this warp's MMAs have retired
+      if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
+      if ((kb + 1) % TC_PROMOTE == 0 || kb == kbn - 1) {   // promote the main partial into the fp32 tile
+        const bool first = kb < TC_PROMOTE;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float2* p = reinterpret_cast<float2*>(tile_s + (fr + 8 * h) * TC_ACC_LD + 8 * j + fc);
+            const float2 v = make_float2(mainacc[4 * j + 2 * h], mainacc[4 * j + 2 * h + 1]);
+            if (first) *p = v;
+            else { const float2 o = *p; *p = make_float2(o.x + v.x, o.y + v.y); }
+          }
+      }
+    }
+    {   // the correction accumulator (units of 2^-11), then the power-of-two output scale (exact)
+      const float osc = ep.out_scale != 0.f ? ep.out_scale : 1.0f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float2* p = reinterpret_cast<float2*>(tile_s + (fr + 8 * h) * TC_ACC_LD + 8 * j + fc);
+          float2 o = kbn > 0 ? *p : make_float2(0.f, 0.f);
+          if (kbn > 0) {
+            o.x = fmaf(corr[4 * j + 2 * h], TC_LO_INV, o.x);
+            o.y = fmaf(corr[4 * j + 2 * h + 1], TC_LO_INV, o.y);
+          }
+          *p = make_float2(o.x * osc, o.y * osc);
+        }
+    }
+    }
+    consumer_bar_sync();   // tile_s complete
+
+    if constexpr (EPI == EPI_LN_TRAIN || EPI == EPI_LN_HEAD) {
+      if (t < 128) {
+        stage_epi_params<EPI>(ep, sp_all, seed, t);
+        float acc[128];
+        const float* row = tile_s + t * TC_ACC_LD;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const float4 v = *reinterpret_cast<const float4*>(row + 4 * j);
+          acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
+        }
+        __syncwarp();   // the warp's own 32 rows of tile_s become its store staging area
+        epilogue_ln_row<EPI>(ep, acc, tile_s + warp * 32 * TC_ACC_LD, sp_all, lane, seed, m0 + warp * 32, gs.M);
+      }
+    } else {
+      // EPI_STORE / EPI_RELU_MASK / EPI_RELU_BITS: the 256 consumers copy tile rows out, 512 B per row and warp
+      // instruction; the ReLU masks are read with the same addressing (dgrad runs in place: out may equal mask)
+      const int64_t base = (int64_t)seed * ep.out_seed_stride + n0;
+      float* out = ep.out + (EPI == EPI_STORE ? (int64_t)ks_idx * ep.split_stride : 0) + base;
+      for (int i = t; i < 128 * 32; i += TC_CONSUMERS) {
+        const int r = i >> 5, c4 = i & 31, m = m0 + r;
+        if (m >= gs.M) break;   // rows ascend with i
+        float4 v = *reinterpret_cast<const float4*>(tile_s + r * TC_ACC_LD + 4 * c4);
+        if constexpr (EPI == EPI_RELU_MASK) {
+          const float4 mk = *reinterpret_cast<const float4*>(ep.mask + base + (int64_t)m * ep.ld_out + 4 * c4);
+          v.x = mk.x > 0.f ? v.x : 0.f; v.y = mk.y > 0.f ? v.y : 0.f;
+          v.z = mk.z > 0.f ? v.z : 0.f; v.w = mk.w > 0.f ? v.w : 0.f;
+        }
+        if constexpr (EPI == EPI_RELU_BITS) {
+          // packed ReLU mask written by the conv forward: one word per (row, 32 columns)
+          const uint32_t wd = __ldg(ep.relu_bits + ((int64_t)seed * ep.rows + m) * (ep.ld_out >> 5) + ((n0 >> 5) + (c4 >> 3)));
+          const uint32_t b = wd >> (4 * (c4 & 7));
+          v.x = (b & 1u) ? v.x : 0.f; v.y = (b & 2u) ? v.y : 0.f;
+          v.z = (b & 4u) ? v.z : 0.f; v.w = (b & 8u) ? v.w : 0.f;
+        }
+        *reinterpret_cast<float4*>(out + (int64_t)m * ep.ld_out + 4 * c4) = v;
+      }
+    }
   }
 }
 
@@ -640,10 +488,11 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// 3-D fp32 tensor [seeds][mid][inner] with a {32, box_mid, 1} box; SWIZZLE_128B for K-major operand tiles,
-// SWIZZLE_128B_ATOM_32B for MN-major ones (see make_sdesc).
+static int num_sms() { return device_sm_count(); }
+
+// 3-D fp32 tensor [seeds][mid][inner] with a {32, box_mid, 1} box (128 bytes x box_mid), SWIZZLE_128B for both majors
 int make_tmap(CUtensorMap* tm, const float* base, uint64_t inner, uint64_t mid, uint64_t seeds, uint64_t mid_stride_elems,
-              uint64_t seed_stride_elems, uint32_t box_mid, int mn_major) {
+              uint64_t seed_stride_elems, uint32_t box_mid) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return set_error(PQN_E_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t dims[3] = {inner, mid, seeds};
@@ -651,28 +500,23 @@ int make_tmap(CUtensorMap* tm, const float* base, uint64_t inner, uint64_t mid, 
   cuuint32_t box[3] = {32, box_mid, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(PQN_E_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
   return PQN_OK;
 }
 
-static int num_sms() { return device_sm_count(); }
-
-template <int A_MN, int B_MN, int EPI, bool F16 = false>
+template <int A_MN, int B_MN, int EPI, bool F16>
 static int launch_t(const CUtensorMap* t, const GemmShape& gs, const EpiParams& ep, cudaStream_t st, int kid) {
   auto kfn = tc_gemm_kernel<A_MN, B_MN, EPI, F16>;
-  constexpr int SMEM = TcSplit<EPI, F16>::smem, THREADS = TcSplit<EPI, F16>::threads;
-  static_assert(SMEM <= 227 * 1024, "dynamic shared memory of the GEMM kernel exceeds the per-CTA limit");
-  if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess)
+  static_assert(TC_SMEM_BYTES <= 227 * 1024, "dynamic shared memory of the GEMM kernel exceeds the per-CTA limit");
+  if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
     return check_launch("tc_gemm(cudaFuncSetAttribute)");
   const int tiles = gs.m_tiles * gs.n_tiles * gs.S * (gs.k_split > 1 ? gs.k_split : 1);
   const int grid = tiles < num_sms() ? tiles : num_sms();
   {
     LaunchScope _ls(kid < 0 ? (int)K_TC_GEMM : kid, st);
-    kfn<<<grid, THREADS, SMEM, st>>>(t[0], t[1], t[2], t[3], gs, ep);
+    kfn<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(t[0], t[1], t[2], t[3], gs, ep);
   }
   return check_launch("tc_gemm");
 }
@@ -680,7 +524,7 @@ static int launch_t(const CUtensorMap* t, const GemmShape& gs, const EpiParams& 
 int launch_gemm(int a_mn, int b_mn, int epi, const CUtensorMap* t, const GemmShape& gs, const EpiParams& ep,
                 cudaStream_t st, int kernel_id) {
 #define PQN_TC_CASE(A, B, E) \
-  if (a_mn == A && b_mn == B && epi == E) return launch_t<A, B, E>(t, gs, ep, st, kernel_id);
+  if (a_mn == A && b_mn == B && epi == E) return launch_t<A, B, E, false>(t, gs, ep, st, kernel_id);
   PQN_TC_CASE(0, 1, EPI_STORE)
   PQN_TC_CASE(0, 1, EPI_LN_TRAIN)
   PQN_TC_CASE(0, 1, EPI_LN_HEAD)
@@ -745,81 +589,6 @@ __global__ void split16_kernel(const float* __restrict__ x, __half* __restrict__
   reinterpret_cast<uint2*>(lo)[i] = make_uint2(*reinterpret_cast<uint32_t*>(&l0), *reinterpret_cast<uint32_t*>(&l1));
 }
 
-// Debug kernel: one CTA, one 128x128x32 tile, no pipelining.  Dumps the smem tiles TMA produced and the TMEM
-// accumulator after `nk` k-steps so that descriptor/layout problems can be diagnosed from the host.
-template <int A_MN, int B_MN>
-__global__ void __launch_bounds__(128, 1)
-    tc_debug_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                    float* __restrict__ dump_a, float* __restrict__ dump_b, float* __restrict__ out_d, int nk,
-                    uint32_t* __restrict__ info) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_al + 2 * TC_TILE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) {
-    info[0] = tmem_base;
-    info[1] = smem_base;
-    mbar_expect_tx(&bars[0], 2 * TC_TILE_BYTES);
-    if (A_MN) {
-      for (int j = 0; j < 4; ++j) tma_load_3d(smem_base + j * 4096, &tm_a, &bars[0], 32 * j, 0, 0);
-    } else {
-      tma_load_3d(smem_base, &tm_a, &bars[0], 0, 0, 0);
-    }
-    if (B_MN) {
-      for (int j = 0; j < 4; ++j) tma_load_3d(smem_base + TC_TILE_BYTES + j * 4096, &tm_b, &bars[0], 32 * j, 0, 0);
-    } else {
-      tma_load_3d(smem_base + TC_TILE_BYTES, &tm_b, &bars[0], 0, 0, 0);
-    }
-  }
-  mbar_wait(&bars[0], 0);
-  const float* sa = reinterpret_cast<const float*>(smem_al);
-  const float* sb = reinterpret_cast<const float*>(smem_al + TC_TILE_BYTES);
-  for (int i = threadIdx.x; i < 4096; i += 128) { dump_a[i] = sa[i]; dump_b[i] = sb[i]; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    tcgen05_fence_after();
-    const uint32_t idesc = make_idesc_tf32(128, 128, A_MN, B_MN);
-    info[2] = idesc;
-    for (int ks = 0; ks < nk; ++ks) {
-      const uint64_t da = make_sdesc<A_MN>(smem_base, ks);
-      const uint64_t db = make_sdesc<B_MN>(smem_base + TC_TILE_BYTES, ks);
-      if (ks == 0) { info[4] = (uint32_t)da; info[5] = (uint32_t)(da >> 32); info[6] = (uint32_t)db; info[7] = (uint32_t)(db >> 32); }
-      umma_tf32(tmem_base, da, db, idesc, ks > 0 ? 1u : 0u);
-    }
-    umma_commit(&bars[1]);
-  }
-  mbar_wait(&bars[1], 0);
-  tcgen05_fence_after();
-  const int row = warp * 32 + lane;
-  for (int c = 0; c < 4; ++c) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(warp * 32) << 16) + c * 32, v);
-    tmem_ld_wait();
-    for (int j = 0; j < 32; ++j) out_d[row * 128 + c * 32 + j] = __uint_as_float(v[j]);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 128);
-  }
-}
-
 }  // namespace tc
 }  // namespace pqn
 
@@ -849,8 +618,11 @@ int pqn_tc_split16(const float* x, void* hi, void* lo, int64_t n, float scale, v
   return check_launch("pqn_tc_split16");
 }
 
-// Test hook: D[s] = A[s] . B[s] * out_scale on the fp16-split tcgen05 path; operands are the (hi, lo') planes written
-// by pqn_tc_split16.  Layout flags as in pqn_tc_gemm_test; N % 128 == 0.
+// Test hook: D[s] = A[s] . B[s] * out_scale on the fp16-split wgmma path; operands are the (hi, lo') planes written
+// by pqn_tc_split16.
+//   a_mn = 0: A is [S][M][K] (K contiguous)   a_mn = 1: A is [S][K][M] (M contiguous)
+//   b_mn = 0: B is [S][N][K] (K contiguous)   b_mn = 1: B is [S][K][N] (N contiguous)
+// N % 128 == 0; rows of a ragged M are guarded, a ragged K is zero-filled by TMA.
 int pqn_tc_gemm16_test(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, float* d, int32_t S,
                        int32_t M, int32_t N, int32_t K, int a_mn, int b_mn, float out_scale, void* stream) {
   if (!a_hi || !a_lo || !b_hi || !b_lo || !d || S <= 0 || M <= 0 || N <= 0 || K <= 0 || (N % 128) || (K % 8) || (M % 8))
@@ -867,65 +639,34 @@ int pqn_tc_gemm16_test(const void* a_hi, const void* a_lo, const void* b_hi, con
   }
   GemmShape gs = {};
   gs.S = S; gs.M = M; gs.m_tiles = (M + 127) / 128; gs.n_tiles = N / 128; gs.k_blocks = (K + TC_BK16 - 1) / TC_BK16;
-  gs.split3 = 1;
   EpiParams ep = {};
   ep.out = d; ep.ld_out = N; ep.out_seed_stride = (int64_t)M * N; ep.out_scale = out_scale;
   return launch_gemm16(a_mn, b_mn, EPI_STORE, t, gs, ep, (cudaStream_t)stream);
 }
 
-// Debug hook (tests only): single 128x128x32 tile; a: [128][32] (a_mn=0) or [32][128] (a_mn=1); same for b.
-int pqn_tc_debug(const float* a, const float* b, float* dump_a, float* dump_b, float* out_d, uint32_t* info, int a_mn,
-                 int b_mn, int nk, void* stream) {
-  CUtensorMap ta, tb;
-  int rc;
-  if (a_mn) { if ((rc = make_tmap(&ta, a, 128, 32, 1, 128, 4096, 32, 1))) return rc; }
-  else { if ((rc = make_tmap(&ta, a, 32, 128, 1, 32, 4096, 128, 0))) return rc; }
-  if (b_mn) { if ((rc = make_tmap(&tb, b, 128, 32, 1, 128, 4096, 32, 1))) return rc; }
-  else { if ((rc = make_tmap(&tb, b, 32, 128, 1, 32, 4096, 128, 0))) return rc; }
-  const int smem = 2 * TC_TILE_BYTES + 1024 + 64;
-  cudaStream_t st = (cudaStream_t)stream;
-#define PQN_DBG(A, B)                                                                                        \
-  if (a_mn == A && b_mn == B) {                                                                              \
-    cudaFuncSetAttribute(tc_debug_kernel<A, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);          \
-    tc_debug_kernel<A, B><<<1, 128, smem, st>>>(ta, tb, dump_a, dump_b, out_d, nk, info);                    \
-  }
-  PQN_DBG(0, 0) PQN_DBG(0, 1) PQN_DBG(1, 0) PQN_DBG(1, 1)
-#undef PQN_DBG
-  return check_launch("pqn_tc_debug");
-}
-
-// Test hook: D[s] = A[s] . B[s] on the tcgen05 path (fp32 in, fp32 out).
-//   a_mn = 0: A is [S][M][K] (K contiguous)   a_mn = 1: A is [S][K][M] (M contiguous)
-//   b_mn = 0: B is [S][N][K] (K contiguous)   b_mn = 1: B is [S][K][N] (N contiguous)
+// Test hook: D[s] = A[s] . B[s] on the TF32 path (fp32 in, fp32 out).  Layout flags as in pqn_tc_gemm16_test.
 //   split3 = 1: 3xTF32 (a_lo / b_lo must hold x - trunc_tf32(x)); 2: same, but A_lo is derived in the kernel
-//   (a_lo unused); 0: single-pass TF32.
-// M, N multiples of 128 are not required for M (rows are guarded); N % 128 == 0, K % 32 == 0 or zero-filled.
+//   (a_lo unused); 0: single-pass TF32.  N % 128 == 0; rows of a ragged M are guarded, a ragged K is zero-filled.
 int pqn_tc_gemm_test(const float* a, const float* a_lo, const float* b, const float* b_lo, float* d, int32_t S,
                      int32_t M, int32_t N, int32_t K, int a_mn, int b_mn, int split3, void* stream) {
-  if (!a || !b || !d || S <= 0 || M <= 0 || N <= 0 || K <= 0 || (N % 128) || (split3 && !b_lo) || (split3 == 1 && !a_lo))
+  if (!a || !b || !d || S <= 0 || M <= 0 || N <= 0 || K <= 0 || (N % 128) || split3 < 0 || split3 > 2 ||
+      (split3 && !b_lo) || (split3 == 1 && !a_lo))
     return set_error(PQN_E_INVALID, "pqn_tc_gemm_test: bad argument");
   CUtensorMap t[4];
   int rc;
   const float* al = split3 == 1 ? a_lo : a;
   const float* bl = split3 ? b_lo : b;
-  if (a_mn) {
-    if ((rc = make_tmap(&t[0], a, M, K, S, M, (uint64_t)M * K, 32, 1))) return rc;
-    if ((rc = make_tmap(&t[1], al, M, K, S, M, (uint64_t)M * K, 32, 1))) return rc;
-  } else {
-    if ((rc = make_tmap(&t[0], a, K, M, S, K, (uint64_t)M * K, 128, 0))) return rc;
-    if ((rc = make_tmap(&t[1], al, K, M, S, K, (uint64_t)M * K, 128, 0))) return rc;
-  }
-  if (b_mn) {
-    if ((rc = make_tmap(&t[2], b, N, K, S, N, (uint64_t)N * K, 32, 1))) return rc;
-    if ((rc = make_tmap(&t[3], bl, N, K, S, N, (uint64_t)N * K, 32, 1))) return rc;
-  } else {
-    if ((rc = make_tmap(&t[2], b, K, N, S, K, (uint64_t)N * K, 128, 0))) return rc;
-    if ((rc = make_tmap(&t[3], bl, K, N, S, K, (uint64_t)N * K, 128, 0))) return rc;
+  const float* ap[2] = {a, al};
+  const float* bp[2] = {b, bl};
+  for (int i = 0; i < 2; ++i) {
+    if (a_mn) { if ((rc = make_tmap(&t[i], ap[i], M, K, S, M, (uint64_t)M * K, 32))) return rc; }
+    else { if ((rc = make_tmap(&t[i], ap[i], K, M, S, K, (uint64_t)M * K, 128))) return rc; }
+    if (b_mn) { if ((rc = make_tmap(&t[2 + i], bp[i], N, K, S, N, (uint64_t)N * K, 32))) return rc; }
+    else { if ((rc = make_tmap(&t[2 + i], bp[i], K, N, S, K, (uint64_t)N * K, 128))) return rc; }
   }
   GemmShape gs = {};
   gs.S = S; gs.M = M; gs.m_tiles = (M + 127) / 128; gs.n_tiles = N / 128; gs.k_blocks = (K + TC_BK - 1) / TC_BK;
-  gs.split3 = split3 ? 1 : 0;
-  gs.a_lo_inline = split3 == 2;
+  gs.split3 = split3;
   EpiParams ep = {};
   ep.out = d; ep.ld_out = N; ep.out_seed_stride = (int64_t)M * N;
   return launch_gemm(a_mn, b_mn, EPI_STORE, t, gs, ep, (cudaStream_t)stream);

@@ -1,4 +1,4 @@
-// PTX wrappers and constants of the tcgen05 / TMEM / TMA GEMM path (sm_100a).
+// PTX wrappers and constants of the wgmma / mma.sync / TMA / mbarrier GEMM path (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -7,23 +7,23 @@
 namespace pqn {
 namespace tc {
 
-constexpr int TC_THREADS = 256;          // warp0 TMA, warp1 MMA, warps 2-5 epilogue (warp2 also owns TMEM alloc),
-                                         // warps 6-7 operand converters (in-kernel A_lo, see GemmShape::a_lo_inline)
-constexpr int TC_CONV_THREADS = 64;
-constexpr int TC_BK = 32;                // fp32 (tf32 path) elements per k-block = one 128-byte swizzle row
-constexpr int TC_BK16 = 64;              // fp16 (f16 path) elements per k-block = one 128-byte swizzle row
-constexpr int TC_STAGES = 3;
-constexpr int TC_PROMOTE = 4;             // k-blocks per in-TMEM main chain (16 MMAs) before promotion to registers
-constexpr int TC_TILE_BYTES = 128 * TC_BK * 4;   // 16 KB: 128 rows x 128 bytes for either element type
+constexpr int TC_CONSUMERS = 256;        // two consumer warpgroups: rows 0-63 and 64-127 of the 128 x 128 tile
+constexpr int TC_THREADS = TC_CONSUMERS + 32;   // + one TMA producer warp (warp 8)
+constexpr int TC_BK16 = 64;              // fp16 elements per k-block = one 128-byte swizzle row
+constexpr int TC_BK = 32;                // fp32 (TF32 path) elements per k-block = one 128-byte swizzle row
+constexpr int TC_STAGES = 2;             // 2 x 64 KB operand stages + the 66 KB fp32 tile fit in 227 KB
+constexpr int TC_PROMOTE = 4;            // k-blocks per register main chain (16 k-steps) before promotion to the fp32 tile
+constexpr int TC_TILE_BYTES = 128 * TC_BK16 * 2;  // 16 KB: 128 rows x 128 bytes
 // fp16 split: x = hi + lo' * 2^-11 with hi = fp16(x), lo' = fp16((x - hi) * 2^11): 22 significant bits, the scaled lo'
-// stays a normal fp16 number down to |x| ~ 1e-7.  The two cross products accumulate in the `corr` TMEM accumulator
-// in units of 2^-11.
+// stays a normal fp16 number down to |x| ~ 1e-7.  The two cross products accumulate in their own `corr` register
+// accumulator in units of 2^-11.
 constexpr float TC_LO_SCALE = 2048.0f, TC_LO_INV = 1.0f / 2048.0f;
 constexpr int TC_A_HI = 0, TC_A_LO = TC_TILE_BYTES, TC_B_HI = 2 * TC_TILE_BYTES, TC_B_LO = 3 * TC_TILE_BYTES;
 constexpr int TC_STAGE_BYTES = 4 * TC_TILE_BYTES;  // 64 KB
-constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ +
-                              4 * 32 * 36 * 4 /*epilogue store staging, 4 warps x [32][36] floats*/ +
-                              (384 + 8 * 128 + 8) * 4 /*per-seed epilogue parameters (LN scale/bias, Q-head)*/;
+constexpr int TC_ACC_LD = 132;           // floats per row of the fp32 result tile (conflict-free 16-byte row reads)
+constexpr int TC_SP_FLOATS = 384 + 8 * 128 + 8;   // per-seed epilogue parameters (LN scale/bias, Q-head)
+constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 128 * TC_ACC_LD * 4 + TC_SP_FLOATS * 4 + 256 /*barriers*/ +
+                              1024 /*align slack*/;
 #define PQN_TC_MAX_A 8
 
 enum Epilogue : int { EPI_STORE = 0, EPI_LN_TRAIN = 1, EPI_LN_HEAD = 2, EPI_RELU_MASK = 3, EPI_RELU_BITS = 4 };
@@ -32,16 +32,15 @@ struct GemmShape {
   int S;         // batch (seeds)
   int M;         // rows of D that exist (rows >= M are not stored)
   int m_tiles, n_tiles, k_blocks;
-  int split3;    // 1: split precision (3 tensor-core products per k-step), 0: single pass
+  int split3;    // TF32 kernel only: 0 single pass, 1 3xTF32 with A_lo from memory, 2 3xTF32 with A_lo derived in the
+                 // kernel (the fp16 kernel always takes both planes of both operands)
   int k_split;   // >1: the k-blocks of every output tile are divided over k_split CTAs; partial ks goes to
                  // out + ks * EpiParams::split_stride (EPI_STORE only) and a reduce kernel adds them in order
-  int a_lo_inline;  // split3 only: 1 = no A_lo tensor in memory; the converter warps derive A_lo = A - trunc_tf32(A)
-                    // from the A tile TMA staged in shared memory (halves the HBM traffic of the A operand)
 };
 
 struct EpiParams {
   int64_t split_stride;  // elements between the partial outputs of a split-K launch
-  float out_scale;  // F16 kernels: result = (main + corr * 2^-11) * out_scale (undoes the operand pre-scaling); 0 => 1
+  float out_scale;  // result = (main + corr * 2^-11) * out_scale (undoes the operand pre-scaling); 0 => 1
   // EPI_STORE / EPI_RELU_MASK
   float* out;
   const float* mask;
@@ -57,7 +56,7 @@ struct EpiParams {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ float tf32_lo(float x) {
-  const float hi = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);  // what the tensor core reads of x
+  const float hi = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);  // what a TF32 tensor-core read keeps of x
   return x - hi;                                                       // exact in fp32
 }
 
@@ -86,9 +85,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   } while (!ok);
 }
 
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma operand reads, TMA)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
 // ---- TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
@@ -100,87 +96,54 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap
       : "memory");
 }
 
-// ---- tcgen05
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols) : "memory");
+// ---- wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads/writes across the asynchronous MMAs
+__device__ __forceinline__ void fence_operands(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x 128] (+)= A[64 x 16] . B[16 x 128], fp16 operands from shared memory, fp32 accumulate in registers.
+// TA / TB = 1: the operand is MN-major in shared memory (transposed read).  scale_d = 0 overwrites D.
+// D fragment of thread t of the warpgroup: rows 16 * (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1):
+// d[4j], d[4j+1] on the first row, d[4j+2], d[4j+3] on the second.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_m64n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+      "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (bits 4-5 = 1), a/b format TF32 (= 2,
-// bits 7-9 / 10-12), a_major bit 15, b_major bit 16 (1 = MN-major), N>>3 at bits 17-22, M>>4 at bits 24-28.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// kind::f16 with fp16 operands (a/b format F16 = 0), fp32 accumulate
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor) for a 128 x 32 fp32 operand tile in SWIZZLE_128B
-// atoms (8 rows x 128 B = 1024 B), k-step `ks` selects 8 of the 32 k values:
-//   K-major  tile: row r (MN index) at r*128 B; 8-row atoms every 1024 B (SBO); the k-step advances 32 B in the row.
-//   MN-major tile (32-bit types need the 32-byte-base swizzle, LayoutType SWIZZLE_128B_BASE32B = 1, written by TMA's
-//                  CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): 4 boxes of [32 k rows][32 mn] at 4096 B (LBO between MN
-//                  atoms); atoms are [4 k][128 B] = 512 B (SBO between k atoms); one k-step (8 k) = 1024 B.
+// Shared-memory matrix descriptor (sm_90 GMMA: start >> 4 at bits 0-13, LBO >> 4 at 16-29, SBO >> 4 at 32-45,
+// layout type at 62-63, 1 = SWIZZLE_128B) for a fp16 operand tile as TMA writes it; k-step `ks` = 16 k values:
+//   K-major : 128-byte rows (64 k), 8-row swizzle atoms every 1024 B (SBO); the k-step advances 32 B in the row.
+//   MN-major: TMA boxes of [64 k rows][64 mn = 128 B] at 8192 B (LBO: next 64 MN elements), 8-row k atoms of
+//             1024 B (SBO); one k-step (16 k rows) = 2048 B.
+// Tile bases are 1024-byte aligned, so the swizzle phase (base offset) is 0.
 template <int MN>
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t tile_addr, int ks) {
-  const uint32_t addr = MN ? tile_addr + ks * 1024 : tile_addr + ks * 32;
-  const uint64_t lbo = MN ? (4096u >> 4) : 1u;
-  const uint64_t sbo = MN ? (512u >> 4) : (1024u >> 4);
-  const uint64_t layout = MN ? 1ull : 2ull;
-  return (uint64_t)((addr >> 4) & 0x3FFFu) | (lbo << 16) | (sbo << 32) | (1ull << 46) /*version*/ | (layout << 61);
-}
-
-// The same for a 128 x 64 fp16 operand tile (k-step = 16 k values):
-//   K-major : identical byte geometry (128-byte rows, 8-row atoms, 32 B per k-step);
-//   MN-major: the ordinary SWIZZLE_128B canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units -- 2 TMA boxes
-//             of [64 k rows][64 mn = 128 B] at 8192 B (LBO between MN atoms), k atoms of 8 rows = 1024 B (SBO); one
-//             k-step (16 k rows) = 2048 B.
-template <int MN>
-__device__ __forceinline__ uint64_t make_sdesc16(uint32_t tile_addr, int ks) {
+__device__ __forceinline__ uint64_t make_gdesc16(uint32_t tile_addr, int ks) {
   const uint32_t addr = MN ? tile_addr + ks * 2048 : tile_addr + ks * 32;
   const uint64_t lbo = MN ? (8192u >> 4) : 1u;
   const uint64_t sbo = 1024u >> 4;
-  return (uint64_t)((addr >> 4) & 0x3FFFu) | (lbo << 16) | (sbo << 32) | (1ull << 46) /*version*/ | (2ull << 61);
+  return (uint64_t)((addr >> 4) & 0x3FFFu) | (lbo << 16) | (sbo << 32) | (1ull << 62);
 }
 
 // fp16 split of an fp32 value (see TC_LO_SCALE); saturates instead of overflowing to inf
@@ -202,13 +165,15 @@ __device__ __forceinline__ void split16x2(float x0, float x1, __half2& hi, __hal
 }
 
 // host-side pieces used by other translation units (pqn_net.cu)
+// fp32 tensor [seeds][mid][inner] with a {32, box_mid, 1} box, SWIZZLE_128B for both majors
 int make_tmap(CUtensorMap* tm, const float* base, uint64_t inner, uint64_t mid, uint64_t seeds, uint64_t mid_stride_elems,
-              uint64_t seed_stride_elems, uint32_t box_mid, int mn_major);
+              uint64_t seed_stride_elems, uint32_t box_mid);
+// the TF32 kernel: t = {A, A_lo, B, B_lo} fp32 maps, gs.k_blocks counts 32-element k-blocks
+int launch_gemm(int a_mn, int b_mn, int epi, const CUtensorMap* t, const GemmShape& gs, const EpiParams& ep, cudaStream_t st,
+                int kernel_id = -1);
 // fp16 tensor [seeds][mid][inner] with a {64, box_mid, 1} box (128 bytes x box_mid), SWIZZLE_128B for both majors
 int make_tmap16(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t mid, uint64_t seeds, uint64_t mid_stride_elems,
                 uint64_t seed_stride_elems, uint32_t box_mid);
-int launch_gemm(int a_mn, int b_mn, int epi, const CUtensorMap* t, const GemmShape& gs, const EpiParams& ep, cudaStream_t st,
-                int kernel_id = -1);
 // the fp16-split kernel: t = {A_hi, A_lo', B_hi, B_lo'} fp16 maps, gs.k_blocks counts 64-element k-blocks
 int launch_gemm16(int a_mn, int b_mn, int epi, const CUtensorMap* t, const GemmShape& gs, const EpiParams& ep,
                   cudaStream_t st, int kernel_id = -1);

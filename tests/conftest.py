@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
 
 
 def _has_cuda():
@@ -31,9 +31,9 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session", autouse=True)
 def _built_library():
-    """Every test may assume the in-tree library exists.  Without a GPU (this container, the driver's CPU run) it is
-    built incrementally (nvcc cross-compiles sm_100a); on the GPU box the .so shipped with the snapshot is used as
-    is -- file times are not meaningful there -- and only a missing library triggers a build."""
+    """Every test may assume the in-tree library exists.  Without a GPU it is built incrementally (nvcc
+    cross-compiles sm_90a); with a GPU an existing .so (the one build() made) is used as is -- file times of a copied
+    tree are not meaningful -- and only a missing library triggers a build."""
     from purejaxql_b200 import build
     if _has_cuda() and os.path.exists(build.OUT):
         return build.OUT

@@ -116,10 +116,10 @@ def test_config_composition_matches_hydra_semantics():
     assert c2["alg"]["ENV_NAME"] == "Acrobot-v1" and c2["alg"]["REW_SCALE"] == 0.1
 
 
-def test_library_sass_has_blackwell_tensor_and_tma_ops():
-    """The built .so must contain the sm_100a-native paths: tcgen05.mma (UTC*MMA), TMEM loads (LDTM),
-    TMA tensor loads (UTMALDG), the warp-level tf32 MMA of the conv kernels, the async-proxy fence of the in-kernel
-    operand converter and the cp.async staging of the conv backward."""
+def test_library_sass_has_hopper_tensor_and_tma_ops():
+    """The built .so must contain the sm_90a-native paths: warpgroup MMAs (HGMMA) behind their register fence
+    (WARPGROUP.ARRIVE), TMA tensor loads (UTMALDG) completing on mbarriers (SYNCS), the warp-level MMA of the conv
+    kernels (HMMA) and the cp.async staging of the conv backward (LDGSTS)."""
     import shutil
     import subprocess
     from purejaxql_b200 import build
@@ -127,8 +127,8 @@ def test_library_sass_has_blackwell_tensor_and_tma_ops():
         pytest.skip("cuobjdump not available")
     so = build.build()
     sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass or "SM100" in sass.upper()
-    for mnemonic in ("UTCHMMA", "LDTM", "UTMALDG", "UTCBAR", "HMMA", "FENCE.VIEW.ASYNC", "LDGSTS"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "WARPGROUP.ARRIVE", "UTMALDG", "SYNCS", "HMMA", "LDGSTS"):
         assert mnemonic in sass, f"{mnemonic} missing from the SASS of {so}"
 
 

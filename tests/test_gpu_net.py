@@ -52,15 +52,16 @@ def _ws(spec, S, rows):
     return torch.empty(n, dtype=torch.uint8, device=dev())
 
 
-@pytest.fixture(params=[(2, 1), (1, 1), (0, 0), (1, 0), (2, 2), (2, 3)],
+@pytest.fixture(params=[(2, 1), (1, 1), (0, 0), (1, 0), (2, 3)],
                 ids=["tcgen05_f16split+f16_mma_conv", "tcgen05_3xtf32+f16_mma_conv", "ffma", "tcgen05_3xtf32+cuda_conv",
-                     "tcgen05_f16split+tcgen05_conv", "tcgen05_f16split+tf32_mma_conv"])
+                     "tcgen05_f16split+tf32_mma_conv"])
 def dense_path(request):
-    """Runs the CNN tests on the implementation variants: dense layer on tcgen05 (fp16-split planes = default,
-    or 3xTF32) or fp32 FFMA; conv on warp-level tf32 MMA (default), fp32 CUDA cores or tcgen05."""
+    """Runs the CNN tests on the implementation variants: dense layer on the tensor cores (wgmma on fp16-split
+    planes, the default, or 3xTF32 on mma.sync; the ids keep their original names) or fp32 FFMA; conv on fp16
+    warp-level MMA (default), tf32 warp-level MMA or fp32 CUDA cores."""
     from purejaxql_b200 import _lib
-    _lib.lib().pqn_set_tensor_core_path(request.param[0])
-    _lib.lib().pqn_set_conv_mma_path(request.param[1])
+    _lib.check(_lib.lib().pqn_set_tensor_core_path(request.param[0]))
+    _lib.check(_lib.lib().pqn_set_conv_mma_path(request.param[1]))
     yield request.param
     _lib.lib().pqn_set_tensor_core_path(2)
     _lib.lib().pqn_set_conv_mma_path(1)
@@ -106,7 +107,7 @@ def test_cnn_forward_other_channel_counts_and_gather(dense_path):
 
 @pytest.fixture(params=[2, 0], ids=["hidden_layer_tcgen05_f16split", "ffma"])
 def mlp_path(request):
-    """The MLP's hidden layer (Dense_1: K = N = HIDDEN_SIZE) runs on the tcgen05 fp16-split GEMMs by default (round 2);
+    """The MLP's hidden layer (Dense_1: K = N = HIDDEN_SIZE) runs on the wgmma fp16-split GEMMs by default;
     path 0 keeps everything on the fp32 FFMA kernels."""
     from purejaxql_b200 import _lib
     _lib.lib().pqn_set_tensor_core_path(request.param)

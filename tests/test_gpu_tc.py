@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 / TMEM / TMA GEMM path (3xTF32) against fp64."""
+"""GPU tests of the tensor-core GEMM paths (TMA ring; 3xTF32 on mma.sync, fp16-split on wgmma) against fp64."""
 import numpy as np
 import pytest
 import torch
@@ -69,7 +69,7 @@ def test_tc_gemm_3xtf32_fp32_accuracy(a_mn, b_mn, S, M, N, K):
 
 
 # --------------------------------------------------------------------------- #
-# fp16-split path (round 2 default): operands as (hi, lo') fp16 planes, kind::f16, 64-element k-blocks
+# fp16-split path: operands as (hi, lo') fp16 planes, wgmma f16 with fp32 accumulate, 64-element k-blocks
 # --------------------------------------------------------------------------- #
 def _run16(S, M, N, K, a_mn, b_mn, seed=0, a_scale=1.0, a_mag=1.0, b_mag=0.05):
     from purejaxql_b200 import _lib
