@@ -286,6 +286,12 @@ int pqn_tc_split16(const float* x, void* hi, void* lo, int64_t n, float scale, v
  *  a_mn=0: A is [S][M][K]; a_mn=1: A is [S][K][M].  b_mn=0: B is [S][N][K]; b_mn=1: B is [S][K][N].  N % 128 == 0. */
 int pqn_tc_gemm16_test(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, float* d, int32_t S,
                        int32_t M, int32_t N, int32_t K, int a_mn, int b_mn, float out_scale, void* stream);
+/* Test hook of the input-gradient epilogues: D[s] = mask[s] * (A[s].B[s]^T) * out_scale on the same path, A [S][M][K]
+ * and B [S][N][K] as planes.  epi 0: no mask; 3: mask[s][m][n] > 0 (mask may equal d); 4: bit n % 32 of
+ * relu_bits[s][m][n / 32].  N % 128 == 0. */
+int pqn_tc_dgrad16_test(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, const float* mask,
+                        const uint32_t* relu_bits, float* d, int32_t S, int32_t M, int32_t N, int32_t K, int epi,
+                        float out_scale, void* stream);
 
 #ifdef __cplusplus
 }

@@ -92,6 +92,8 @@ _SIGS = {
                                  c_int32, c_int, c_int, c_int, c_void_p]),
     "pqn_tc_gemm16_test": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                    c_int32, c_int, c_int, c_float, c_void_p]),
+    "pqn_tc_dgrad16_test": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
+                                    c_int32, c_int32, c_int32, c_int, c_float, c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

@@ -274,12 +274,23 @@ __device__ __forceinline__ void tf32_tile(const uint8_t* smem_al, float* tile_s,
 //     whole K -- their accumulation error is negligible at that magnitude;
 //   * the main A_hi.B_hi chain is cut every TC_PROMOTE k-blocks (16 k-steps): the partial is added to the fp32 tile in
 //     shared memory (round-to-nearest FADD) and the chain restarts with scale-d = 0.
+//
+// ReLU-mask epilogues of the fp16 kernel (the input gradients) finish the tile in registers and store it through TMA
+// (tm_out): the mask words are loaded before the tile's MMAs, each warpgroup writes its 64 rows into a swizzled
+// staging area and one thread issues the bulk store, which runs while the warpgroup goes on to the next tile's MMAs.
+// The two warpgroups do not synchronise with each other.  Rows >= gs.M are clipped by the tensor map.
 // ---------------------------------------------------------------------------
+template <int EPI, bool F16>
+__host__ __device__ constexpr bool tma_store_epilogue() { return F16 && (EPI == EPI_RELU_MASK || EPI == EPI_RELU_BITS); }
+
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(3 + wg) : "memory"); }
+
 template <int A_MN, int B_MN, int EPI, bool F16 = true>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                    const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
-                   const GemmShape gs, const EpiParams ep) {
+                   const __grid_constant__ CUtensorMap tm_out, const GemmShape gs, const EpiParams ep) {
+  constexpr bool TMA_EPI = tma_store_epilogue<EPI, F16>();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte aligned operand ring (swizzle atoms), then the fp32 tile, the epilogue parameters and the barriers
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -293,6 +304,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 
   if (warp == 8 && lane == 0) {
     prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
+    if (TMA_EPI) prefetch_tmap(&tm_out);
     for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TC_CONSUMERS / 32); }
     fence_barrier_init();
   }
@@ -366,12 +378,40 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const uint32_t a_off = wg * 8192;
   // fragment coordinates (see wgmma_f16_m64n128): rows fr, fr + 8; columns 8 j + fc, 8 j + fc + 1
   const int fr = 64 * wg + 16 * ((t & 127) >> 5) + (lane >> 2), fc = 2 * (lane & 3);
+  const int et = t & 127;                    // thread in the warpgroup; et == 0 issues the warpgroup's bulk stores
+  uint8_t* out_stage = reinterpret_cast<uint8_t*>(tile_s) + wg * TC_OUT_STAGE_WG;   // TMA_EPI only
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int seed, m0, n0, kb0, kbn;
     const int ks_idx = decode(tile, seed, m0, n0, kb0, kbn);
-    consumer_bar_sync();   // the previous tile's epilogue is done with tile_s
+    uint32_t rbits[2][4];   // EPI_RELU_BITS: the mask words of rows fr, fr + 8 (bit c of word w = column 32 w + c)
+    if constexpr (TMA_EPI) {
+      // fetch the tile's ReLU mask now, so that its latency hides behind the MMAs
+      if constexpr (EPI == EPI_RELU_BITS) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = m0 + fr + 8 * h;
+          const uint4 w = m < gs.M ? __ldg(reinterpret_cast<const uint4*>(
+                                         ep.relu_bits + ((int64_t)seed * ep.rows + m) * (ep.ld_out >> 5) + (n0 >> 5)))
+                                   : make_uint4(0u, 0u, 0u, 0u);
+          rbits[h][0] = w.x; rbits[h][1] = w.y; rbits[h][2] = w.z; rbits[h][3] = w.w;
+        }
+      } else {   // fp32 mask: 64 KB per tile is too much to hold, so it is pulled into L2 for the epilogue's loads
+        const int m = m0 + 64 * wg + (et >> 1);
+        const float* p = ep.mask + (int64_t)seed * ep.out_seed_stride + (int64_t)m * ep.ld_out + n0 + 64 * (et & 1);
+        if (m < gs.M) {
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(p + 32));
+        }
+      }
+      if (kbn > TC_PROMOTE) {   // the promotions below write tile rows that hold the previous tile's output staging
+        if (et == 0) bulk_wait_read_all();
+        wg_bar_sync(wg);
+      }
+    } else {
+      consumer_bar_sync();   // the previous tile's epilogue is done with tile_s
+    }
     if constexpr (!F16) {
       tf32_tile<A_MN, B_MN>(smem_al, tile_s, full, empty, stage, phase, kbn, gs.split3,
                             ep.out_scale != 0.f ? ep.out_scale : 1.0f, warp, lane);
@@ -399,7 +439,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[stage]);   // smem slot free: this warp's MMAs have retired
       if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
-      if ((kb + 1) % TC_PROMOTE == 0 || kb == kbn - 1) {   // promote the main partial into the fp32 tile
+      // promote the main partial into the fp32 tile (TMA_EPI adds the last partial in registers instead)
+      const bool promote = TMA_EPI ? (kb + 1) % TC_PROMOTE == 0 && kb != kbn - 1
+                                   : (kb + 1) % TC_PROMOTE == 0 || kb == kbn - 1;
+      if (promote) {
         const bool first = kb < TC_PROMOTE;
 #pragma unroll
         for (int j = 0; j < 16; ++j)
@@ -411,6 +454,63 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             else { const float2 o = *p; *p = make_float2(o.x + v.x, o.y + v.y); }
           }
       }
+    }
+    if constexpr (TMA_EPI) {
+      // the same operations as the fp32-tile path below: main (+ promoted partials), + corr * 2^-11, * out_scale;
+      // then the ReLU mask
+      const float osc = ep.out_scale != 0.f ? ep.out_scale : 1.0f;
+      const float* mrow = ep.mask + (int64_t)seed * ep.out_seed_stride + n0;   // EPI_RELU_MASK
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int i = 4 * j + 2 * h;
+          float2 o = make_float2(mainacc[i], mainacc[i + 1]);
+          if (kbn > TC_PROMOTE) {
+            const float2 p = *reinterpret_cast<const float2*>(tile_s + (fr + 8 * h) * TC_ACC_LD + 8 * j + fc);
+            o = make_float2(p.x + o.x, p.y + o.y);
+          }
+          mainacc[i] = fmaf(corr[i], TC_LO_INV, o.x) * osc;
+          mainacc[i + 1] = fmaf(corr[i + 1], TC_LO_INV, o.y) * osc;
+        }
+#pragma unroll
+      for (int j = 0; j < 16; ++j)   // a second pass: the fp32 mask's loads do not compete with corr for registers
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float& x = mainacc[4 * j + 2 * h];
+          float& y = mainacc[4 * j + 2 * h + 1];
+          if constexpr (EPI == EPI_RELU_BITS) {
+            const uint32_t b = rbits[h][j >> 2] >> (8 * (j & 3) + fc);
+            x = (b & 1u) ? x : 0.f; y = (b & 2u) ? y : 0.f;
+          } else {
+            const int m = m0 + fr + 8 * h;
+            if (m < gs.M) {   // rows >= gs.M are not stored
+              const float2 mk = *reinterpret_cast<const float2*>(mrow + (int64_t)m * ep.ld_out + 8 * j + fc);
+              x = mk.x > 0.f ? x : 0.f; y = mk.y > 0.f ? y : 0.f;
+            }
+          }
+        }
+      if (et == 0) bulk_wait_read_all();   // the previous tile's store has read the staging area
+      wg_bar_sync(wg);
+      // staging: box j / 4 holds columns 32 (j / 4) ..; 128-byte rows, 16-byte chunk c of row r at c ^ (r % 8)
+      const int rl = fr - 64 * wg;   // rl % 8 == lane / 4, rows rl and rl + 8
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int chunk = 2 * (j & 3) + (fc >> 2);
+          const int off = (j >> 2) * TC_OUT_BOX_BYTES + (rl + 8 * h) * 128 + ((chunk ^ (lane >> 2)) << 4) + (fc & 3) * 4;
+          *reinterpret_cast<float2*>(out_stage + off) = make_float2(mainacc[4 * j + 2 * h], mainacc[4 * j + 2 * h + 1]);
+        }
+      fence_proxy_async_smem();
+      wg_bar_sync(wg);
+      if (et == 0) {
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+          tma_store_3d(&tm_out, smem_u32(out_stage + b * TC_OUT_BOX_BYTES), n0 + 32 * b, m0 + 64 * wg, seed);
+        bulk_commit();
+      }
+      continue;
     }
     {   // the correction accumulator (units of 2^-11), then the power-of-two output scale (exact)
       const float osc = ep.out_scale != 0.f ? ep.out_scale : 1.0f;
@@ -468,6 +568,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
     }
   }
+  if constexpr (TMA_EPI) {
+    if (et == 0) bulk_wait_all();   // the staging area must outlive the last bulk store's reads
+  }
 }
 
 // ---------------------------------------------------------------------------
@@ -512,11 +615,20 @@ static int launch_t(const CUtensorMap* t, const GemmShape& gs, const EpiParams& 
   static_assert(TC_SMEM_BYTES <= 227 * 1024, "dynamic shared memory of the GEMM kernel exceeds the per-CTA limit");
   if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
     return check_launch("tc_gemm(cudaFuncSetAttribute)");
+  CUtensorMap tm_out = t[0];   // not read unless the epilogue stores through TMA
+  if (tma_store_epilogue<EPI, F16>()) {
+    // out[S][M][ld_out] in boxes of 64 rows x 32 floats; the row bound clips a ragged last m-tile
+    if (ep.ld_out != (int64_t)gs.n_tiles * 128 || gs.k_split > 1)
+      return set_error(PQN_E_INVALID, "tc_gemm16: ReLU-mask epilogues need ld_out == N and no split-K");
+    int rc = make_tmap(&tm_out, ep.out, (uint64_t)ep.ld_out, (uint64_t)gs.M, (uint64_t)gs.S, (uint64_t)ep.ld_out,
+                       (uint64_t)ep.out_seed_stride, 64);
+    if (rc) return rc;
+  }
   const int tiles = gs.m_tiles * gs.n_tiles * gs.S * (gs.k_split > 1 ? gs.k_split : 1);
   const int grid = tiles < num_sms() ? tiles : num_sms();
   {
     LaunchScope _ls(kid < 0 ? (int)K_TC_GEMM : kid, st);
-    kfn<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(t[0], t[1], t[2], t[3], gs, ep);
+    kfn<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(t[0], t[1], t[2], t[3], tm_out, gs, ep);
   }
   return check_launch("tc_gemm");
 }
@@ -642,6 +754,33 @@ int pqn_tc_gemm16_test(const void* a_hi, const void* a_lo, const void* b_hi, con
   EpiParams ep = {};
   ep.out = d; ep.ld_out = N; ep.out_seed_stride = (int64_t)M * N; ep.out_scale = out_scale;
   return launch_gemm16(a_mn, b_mn, EPI_STORE, t, gs, ep, (cudaStream_t)stream);
+}
+
+// Test hook for the input-gradient epilogues: D[s] = mask[s] * (A[s] . B[s]^T) * out_scale on the fp16-split wgmma
+// path, A [S][M][K] and B [S][N][K] as planes (both K-major, the dgrad layout).
+//   epi = 0 (EPI_STORE): no mask;  3 (EPI_RELU_MASK): mask[s][m][n] > 0, mask may equal d (in place);
+//   4 (EPI_RELU_BITS): bit n % 32 of relu_bits[s][m][n / 32].
+// N % 128 == 0; rows of a ragged M are not written.
+int pqn_tc_dgrad16_test(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, const float* mask,
+                        const uint32_t* relu_bits, float* d, int32_t S, int32_t M, int32_t N, int32_t K, int epi,
+                        float out_scale, void* stream) {
+  if (!a_hi || !a_lo || !b_hi || !b_lo || !d || S <= 0 || M <= 0 || N <= 0 || K <= 0 || (N % 128) || (K % 8) ||
+      (M % 8) || !(epi == EPI_STORE || epi == EPI_RELU_MASK || epi == EPI_RELU_BITS) ||
+      (epi == EPI_RELU_MASK && !mask) || (epi == EPI_RELU_BITS && !relu_bits))
+    return set_error(PQN_E_INVALID, "pqn_tc_dgrad16_test: bad argument");
+  CUtensorMap t[4];
+  int rc;
+  const void* p[4] = {a_hi, a_lo, b_hi, b_lo};
+  for (int i = 0; i < 2; ++i) {
+    if ((rc = make_tmap16(&t[i], p[i], K, M, S, K, (uint64_t)M * K, 128))) return rc;
+    if ((rc = make_tmap16(&t[2 + i], p[2 + i], K, N, S, K, (uint64_t)N * K, 128))) return rc;
+  }
+  GemmShape gs = {};
+  gs.S = S; gs.M = M; gs.m_tiles = (M + 127) / 128; gs.n_tiles = N / 128; gs.k_blocks = (K + TC_BK16 - 1) / TC_BK16;
+  EpiParams ep = {};
+  ep.out = d; ep.mask = mask; ep.relu_bits = relu_bits; ep.rows = M;
+  ep.ld_out = N; ep.out_seed_stride = (int64_t)M * N; ep.out_scale = out_scale;
+  return launch_gemm16(0, 0, epi, t, gs, ep, (cudaStream_t)stream);
 }
 
 // Test hook: D[s] = A[s] . B[s] on the TF32 path (fp32 in, fp32 out).  Layout flags as in pqn_tc_gemm16_test.

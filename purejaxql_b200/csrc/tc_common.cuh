@@ -24,6 +24,12 @@ constexpr int TC_ACC_LD = 132;           // floats per row of the fp32 result ti
 constexpr int TC_SP_FLOATS = 384 + 8 * 128 + 8;   // per-seed epilogue parameters (LN scale/bias, Q-head)
 constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 128 * TC_ACC_LD * 4 + TC_SP_FLOATS * 4 + 256 /*barriers*/ +
                               1024 /*align slack*/;
+// TMA-store epilogues: warpgroup wg stages its 64 x 128 fp32 result as four SWIZZLE_128B boxes of [64 rows][32 floats]
+// at byte wg * TC_OUT_STAGE_WG of the fp32 tile region, which lies inside the tile rows that warpgroup owns
+constexpr int TC_OUT_BOX_BYTES = 64 * 32 * 4;     // 8 KB
+constexpr int TC_OUT_STAGE_WG = 34 * 1024;
+static_assert(TC_OUT_STAGE_WG >= 64 * TC_ACC_LD * 4 && TC_OUT_STAGE_WG + 4 * TC_OUT_BOX_BYTES <= 128 * TC_ACC_LD * 4,
+              "each warpgroup's output staging lies within its own 64 rows of the fp32 tile, 1024-byte aligned");
 #define PQN_TC_MAX_A 8
 
 enum Epilogue : int { EPI_STORE = 0, EPI_LN_TRAIN = 1, EPI_LN_HEAD = 2, EPI_RELU_MASK = 3, EPI_RELU_BITS = 4 };
@@ -95,6 +101,19 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// shared -> global tensor store; completion is tracked per issuing thread by bulk async-groups
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory sources of all committed bulk stores have been read (the staging area may be rewritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// all committed bulk stores are complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// makes this thread's generic-proxy shared-memory writes visible to a following TMA (async-proxy) read
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- wgmma
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
