@@ -43,11 +43,12 @@ extern "C" {
 #define PQN_ENV_SEAQUEST 4        /* "Seaquest-MinAtar" */
 #define PQN_ENV_CARTPOLE 16       /* "CartPole-v1" */
 #define PQN_ENV_ACROBOT 17        /* "Acrobot-v1" */
+#define PQN_ENV_MEMORY_CHAIN 32   /* "MemoryChain-bsuite" */
 
 typedef struct pqn_env_info_t {
   int32_t state_words;      /* uint32 words per env in the SoA state block (incl. 5 LogWrapper words) */
-  int32_t obs_dim;          /* flattened observation length (400 for Breakout, 4 CartPole, 6 Acrobot) */
-  int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control */
+  int32_t obs_dim;          /* flattened observation length (400 Breakout, 4 CartPole, 6 Acrobot, 3 MemoryChain) */
+  int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control and bsuite */
   int32_t num_actions;      /* env.action_space(params).n  — pqn_minatar.py:151 */
   int32_t max_steps;        /* env_params.max_steps_in_episode default — pqn_minatar.py:105 */
   int32_t binary_obs;       /* 1: obs are {0,1}; the rollout buffer stores them bit-packed */
@@ -103,9 +104,20 @@ int pqn_env_step(int env_id, const uint32_t* keys, uint32_t* state, const int32_
                  float* reward, uint8_t* done, float* info_discount, float* info_returned_episode_returns,
                  int32_t* info_returned_episode_lengths, int32_t* info_timestep, int64_t N, int max_steps,
                  int rng_mode, void* stream);
+/* env.reset(key, params) with gymnax EnvParams beyond max_steps_in_episode.  pqn_env_reset(.., max_steps, ..) equals
+ * this call with {max_steps, 5}.  max_steps <= 0 selects the env default.  memory_length is MemoryChain-bsuite's
+ * EnvParams.memory_length (gymnax default 5; < 1 is rejected with PQN_E_INVALID); other envs ignore it.
+ * params_host == NULL selects every default.  A parameter other than max_steps is kept in the env's state words, so
+ * pqn_env_step, pqn_env_obs and pqn_rollout_act_step (and their auto-resets) use the value the reset stored. */
+typedef struct pqn_env_params_t {
+  int32_t max_steps;
+  int32_t memory_length;
+} pqn_env_params_t;
+int pqn_env_reset_params(int env_id, const uint32_t* keys, uint32_t* state, float* obs, int64_t N,
+                         const pqn_env_params_t* params_host, int rng_mode, void* stream);
 /* current observation of `state` as packed bits (binary_obs envs): uint32[N][packed_obs_words] */
 int pqn_env_obs_packed(int env_id, const uint32_t* state, uint32_t* obs_packed, int64_t N, void* stream);
-/* current observation of `state` as float32[N][obs_dim] */
+/* current observation of `state` as float32[N][obs_dim]: the one the reset or step that produced `state` returned */
 int pqn_env_obs(int env_id, const uint32_t* state, float* obs, int64_t N, void* stream);
 
 /* ---- epsilon-greedy (eps_greedy_exploration, pqn_minatar.py:115-128,194-196) */

@@ -27,9 +27,20 @@ enum EnvId : int {
   ENV_SEAQUEST = 4,
   ENV_CARTPOLE = 16,
   ENV_ACROBOT = 17,
+  ENV_MEMORY_CHAIN = 32,
 };
 
 constexpr int LOG_WORDS = 5;
+
+// gymnax EnvParams fields other than max_steps_in_episode (pqn_env_params_t of the C ABI).  An env that has such a
+// parameter keeps it in its state words: the reset kernels call env_set_params before reset_env, and reset_env
+// leaves the parameter word alone, so the auto-reset of a step carries it over.  Envs without one ignore them.
+struct EnvParams {
+  int memory_length;
+};
+
+template <class S>
+PQN_HD void env_set_params(S&, const EnvParams&) {}
 
 PQN_HD uint32_t f2u(float f) {
 #if defined(__CUDA_ARCH__)

@@ -208,8 +208,7 @@ class PQNEngine:
         # ---- reset (vmap_reset, :107-109,419)
         reset_keys = jr.split(kR, E_total, mode)[:, env_lo:env_lo + E].reshape(S * E, 2).contiguous()
         state = torch.empty((self.env.state_words, S * E), dtype=torch.int32, device=dev)
-        _lib.check(L.pqn_env_reset(self.env.env_id, _lib.p(reset_keys), _lib.p(state), None, S * E, self.max_steps,
-                                   mode, _lib.stream_ptr()), "pqn_env_reset")
+        envs.reset_into(self.env.env_id, reset_keys, state, None, S * E, self.env_params, mode)
         self._write_obs(state, obs_buf, T, S)                        # update_body moves row T to row 0
         rng = jr.split(K3, 2, mode)[:, 1].contiguous()              # :422-423 runner rng
 
@@ -416,9 +415,8 @@ class PQNEngine:
         k = jr.split(rng, 2, mode)
         kr = k[:, 1].contiguous()                                    # :396 `_rng`
         state = torch.empty((self.env.state_words, S * N), dtype=torch.int32, device=dev)
-        _lib.check(L.pqn_env_reset(self.env.env_id, _lib.p(jr.split(kr, N, mode).reshape(S * N, 2).contiguous()),
-                                   _lib.p(state), None, S * N, self.max_steps, mode, _lib.stream_ptr()),
-                   "pqn_env_reset")
+        envs.reset_into(self.env.env_id, jr.split(kr, N, mode).reshape(S * N, 2).contiguous(), state, None, S * N,
+                        self.env_params, mode)
         obs = torch.zeros((S, 2, N, W), dtype=self.obs_dtype, device=dev)   # ping-pong rows
         self._write_obs(state, obs, 0, S)
         q = torch.zeros((S * N, A), dtype=torch.float32, device=dev)

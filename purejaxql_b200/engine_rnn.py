@@ -21,7 +21,7 @@ from .networks import NET_RNN, QNetworkSpec
 
 
 class PQNRnnEngine:
-    def __init__(self, config: dict, device=None):
+    def __init__(self, config: dict, device=None, env_params: envs.EnvParams | None = None):
         self.cfg = c = config
         self.device = torch.device(device or "cuda")
         if self.device.type != "cuda" or not torch.cuda.is_available():
@@ -32,8 +32,11 @@ class PQNRnnEngine:
                                       "(the shipped pqn_rnn_cartpole.yaml)")
         self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
         self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=True, rng_mode=self.rng_mode)
+        if env_params is not None:                                   # e.g. MemoryChain's memory_length (:134-136)
+            self.env_params = env_params
         if self.env.binary_obs:
-            raise NotImplementedError("the recurrent script is built for the classic-control envs")
+            raise NotImplementedError("the recurrent script is built for the float-observation envs "
+                                      "(classic control, MemoryChain-bsuite)")
         self.max_steps = int(self.env_params.max_steps_in_episode)
         self.T, self.E, self.NU = int(c["NUM_STEPS"]), int(c["NUM_ENVS"]), int(c["NUM_UPDATES"])
         self.W = int(c["MEMORY_WINDOW"])
@@ -73,9 +76,8 @@ class PQNRnnEngine:
         dev, mode = self.device, self.rng_mode
         state = torch.empty((self.env.state_words, S * N), dtype=torch.int32, device=dev)
         obs = torch.empty((S, N, self.D), dtype=torch.float32, device=dev)
-        _lib.check(_lib.lib().pqn_env_reset(self.env.env_id, _lib.p(jr.split(key, N, mode).reshape(S * N, 2).contiguous()),
-                                            _lib.p(state), _lib.p(obs), S * N, self.max_steps, mode, _lib.stream_ptr()),
-                   "pqn_env_reset")
+        envs.reset_into(self.env.env_id, jr.split(key, N, mode).reshape(S * N, 2).contiguous(), state, obs, S * N,
+                        self.env_params, mode)
         return obs, state
 
     # ------------------------------------------------------------------ #

@@ -31,6 +31,7 @@ ENV_IDS = {
     "Freeway-MinAtar": 3,
     "CartPole-v1": 16,
     "Acrobot-v1": 17,
+    "MemoryChain-bsuite": 32,
 }
 # PQN_ENV_SEAQUEST (4) is reserved in include/pqn_b200.h but not built: gymnax 0.0.6 (the reference's pin) does not
 # register "Seaquest-MinAtar" in gymnax.make either (DESIGN.md section 8), so the reference cannot run it.
@@ -43,6 +44,11 @@ LOG_FIELDS = ("episode_returns", "episode_lengths", "returned_episode_returns",
 @dataclass
 class EnvParams:
     max_steps_in_episode: int
+    memory_length: int = 5          # MemoryChain-bsuite's EnvParams.memory_length (gymnax default); other envs ignore it
+
+    def as_c(self) -> _lib.EnvParams:
+        """The ``pqn_env_params_t`` of ``pqn_env_reset_params``."""
+        return _lib.EnvParams(int(self.max_steps_in_episode), int(self.memory_length))
 
 
 def _u2f(t):
@@ -137,6 +143,11 @@ def state_to_fields(env_name: str, state: torch.Tensor) -> dict:
             f[k] = _u2f(st[j])
         f["time"] = st[4]
         core = 5
+    elif env_name == "MemoryChain-bsuite":
+        f["context"] = (st[0] != 0).unsqueeze(1)                           # [N, num_bits = 1]
+        for j, k in enumerate(("query", "total_perfect", "total_regret", "time", "memory_length"), 1):
+            f[k] = st[j]                                                    # memory_length: the EnvParams word
+        core = 6
     else:
         raise KeyError(env_name)
     f["log_episode_returns"] = _u2f(st[core + 0])
@@ -207,6 +218,10 @@ def fields_to_state(env_name: str, f: dict) -> torch.Tensor:
     elif env_name == "Acrobot-v1":
         core = [_f2u(torch.as_tensor(f[k])) for k in
                 ("joint_angle1", "joint_angle2", "velocity_1", "velocity_2")] + [i32(f["time"])]
+    elif env_name == "MemoryChain-bsuite":
+        ctx = i32(f["context"])
+        core = [ctx.reshape(ctx.shape[0], -1)[:, 0]] + [i32(f[k]) for k in
+                                                         ("query", "total_perfect", "total_regret", "time", "memory_length")]
     else:
         raise KeyError(env_name)
     log = [_f2u(torch.as_tensor(f["log_episode_returns"])), i32(f["log_episode_lengths"]),
@@ -229,6 +244,14 @@ def pack_observation(obs: torch.Tensor) -> torch.Tensor:
     words = (padded.view(n, pw, 32) << sh).sum(-1)
     words = torch.where(words >= 2 ** 31, words - 2 ** 32, words)
     return words.to(torch.int32).contiguous()
+
+
+def reset_into(env_id: int, keys: torch.Tensor, state: torch.Tensor, obs: torch.Tensor | None, n: int,
+               params: EnvParams, rng_mode: int):
+    """``pqn_env_reset_params``: reset n envs into ``state`` (and ``obs`` unless None) with ``params``.  Parameters
+    other than max_steps stay in the state block, so steps and auto-resets need nothing more."""
+    _lib.check(_lib.lib().pqn_env_reset_params(env_id, _lib.p(keys), _lib.p(state), _lib.p(obs), n, params.as_c(),
+                                               rng_mode, _lib.stream_ptr()), "pqn_env_reset_params")
 
 
 # --------------------------------------------------------------------------- #
@@ -269,9 +292,7 @@ class BatchedEnv:
         n = keys.shape[0]
         state = torch.empty((self.state_words, n), dtype=torch.int32, device=keys.device)
         obs = torch.empty((n,) + self._obs_shape, dtype=torch.float32, device=keys.device)
-        _lib.check(_lib.lib().pqn_env_reset(self.env_id, _lib.p(keys), _lib.p(state), _lib.p(obs), n,
-                                            params.max_steps_in_episode, self.rng_mode, _lib.stream_ptr()),
-                   "pqn_env_reset")
+        reset_into(self.env_id, keys, state, obs, n, params, self.rng_mode)
         return obs, state
 
     def step(self, keys: torch.Tensor, state: torch.Tensor, action: torch.Tensor,

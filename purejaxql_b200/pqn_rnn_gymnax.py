@@ -1,6 +1,7 @@
-"""Recurrent (GRU) PQN on gymnax classic control — drop-in for purejaxql/pqn_rnn_gymnax.py.
+"""Recurrent (GRU) PQN on gymnax classic control and MemoryChain-bsuite — drop-in for purejaxql/pqn_rnn_gymnax.py.
 
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole NUM_SEEDS=4
+    python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_memory_chain
 
 ``make_train(config)`` keeps the reference's contract (pqn_rnn_gymnax.py:117-560): config mutation (NUM_UPDATES,
 NUM_UPDATES_DECAY, TEST_NUM_STEPS), ``RNNQNetwork`` (MLP trunk -> one-hot last action -> scanned GRU with done-resets ->
@@ -16,11 +17,17 @@ from .engine_rnn import PQNRnnEngine
 
 
 def make_train(config):
-    if config["ENV_NAME"] == "MemoryChain-bsuite":
-        raise NotImplementedError("MemoryChain-bsuite is not built (CartPole-v1 / Acrobot-v1 are)")
     env, env_params = envs.make(config["ENV_NAME"], flatten_obs=True)      # :134-139
+    if config["ENV_NAME"] == "MemoryChain-bsuite":
+        # :134-136 -- EnvParams(memory_length=ENV_KWARGS.get("memory_length", 10)): the script's default is 10, not
+        # gymnax's 5; max_steps_in_episode keeps its default (1000), which is also TEST_NUM_STEPS's
+        memory_length = (config.get("ENV_KWARGS") or {}).get("memory_length", 10)
+        if isinstance(memory_length, bool) or not isinstance(memory_length, int) or memory_length < 1:
+            raise ValueError(f"MemoryChain-bsuite needs ENV_KWARGS.memory_length to be a positive int, "
+                             f"got {memory_length!r}")
+        env_params = envs.EnvParams(env_params.max_steps_in_episode, memory_length=memory_length)
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=True)    # :119-132,140
-    engine = PQNRnnEngine(config)
+    engine = PQNRnnEngine(config, env_params=env_params)
 
     def train(rngs):
         return engine.train(rngs)
