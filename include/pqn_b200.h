@@ -173,13 +173,15 @@ int pqn_qlambda(const float* reward, const uint8_t* done, const float* maxq, con
 typedef struct pqn_net_desc_t {
   int32_t kind;        /* PQN_NET_* */
   int32_t in_c;        /* CNN: input channels C (obs 10x10xC)   | MLP: input dim D */
-  int32_t hidden;      /* CNN: 128 (fixed)                      | MLP: HIDDEN_SIZE */
-  int32_t layers;      /* CNN: ignored                          | MLP: NUM_LAYERS (1 or 2) */
+  int32_t hidden;      /* CNN: 128 (fixed)                      | MLP: HIDDEN_SIZE (64, 128, 256 or 512) */
+  int32_t layers;      /* CNN: ignored                          | MLP: NUM_LAYERS (1 .. PQN_MAX_LAYERS) */
   int32_t num_actions; /* A */
   int32_t norm_type;   /* NORM_TYPE: 0 layer_norm (default), 1 batch_norm, 2 none   (pqn_minatar.py:31-36) */
   int32_t norm_input;  /* NORM_INPUT: 1 = the input BatchNorm normalises the observation (replaces x/255 in the CNN)
                           and is trained; 0 = it is the dummy of pqn_minatar.py:61-66 */
 } pqn_net_desc_t;
+/* the MLP and GRU networks are built for 1 <= NUM_LAYERS <= PQN_MAX_LAYERS */
+#define PQN_MAX_LAYERS 8
 #define PQN_NORM_LAYER 0
 #define PQN_NORM_BATCH 1
 #define PQN_NORM_NONE 2
@@ -192,8 +194,8 @@ typedef struct pqn_net_layout_t {
   int64_t conv_w, conv_b;        /* CNN_0/Conv_0 kernel [3,3,C,16] HWIO, bias [16] */
   int64_t ln0_scale, ln0_bias;   /* CNN: CNN_0/LayerNorm_0 [16] | MLP: LayerNorm_0 [H] */
   int64_t d0_w, d0_b;            /* CNN: CNN_0/Dense_0 [1024,128]/[128] | MLP: Dense_0 [D,H]/[H] */
-  int64_t ln1_scale, ln1_bias;   /* CNN: CNN_0/LayerNorm_1 [128] | MLP: LayerNorm_1 [H] (layers==2) */
-  int64_t d1_w, d1_b;            /* MLP only: Dense_1 [H,H]/[H] (layers==2) */
+  int64_t ln1_scale, ln1_bias;   /* CNN: CNN_0/LayerNorm_1 [128] | MLP: LayerNorm_1 [H] (layers >= 2) */
+  int64_t d1_w, d1_b;            /* MLP only: Dense_1 [H,H]/[H] (layers >= 2); layers 2.. follow: pqn_net_dense_layer */
   int64_t head_w, head_b;        /* final Dense [H,A]/[A] */
   /* PQN_NET_RNN only (-1 otherwise): ScannedRNN_0/GRUCell_0/{ir,iz,in} kernel [H+A,H] + bias [H], {hr,hz} kernel [H,H],
    * hn kernel [H,H] + bias [H] */
@@ -201,6 +203,11 @@ typedef struct pqn_net_layout_t {
 } pqn_net_layout_t;
 
 int pqn_net_layout(const pqn_net_desc_t* desc_host, pqn_net_layout_t* out_host);
+/* offsets_host[4] = (Dense_l kernel [in,H], Dense_l bias [H], norm scale [H], norm bias [H]) of hidden layer
+ * 0 <= layer < NUM_LAYERS of an MLP / GRU network, -1 where there is none (norm_type none).  The norm is LayerNorm_l,
+ * or BatchNorm_{l+1} in the MLP.  Layers 0 and 1 equal the d0_* / ln0_* and d1_* / ln1_* fields of pqn_net_layout;
+ * layers >= 2 follow layer 1's norm, before the GRU block and the head. */
+int pqn_net_dense_layer(const pqn_net_desc_t* desc_host, int32_t layer, int64_t* offsets_host);
 /* floats per seed of the batch_stats block (flax "batch_stats" collection): [mean in][var in] of the input BatchNorm,
  * then, for norm_type == batch_norm, (mean[n], var[n]) of every hidden BatchNorm in network order (CNN: 16, 128;
  * MLP: hidden x layers).  With norm_type none the ln*_scale / ln*_bias layout entries are -1 (no such parameters). */

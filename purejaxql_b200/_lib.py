@@ -73,6 +73,7 @@ _SIGS = {
     "pqn_qlambda": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
                             c_float, c_float, c_void_p]),
     "pqn_net_layout": (c_int, [POINTER(NetDesc), POINTER(NetLayout)]),
+    "pqn_net_dense_layer": (c_int, [POINTER(NetDesc), c_int32, POINTER(c_int64)]),
     "pqn_net_stats_floats": (c_int64, [POINTER(NetDesc)]),
     "pqn_net_workspace_bytes": (c_int64, [POINTER(NetDesc), c_int32, c_int64]),
     "pqn_net_init": (c_int, [POINTER(NetDesc), c_void_p, c_void_p, c_int32, c_void_p]),

@@ -34,7 +34,7 @@ static int g_use_tc = 2;  // 0 FFMA, 1 3xTF32 on mma.sync (A_lo derived in the k
 static int g_conv_mma = 1;   // 0: fp32 CUDA cores, 1: fp16 mma.sync forward (default), 3: tf32 mma.sync forward
                              // (1, 3: mma.sync backward)
 
-static inline int64_t align4(int64_t x) { return (x + 3) & ~(int64_t)3; }
+__host__ __device__ static inline int64_t align4(int64_t x) { return (x + 3) & ~(int64_t)3; }
 
 static int make_layout(const pqn_net_desc_t* d, pqn_net_layout_t* L) {
   int64_t off = 0;
@@ -59,9 +59,11 @@ static int make_layout(const pqn_net_desc_t* d, pqn_net_layout_t* L) {
     L->d0_w = take((int64_t)D * H); L->d0_b = take(H);
     L->ln0_scale = L->ln0_bias = -1;
     if (has_norm) { L->ln0_scale = take(H); L->ln0_bias = take(H); }
-    if (d->layers == 2) {
-      L->d1_w = take((int64_t)H * H); L->d1_b = take(H);
-      if (has_norm) { L->ln1_scale = take(H); L->ln1_bias = take(H); }
+    // layers >= 2 follow layer 1 in the same pattern; dense_off restates this order for any layer (keep the two in step)
+    for (int l = 1; l < d->layers; ++l) {
+      const int64_t w = take((int64_t)H * H), b = take(H);
+      const int64_t sc = has_norm ? take(H) : -1, bi = has_norm ? take(H) : -1;
+      if (l == 1) { L->d1_w = w; L->d1_b = b; L->ln1_scale = sc; L->ln1_bias = bi; }
     }
     if (d->kind == PQN_NET_RNN) {   // flax GRUCell: input denses with bias, recurrent ones without (except hn)
       L->gru_ir_w = take((int64_t)(H + A) * H); L->gru_ir_b = take(H);
@@ -78,11 +80,31 @@ static int make_layout(const pqn_net_desc_t* d, pqn_net_layout_t* L) {
   return 0;
 }
 
+// Offsets of hidden layer l (Dense_l kernel / bias, its norm's scale / bias; -1 where there is none) of an MLP / GRU
+// layout: layers 0 and 1 are the d0/ln0 and d1/ln1 fields, layers >= 2 follow layer 1's norm with the same stride.
+struct DenseOff { int64_t w, b, g, bi; };
+__host__ __device__ inline DenseOff dense_off(const pqn_net_layout_t& L, int H, int l) {
+  if (l == 0) return DenseOff{L.d0_w, L.d0_b, L.ln0_scale, L.ln0_bias};
+  if (l == 1) return DenseOff{L.d1_w, L.d1_b, L.ln1_scale, L.ln1_bias};
+  const bool norm = L.ln1_scale >= 0;
+  const int64_t stride = align4((int64_t)H * H) + (norm ? 3 : 1) * align4(H);
+  const int64_t w = (norm ? L.ln1_bias : L.d1_b) + align4(H) + (l - 2) * stride;
+  const int64_t b = w + align4((int64_t)H * H);
+  return DenseOff{w, b, norm ? b + align4(H) : -1, norm ? b + 2 * align4(H) : -1};
+}
+
 static int check_desc(const pqn_net_desc_t* d, const char* who) {
   if (!d) return set_error(PQN_E_INVALID, "%s: desc is NULL", who);
   if (d->num_actions < 1 || d->num_actions > 32) return set_error(PQN_E_INVALID, "%s: num_actions=%d out of [1,32]", who, d->num_actions);
   if (d->norm_type < 0 || d->norm_type > 2 || d->norm_input < 0 || d->norm_input > 1)
     return set_error(PQN_E_INVALID, "%s: norm_type=%d norm_input=%d", who, d->norm_type, d->norm_input);
+  if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN) {
+    const int H = d->hidden;
+    if (H != 64 && H != 128 && H != 256 && H != 512)
+      return set_error(PQN_E_UNSUPPORTED, "%s: hidden=%d (64, 128, 256 or 512 built)", who, H);
+    if (d->layers < 1 || d->layers > PQN_MAX_LAYERS)
+      return set_error(PQN_E_UNSUPPORTED, "%s: layers=%d (1 to %d built)", who, d->layers, PQN_MAX_LAYERS);
+  }
   {
     // row_bwd_kernel keeps [A][N] head weights + eight warp-private [A][N] gradient slices in shared memory
     const int Nh = d->kind == PQN_NET_MINATAR_CNN ? 128 : d->hidden;
@@ -97,8 +119,6 @@ static int check_desc(const pqn_net_desc_t* d, const char* who) {
     return PQN_OK;
   }
   if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN) {
-    if (d->hidden != 128 && d->hidden != 256) return set_error(PQN_E_UNSUPPORTED, "%s: MLP hidden=%d (128 or 256 built)", who, d->hidden);
-    if (d->layers != 1 && d->layers != 2) return set_error(PQN_E_UNSUPPORTED, "%s: MLP layers=%d (1 or 2 built)", who, d->layers);
     if (d->in_c < 1 || d->in_c > 4096) return set_error(PQN_E_INVALID, "%s: MLP in dim %d", who, d->in_c);
     return PQN_OK;
   }
@@ -150,7 +170,7 @@ __device__ __forceinline__ float4 load4_guard(const float* __restrict__ src, int
 //   MODE 1: write H, XHAT, RSTD  (training forward: what the backward needs)
 //   MODE 2: write Q = H @ Wh + bh only (inference last layer, Q-head fused)
 //   MODE 3: write the raw pre-activation X @ W + b to H (no LayerNorm; modular NORM_TYPE path)
-// grid = (ceil(rows/BM), S)
+// grid = (ceil(rows/BM), S, column tiles); more than one column tile (rows of gridDim.z * BN outputs) for MODE 3 only
 // ---------------------------------------------------------------------------
 template <int BN, int MODE>
 __global__ void __launch_bounds__(GT) dense_fwd_kernel(
@@ -166,9 +186,10 @@ __global__ void __launch_bounds__(GT) dense_fwd_kernel(
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int seed = blockIdx.y;
   const int m0 = blockIdx.x * BM;
+  const int n0 = blockIdx.z * BN, ldn = gridDim.z * BN;   // this CTA's output columns, row stride of W and H
   const float* __restrict__ Xs = X + (int64_t)seed * x_seed_stride;
   const float* __restrict__ prm = params + (int64_t)seed * P;
-  const float* __restrict__ W = prm + off_w;
+  const float* __restrict__ W = prm + off_w + n0;
   const bool vecA = (ldx % 4 == 0) && ((reinterpret_cast<uintptr_t>(Xs) & 15) == 0);
 
   float acc[TM][TN];
@@ -193,7 +214,7 @@ __global__ void __launch_bounds__(GT) dense_fwd_kernel(
       const int f = tid + i * GT;
       const int r = f / (BN / 4), n4 = f % (BN / 4);
       const int k = kt * BK + r;
-      rb[i] = (k < K) ? __ldg(reinterpret_cast<const float4*>(W + (int64_t)k * BN + n4 * 4))
+      rb[i] = (k < K) ? __ldg(reinterpret_cast<const float4*>(W + (int64_t)k * ldn + n4 * 4))
                       : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   };
@@ -224,7 +245,7 @@ __global__ void __launch_bounds__(GT) dense_fwd_kernel(
   }
 
   // ---- epilogue: bias, LayerNorm over the BN columns of each row, ReLU
-  const float* __restrict__ bvec = prm + (off_b >= 0 ? off_b : 0);
+  const float* __restrict__ bvec = prm + (off_b >= 0 ? off_b + n0 : 0);
   const float* __restrict__ sc = prm + off_scale;
   const float* __restrict__ bi = prm + off_bias;
   float colb[TN], cols_[TN], colbi[TN];
@@ -241,7 +262,7 @@ __global__ void __launch_bounds__(GT) dense_fwd_kernel(
         const int64_t grow3 = (int64_t)seed * rows + row;
 #pragma unroll
         for (int c = 0; c < TN / 4; ++c)
-          *reinterpret_cast<float4*>(H + grow3 * BN + c * 64 + tx * 4) =
+          *reinterpret_cast<float4*>(H + grow3 * ldn + n0 + c * 64 + tx * 4) =
               make_float4(acc[i][4 * c] + colb[4 * c], acc[i][4 * c + 1] + colb[4 * c + 1], acc[i][4 * c + 2] + colb[4 * c + 2],
                           acc[i][4 * c + 3] + colb[4 * c + 3]);
       }
@@ -302,13 +323,15 @@ __global__ void __launch_bounds__(GT) dense_fwd_kernel(
 
 // ---------------------------------------------------------------------------
 // wgrad: dW[kin][n] (+)= sum_rows X[row][kin] * dZ[row][n]
-// grid = (ceil(Kin/128), N/128, S*splits); splits > 1 writes per-split partials (launch through run_wgrad_ffma)
+// grid = (ceil(Kin/128), N/BN, S*splits); splits > 1 writes per-split partials (launch through run_wgrad_ffma).
+// BN = 128, or 64 for a 64-wide layer (HIDDEN_SIZE 64)
 // ---------------------------------------------------------------------------
+template <int BN>
 __global__ void __launch_bounds__(GT) wgrad_kernel(const float* __restrict__ X, int64_t x_seed_stride, int ldx,
                                                    const float* __restrict__ DZ, int64_t dz_seed_stride, int N,
                                                    float* __restrict__ grads, int64_t P, int64_t off_w, int rows,
                                                    int Kin, int splits, float* __restrict__ part) {
-  constexpr int BM = 128, BN = 128, TM = 8, TN = 8;
+  constexpr int BM = 128, TM = 8, TN = BN / 16, B_LD = BN / 64;
   __shared__ __align__(16) float As[2][BK * BM];
   __shared__ __align__(16) float Bs[2][BK * BN];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -329,7 +352,7 @@ __global__ void __launch_bounds__(GT) wgrad_kernel(const float* __restrict__ X, 
     for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
 
   const int nk = (r_end > r_begin) ? (r_end - r_begin + BK - 1) / BK : 0;
-  float4 ra[2], rb[2];
+  float4 ra[2], rb[B_LD];
   auto gload = [&](int kt) {
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -338,7 +361,13 @@ __global__ void __launch_bounds__(GT) wgrad_kernel(const float* __restrict__ X, 
       const int row = r_begin + kt * BK + r;
       const int kin = m0 + m4 * 4;
       ra[i] = load4_guard(Xs + (int64_t)row * ldx + kin, kin, Kin, vecA, row < r_end);
-      rb[i] = (row < r_end) ? __ldg(reinterpret_cast<const float4*>(Zs + (int64_t)row * N + n0 + m4 * 4))
+    }
+#pragma unroll
+    for (int i = 0; i < B_LD; ++i) {
+      const int f = tid + i * GT;
+      const int r = f / (BN / 4), n4 = f % (BN / 4);
+      const int row = r_begin + kt * BK + r;
+      rb[i] = (row < r_end) ? __ldg(reinterpret_cast<const float4*>(Zs + (int64_t)row * N + n0 + n4 * 4))
                             : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   };
@@ -348,7 +377,12 @@ __global__ void __launch_bounds__(GT) wgrad_kernel(const float* __restrict__ X, 
       const int f = tid + i * GT;
       const int r = f >> 5, m4 = f & 31;
       *reinterpret_cast<float4*>(&As[buf][r * BM + m4 * 4]) = ra[i];
-      *reinterpret_cast<float4*>(&Bs[buf][r * BN + m4 * 4]) = rb[i];
+    }
+#pragma unroll
+    for (int i = 0; i < B_LD; ++i) {
+      const int f = tid + i * GT;
+      const int r = f / (BN / 4), n4 = f % (BN / 4);
+      *reinterpret_cast<float4*>(&Bs[buf][r * BN + n4 * 4]) = rb[i];
     }
   };
   if (nk > 0) {
@@ -381,13 +415,14 @@ __global__ void __launch_bounds__(GT) wgrad_kernel(const float* __restrict__ X, 
 // ---------------------------------------------------------------------------
 // dgrad: OUT[row][c] = (HPREV[row][c] > 0) * sum_n dZ[row][n] * W[c][n]
 // (ReLU mask of the previous layer fused; OUT may alias HPREV)
-// grid = (ceil(rows/128), Kprev/128, S)
+// grid = (ceil(rows/128), Kprev/BN, S); BN = 128, or 64 for a 64-wide layer (launch through launch_dgrad)
 // ---------------------------------------------------------------------------
+template <int BN>
 __global__ void __launch_bounds__(GT) dgrad_kernel(const float* __restrict__ DZ, int64_t dz_seed_stride, int N,
                                                    const float* __restrict__ params, int64_t P, int64_t off_w,
                                                    const float* HPREV, float* OUT, int64_t h_seed_stride, int rows,
-                                                   int Kprev, int accumulate = 0) {
-  constexpr int BM = 128, BN = 128, TM = 8, TN = 8;
+                                                   int Kprev, int accumulate) {
+  constexpr int BM = 128, TM = 8, TN = BN / 16, B_LD = BN / 64;
   __shared__ __align__(16) float As[2][BK * BM];
   __shared__ __align__(16) float Bs[2][BK * BN];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -402,7 +437,7 @@ __global__ void __launch_bounds__(GT) dgrad_kernel(const float* __restrict__ DZ,
 #pragma unroll
     for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
   const int nk = N / BK;
-  float4 ra[2], rb[2];
+  float4 ra[2], rb[B_LD];
   auto gload = [&](int kt) {
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -412,7 +447,7 @@ __global__ void __launch_bounds__(GT) dgrad_kernel(const float* __restrict__ DZ,
       const int row = m0 + m;
       ra[i] = (row < rows) ? __ldg(reinterpret_cast<const float4*>(Zs + (int64_t)row * N + n))
                            : make_float4(0.f, 0.f, 0.f, 0.f);
-      rb[i] = __ldg(reinterpret_cast<const float4*>(W + (int64_t)(c0 + m) * N + n));
+      if (i < B_LD) rb[i] = __ldg(reinterpret_cast<const float4*>(W + (int64_t)(c0 + m) * N + n));
     }
   };
   auto sstore = [&](int buf) {
@@ -422,8 +457,10 @@ __global__ void __launch_bounds__(GT) dgrad_kernel(const float* __restrict__ DZ,
       const int m = f >> 2, r4 = f & 3;
       float* da = &As[buf][(r4 * 4) * BM + m];
       da[0] = ra[i].x; da[BM] = ra[i].y; da[2 * BM] = ra[i].z; da[3 * BM] = ra[i].w;
-      float* db = &Bs[buf][(r4 * 4) * BN + m];
-      db[0] = rb[i].x; db[BN] = rb[i].y; db[2 * BN] = rb[i].z; db[3 * BN] = rb[i].w;
+      if (i < B_LD) {
+        float* db = &Bs[buf][(r4 * 4) * BN + m];
+        db[0] = rb[i].x; db[BN] = rb[i].y; db[2 * BN] = rb[i].z; db[3 * BN] = rb[i].w;
+      }
     }
   };
   gload(0);
@@ -467,6 +504,23 @@ __global__ void __launch_bounds__(GT) dgrad_kernel(const float* __restrict__ DZ,
 // grid = (ceil(rows/ROWS_PER_CTA), S)
 // ---------------------------------------------------------------------------
 
+// V consecutive features of a lane (V = 4: float4, V = 2: float2)
+template <int V>
+__device__ __forceinline__ void ld_feat(const float* p, float* o) {
+  if constexpr (V == 4) {
+    const float4 v = *reinterpret_cast<const float4*>(p);
+    o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
+  } else {
+    const float2 v = *reinterpret_cast<const float2*>(p);
+    o[0] = v.x; o[1] = v.y;
+  }
+}
+template <int V>
+__device__ __forceinline__ void st_feat(float* p, const float* o) {
+  if constexpr (V == 4) *reinterpret_cast<float4*>(p) = make_float4(o[0], o[1], o[2], o[3]);
+  else *reinterpret_cast<float2*>(p) = make_float2(o[0], o[1]);
+}
+
 template <int N, bool HEAD>
 __global__ void __launch_bounds__(256) row_bwd_kernel(
     const float* __restrict__ Hh, const float* __restrict__ XHAT, const float* __restrict__ RSTD,
@@ -478,7 +532,8 @@ __global__ void __launch_bounds__(256) row_bwd_kernel(
   // Reductions over rows are deterministic: lane-private registers -> warp-private shared-memory slices -> a fixed-order
   // sum over the 8 warps -> this CTA's partial vector part[seed][cta][3N (+ A*N + A + 2)], which row_bwd_final_kernel
   // adds over the CTAs in index order (no float atomics anywhere).
-  constexpr int F = N / 32;  // features per lane, in float4 chunks at lane*4 + c*128
+  constexpr int F = N / 32;  // features per lane, in chunks of V at lane*V + c*32*V
+  constexpr int V = N >= 128 ? 4 : 2, CW = 32 * V;
   extern __shared__ float smem[];
   float* s_red3 = smem;           // [8 warps][3N]  d scale, d bias, d dense-bias slices
   float* s_hw = smem + 24 * N;    // [A][N]  head weights, transposed copy (HEAD)
@@ -497,7 +552,7 @@ __global__ void __launch_bounds__(256) row_bwd_kernel(
   __syncthreads();
   float scale[F];
 #pragma unroll
-  for (int j = 0; j < F; ++j) scale[j] = __ldg(prm + off_scale + (j >> 2) * 128 + lane * 4 + (j & 3));
+  for (int j = 0; j < F; ++j) scale[j] = __ldg(prm + off_scale + (j / V) * CW + lane * V + (j % V));
   float a_dsc[F], a_dbi[F], a_db[F];
 #pragma unroll
   for (int j = 0; j < F; ++j) a_dsc[j] = a_dbi[j] = a_db[j] = 0.f;
@@ -510,17 +565,11 @@ __global__ void __launch_bounds__(256) row_bwd_kernel(
     const int64_t grow = (int64_t)seed * rows + row;
     float h[F], xh[F], dy[F];
 #pragma unroll
-    for (int c = 0; c < F / 4; ++c) {
-      const float4 v = *reinterpret_cast<const float4*>(XHAT + grow * N + c * 128 + lane * 4);
-      xh[4 * c] = v.x; xh[4 * c + 1] = v.y; xh[4 * c + 2] = v.z; xh[4 * c + 3] = v.w;
-    }
+    for (int c = 0; c < F / V; ++c) ld_feat<V>(XHAT + grow * N + c * CW + lane * V, xh + V * c);
     const float rstd = RSTD[grow];
     if (HEAD) {
 #pragma unroll
-      for (int c = 0; c < F / 4; ++c) {
-        const float4 v = *reinterpret_cast<const float4*>(Hh + grow * N + c * 128 + lane * 4);
-        h[4 * c] = v.x; h[4 * c + 1] = v.y; h[4 * c + 2] = v.z; h[4 * c + 3] = v.w;
-      }
+      for (int c = 0; c < F / V; ++c) ld_feat<V>(Hh + grow * N + c * CW + lane * V, h + V * c);
       const int src = gather ? gather[(int64_t)seed * rows + row] : row;
       const int act = action[(int64_t)seed * tr_rows_per_seed + src];
       const float tgt = target[(int64_t)seed * tr_rows_per_seed + src];
@@ -528,10 +577,7 @@ __global__ void __launch_bounds__(256) row_bwd_kernel(
       float pq = 0.f;
       float wcol[F];
 #pragma unroll
-      for (int c = 0; c < F / 4; ++c) {
-        const float4 v = *reinterpret_cast<const float4*>(s_hw + act * N + c * 128 + lane * 4);
-        wcol[4 * c] = v.x; wcol[4 * c + 1] = v.y; wcol[4 * c + 2] = v.z; wcol[4 * c + 3] = v.w;
-      }
+      for (int c = 0; c < F / V; ++c) ld_feat<V>(s_hw + act * N + c * CW + lane * V, wcol + V * c);
 #pragma unroll
       for (int j = 0; j < F; ++j) pq = fmaf(h[j], wcol[j], pq);
 #pragma unroll
@@ -545,21 +591,19 @@ __global__ void __launch_bounds__(256) row_bwd_kernel(
         s_dhb[warp * A + act] += dq;   // warp-private slot, one writer
       }
 #pragma unroll
-      for (int c = 0; c < F / 4; ++c) {  // warp-private slice: plain read-modify-write, no atomics
-        float4* dst = reinterpret_cast<float4*>(my_dhw + act * N + c * 128 + lane * 4);
-        float4 v = *dst;
-        v.x = fmaf(h[4 * c], dq, v.x); v.y = fmaf(h[4 * c + 1], dq, v.y);
-        v.z = fmaf(h[4 * c + 2], dq, v.z); v.w = fmaf(h[4 * c + 3], dq, v.w);
-        *dst = v;
+      for (int c = 0; c < F / V; ++c) {  // warp-private slice: plain read-modify-write, no atomics
+        float* dst = my_dhw + act * N + c * CW + lane * V;
+        float v[V];
+        ld_feat<V>(dst, v);
+#pragma unroll
+        for (int k = 0; k < V; ++k) v[k] = fmaf(h[V * c + k], dq, v[k]);
+        st_feat<V>(dst, v);
       }
 #pragma unroll
       for (int j = 0; j < F; ++j) dy[j] = h[j] > 0.f ? dq * wcol[j] : 0.f;
     } else {
 #pragma unroll
-      for (int c = 0; c < F / 4; ++c) {
-        const float4 v = *reinterpret_cast<const float4*>(DH + grow * N + c * 128 + lane * 4);
-        dy[4 * c] = v.x; dy[4 * c + 1] = v.y; dy[4 * c + 2] = v.z; dy[4 * c + 3] = v.w;
-      }
+      for (int c = 0; c < F / V; ++c) ld_feat<V>(DH + grow * N + c * CW + lane * V, dy + V * c);
     }
     float m1 = 0.f, m2 = 0.f;
     float dxh[F];
@@ -585,30 +629,37 @@ __global__ void __launch_bounds__(256) row_bwd_kernel(
       a_db[j] += dz[j];
     }
 #pragma unroll
-    for (int c = 0; c < F / 4; ++c)
+    for (int c = 0; c < F / V; ++c)
     {
+      const int64_t e = grow * N + c * CW + lane * V;
       if (DZ16H != nullptr) {  // fp16-split planes of dz * gscale for the tensor-core wgrad / dgrad (no fp32 copy)
         __half2 h0, h1, l0, l1;
-        tc::split16x2(dz[4 * c] * gscale, dz[4 * c + 1] * gscale, h0, l0);
-        tc::split16x2(dz[4 * c + 2] * gscale, dz[4 * c + 3] * gscale, h1, l1);
-        *reinterpret_cast<uint2*>(DZ16H + grow * N + c * 128 + lane * 4) =
-            make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
-        *reinterpret_cast<uint2*>(DZ16L + grow * N + c * 128 + lane * 4) =
-            make_uint2(*reinterpret_cast<uint32_t*>(&l0), *reinterpret_cast<uint32_t*>(&l1));
+        tc::split16x2(dz[V * c] * gscale, dz[V * c + 1] * gscale, h0, l0);
+        if constexpr (V == 4) {
+          tc::split16x2(dz[4 * c + 2] * gscale, dz[4 * c + 3] * gscale, h1, l1);
+          *reinterpret_cast<uint2*>(DZ16H + e) =
+              make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
+          *reinterpret_cast<uint2*>(DZ16L + e) =
+              make_uint2(*reinterpret_cast<uint32_t*>(&l0), *reinterpret_cast<uint32_t*>(&l1));
+        } else {
+          *reinterpret_cast<__half2*>(DZ16H + e) = h0;
+          *reinterpret_cast<__half2*>(DZ16L + e) = l0;
+        }
         continue;
       }
-      *reinterpret_cast<float4*>(DZ + grow * N + c * 128 + lane * 4) =
-          make_float4(dz[4 * c], dz[4 * c + 1], dz[4 * c + 2], dz[4 * c + 3]);
-      if (DZLO != nullptr)
-        *reinterpret_cast<float4*>(DZLO + grow * N + c * 128 + lane * 4) =
-            make_float4(tc::tf32_lo(dz[4 * c]), tc::tf32_lo(dz[4 * c + 1]), tc::tf32_lo(dz[4 * c + 2]),
-                        tc::tf32_lo(dz[4 * c + 3]));
+      st_feat<V>(DZ + e, dz + V * c);
+      if (DZLO != nullptr) {
+        float lo[V];
+#pragma unroll
+        for (int k = 0; k < V; ++k) lo[k] = tc::tf32_lo(dz[V * c + k]);
+        st_feat<V>(DZLO + e, lo);
+      }
     }
   }
   // warp-private slices (each lane owns its features: plain stores)
 #pragma unroll
   for (int j = 0; j < F; ++j) {
-    const int f = (j >> 2) * 128 + lane * 4 + (j & 3);
+    const int f = (j / V) * CW + lane * V + (j % V);
     s_red3[warp * 3 * N + f] = a_dsc[j];
     s_red3[warp * 3 * N + N + f] = a_dbi[j];
     s_red3[warp * 3 * N + 2 * N + f] = a_db[j];
@@ -2234,9 +2285,11 @@ struct Workspace {
   uint32_t* relu_bits;            // packed (h1 > 0) mask, 1024 bits per row (MMA conv path -> tensor-core dgrad epilogue)
   float *rb_part, *cb_part;       // per-CTA partial vectors of the deterministic row_bwd / conv_bwd reductions
   float* wg_part;                 // split-K partial outputs of the tensor-core weight gradient (small S: few output tiles)
-  // MLP
-  float *xg, *h0, *xhat0, *rstd0, *hh1, *xhat1, *rstd1, *dzl, *dh0;
-  float *m16_h0, *m16_w, *m16_dz;   // fp16 (hi, lo') planes of h0 / Dense_1 kernel / dz1 for the tensor-core hidden layer
+  // MLP: per hidden layer l the output h, LayerNorm xhat and rstd; dz / dh of the layer being differentiated
+  float *xg, *h[PQN_MAX_LAYERS], *xhat[PQN_MAX_LAYERS], *rstd[PQN_MAX_LAYERS], *dzl, *dh0;
+  // fp16 (hi, lo') planes for the tensor-core hidden layers l >= 1: of h_{l-1} and of Dense_l's kernel (one block per
+  // hidden layer each, see mlp_planes), and of dz of the layer being differentiated
+  float *m16_h0, *m16_w, *m16_dz;
 };
 
 // split-K of the tensor-core weight gradient: when S * m_tiles * n_tiles output tiles cannot fill the SMs (one seed of
@@ -2271,14 +2324,21 @@ static void launch_split_reduce(const float* part, int ksplit, int64_t split_str
     wgrad_split_reduce_kernel<8><<<dim3((unsigned)((n + 31) / 32), S), 256, 0, st>>>(part, ksplit, split_stride, n, out, out_seed_stride);
 }
 
+// N tile of the FFMA gradient kernels: 128, or 64 for a 64-wide layer; output tiles of a [Kin][N] weight gradient
+static inline int ffma_ntile(int N) { return N % 128 == 0 ? 128 : 64; }
+static inline int ffma_tiles(int Kin, int N) { return (Kin + 127) / 128 * (N / ffma_ntile(N)); }
+
 // The register-tiled FFMA weight gradient + (splits > 1) its ordered reduction.  `part` needs splits * S * Kin * N floats
 // (<= wgrad_split_tiles() tiles of 128 x 128: wgrad_splits keeps tiles * S * splits below 4 * SMs).
 static void run_wgrad_ffma(const float* X, int64_t x_seed_stride, int ldx, const float* DZ, int64_t dz_seed_stride, int N,
                            float* grads, int64_t P, int64_t off_w, int rows, int Kin, int S, int splits, float* part,
                            cudaStream_t st) {
   { LaunchScope _ls(K_WGRAD, st);
-    wgrad_kernel<<<dim3((unsigned)((Kin + 127) / 128), (unsigned)(N / 128), (unsigned)(S * splits)), GT, 0, st>>>(
-        X, x_seed_stride, ldx, DZ, dz_seed_stride, N, grads, P, off_w, rows, Kin, splits, part); }
+    const dim3 grid((unsigned)((Kin + 127) / 128), (unsigned)(N / ffma_ntile(N)), (unsigned)(S * splits));
+    if (ffma_ntile(N) == 128)
+      wgrad_kernel<128><<<grid, GT, 0, st>>>(X, x_seed_stride, ldx, DZ, dz_seed_stride, N, grads, P, off_w, rows, Kin, splits, part);
+    else
+      wgrad_kernel<64><<<grid, GT, 0, st>>>(X, x_seed_stride, ldx, DZ, dz_seed_stride, N, grads, P, off_w, rows, Kin, splits, part); }
   if (splits > 1) {
     const int64_t n = (int64_t)Kin * N;
     launch_split_reduce(part, splits, (int64_t)S * n, n, S, grads + off_w, P, st);
@@ -2298,7 +2358,7 @@ __global__ void __launch_bounds__(256) wgrad_thin_kernel(const float* __restrict
   __shared__ float xs[THIN_ROWS * THIN_KMAX];
   __shared__ float4 red[256];
   const int seed = blockIdx.y, S = gridDim.y;
-  const int cols4 = N >> 2;                                             // threads per row (float4 columns); N in {128, 256}
+  const int cols4 = N >> 2;                                             // threads per row (float4 columns); N in 64..512
   const int groups = 256 / cols4, c4 = threadIdx.x % cols4, grp = threadIdx.x / cols4;
   const float* __restrict__ Xs = X + (int64_t)seed * x_seed_stride;
   const float4* __restrict__ Zs = reinterpret_cast<const float4*>(DZ + (int64_t)seed * dz_seed_stride);
@@ -2356,7 +2416,7 @@ static inline unsigned cdiv(int64_t a, int64_t b) { return (unsigned)((a + b - 1
 // the stream; chunks * S * D * H floats are far below its size).
 static void run_wgrad_first(const float* X, const float* DZ, float* grads, int64_t P, int64_t off_w, int S, int rows,
                             int D, int H, float* part, float* wg_part, cudaStream_t st) {
-  if (D <= THIN_KMAX && (H == 128 || H == 256)) {
+  if (D <= THIN_KMAX) {
     int chunks = (2 * device_sm_count()) / S;
     const int max_chunks = (rows + THIN_ROWS - 1) / THIN_ROWS;
     if (chunks > max_chunks) chunks = max_chunks;
@@ -2371,7 +2431,19 @@ static void run_wgrad_first(const float* X, const float* DZ, float* grads, int64
     return;
   }
   run_wgrad_ffma(X, (int64_t)rows * D, D, DZ, (int64_t)rows * H, H, grads, P, off_w, rows, D, S,
-                 wgrad_splits((D + 127) / 128 * (H / 128), S, rows), wg_part, st);
+                 wgrad_splits(ffma_tiles(D, H), S, rows), wg_part, st);
+}
+
+// OUT[S][rows][Kprev] (=, or += with accumulate) relu_mask(HPREV) * (DZ[S][rows][N] . W[Kprev][N]^T) on the FFMA kernel
+static void launch_dgrad(const float* DZ, int64_t dz_seed_stride, int N, const float* params, int64_t P, int64_t off_w,
+                         const float* HPREV, float* OUT, int64_t h_seed_stride, int rows, int Kprev, int accumulate, int S,
+                         cudaStream_t st) {
+  LaunchScope _ls(K_DGRAD, st);
+  const dim3 grid(cdiv(rows, 128), (unsigned)(Kprev / ffma_ntile(Kprev)), (unsigned)S);
+  if (ffma_ntile(Kprev) == 128)
+    dgrad_kernel<128><<<grid, GT, 0, st>>>(DZ, dz_seed_stride, N, params, P, off_w, HPREV, OUT, h_seed_stride, rows, Kprev, accumulate);
+  else
+    dgrad_kernel<64><<<grid, GT, 0, st>>>(DZ, dz_seed_stride, N, params, P, off_w, HPREV, OUT, h_seed_stride, rows, Kprev, accumulate);
 }
 
 static int64_t carve(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* base, Workspace* w) {
@@ -2400,34 +2472,38 @@ static int64_t carve(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* bas
     ww->cb_part = take(part_ctas(S) * (int64_t)(9 * d->in_c * CONV_O + 3 * CONV_O));
     ww->wg_part = take(wgrad_split_tiles() * 128 * 128);
   } else {
-    const int H = d->hidden;
+    const int H = d->hidden, nl = d->layers > 2 ? d->layers : 2, nh = nl - 1;
     ww->xg = take(R * d->in_c);
-    ww->h0 = take(R * H);
-    ww->xhat0 = take(R * H);
-    ww->rstd0 = take(R);
-    ww->hh1 = take(R * H);
-    ww->xhat1 = take(R * H);
-    ww->rstd1 = take(R);
+    for (int l = 0; l < nl; ++l) { ww->h[l] = take(R * H); ww->xhat[l] = take(R * H); ww->rstd[l] = take(R); }
     ww->dzl = take(R * H);
     ww->dh0 = take(R * H);
     ww->rb_part = take(part_ctas(S) * row_bwd_part_floats(H, d->num_actions));
     ww->cb_part = nullptr;
     ww->wg_part = take(wgrad_split_tiles() * 128 * 128);
-    ww->m16_h0 = take(R * H);                       // 2 planes x 2 bytes = 4 bytes per element
-    ww->m16_w = take((int64_t)S * H * H);
+    ww->m16_h0 = take(nh * R * H);                  // 2 planes x 2 bytes = 4 bytes per element
+    ww->m16_w = take(nh * (int64_t)S * H * H);
     ww->m16_dz = take(R * H);
   }
   return off;
 }
 
+// BN = the layer's width: 64, 128 or 256, and 512 for MODE 3 only (two 256-column tiles; dense_ln_fwd adds the
+// LayerNorm at 512).  Any other combination is refused, not launched with a narrower tile.
 template <int MODE>
-static void launch_dense(int BN, dim3 grid, cudaStream_t st, const float* X, int64_t xss, int ldx, const float* params,
+static int launch_dense(int BN, dim3 grid, cudaStream_t st, const float* X, int64_t xss, int ldx, const float* params,
                          int64_t P, int64_t ow, int64_t ob, int64_t osc, int64_t obi, int64_t ohw, int64_t ohb, int A,
                          float* H, float* XH, float* RS, float* Q, int rows, int K) {
-  if (BN == 128)
+  if (BN != 64 && BN != 128 && BN != 256 && !(MODE == 3 && BN == 512))
+    return set_error(PQN_E_UNSUPPORTED, "dense_fwd: width %d is not built for mode %d", BN, MODE);
+  if (BN == 64)
+    { LaunchScope _ls(K_DENSE_FWD, st); dense_fwd_kernel<64, MODE><<<grid, GT, 0, st>>>(X, xss, ldx, params, P, ow, ob, osc, obi, ohw, ohb, A, H, XH, RS, Q, rows, K); }
+  else if (MODE == 3 && BN == 512)
+    { LaunchScope _ls(K_DENSE_FWD, st); dense_fwd_kernel<256, 3><<<dim3(grid.x, grid.y, 2), GT, 0, st>>>(X, xss, ldx, params, P, ow, ob, osc, obi, ohw, ohb, A, H, XH, RS, Q, rows, K); }
+  else if (BN == 128)
     { LaunchScope _ls(K_DENSE_FWD, st); dense_fwd_kernel<128, MODE><<<grid, GT, 0, st>>>(X, xss, ldx, params, P, ow, ob, osc, obi, ohw, ohb, A, H, XH, RS, Q, rows, K); }
   else
     { LaunchScope _ls(K_DENSE_FWD, st); dense_fwd_kernel<256, MODE><<<grid, GT, 0, st>>>(X, xss, ldx, params, P, ow, ob, osc, obi, ohw, ohb, A, H, XH, RS, Q, rows, K); }
+  return 0;
 }
 
 
@@ -2508,10 +2584,14 @@ static int run_row_bwd(int N, bool head, dim3 rbg, int A, cudaStream_t st, const
   rc = launch_row_bwd<NN, HH>(rbg, A, st, Hh, XHAT, RSTD, DH, DZ, DZLO, DZ16H, DZ16L, gscale, params, grads, P,     \
                               off_scale, off_scale, off_bias, off_db, off_hw, off_hb, A, gather, action, target, trps, \
                               part, rows)
-  if (N == 128 && head) PQN_RB(128, true);
+  if (N == 64 && head) PQN_RB(64, true);
+  else if (N == 64) PQN_RB(64, false);
+  else if (N == 128 && head) PQN_RB(128, true);
   else if (N == 128) PQN_RB(128, false);
   else if (N == 256 && head) PQN_RB(256, true);
   else if (N == 256) PQN_RB(256, false);
+  else if (N == 512 && head) PQN_RB(512, true);
+  else if (N == 512) PQN_RB(512, false);
   else return set_error(PQN_E_UNSUPPORTED, "row_bwd width %d", N);
 #undef PQN_RB
   if (rc) return rc;
@@ -2842,9 +2922,74 @@ static int tc_dgrad(const float* params, int64_t P, const pqn_net_layout_t& L, c
 }
 
 #include "pqn_norm.cuh"
+
+// Dense -> LayerNorm -> ReLU (MODE 0: h; MODE 1: h, xhat, rstd) or Dense -> LayerNorm -> ReLU -> Q head (MODE 2) on the
+// FFMA kernels, at every built width.  Up to 256 columns this is dense_fwd_kernel with the fused epilogue.  A 512-wide
+// row does not fit its register tile, so the raw product (MODE 3, two 256-column tiles) goes to H and ln_fwd_kernel<512>
+// normalises it in place (MODE 2: H is scratch, head_fwd_kernel adds the head).
+template <int MODE>
+static int dense_ln_fwd(int N, dim3 grid, cudaStream_t st, const float* X, int64_t xss, int ldx, const float* params,
+                         int64_t P, const DenseOff& o, int64_t ohw, int64_t ohb, int A, float* H, float* XH, float* RS,
+                         float* Q, int rows, int K) {
+  if (N != 512)
+    return launch_dense<MODE>(N, grid, st, X, xss, ldx, params, P, o.w, o.b, o.g, o.bi, ohw, ohb, A, H, XH, RS, Q, rows, K);
+  int rc = launch_dense<3>(N, grid, st, X, xss, ldx, params, P, o.w, o.b, 0, 0, 0, 0, A, H, nullptr, nullptr, nullptr, rows, K);
+  if (rc) return rc;
+  { LaunchScope _ls(K_DENSE_FWD, st);
+    nrm::ln_fwd_kernel<512><<<dim3(cdiv(rows, 8), grid.y), 256, 0, st>>>(H, rows, params, P, o.g, o.bi, MODE == 1 ? XH : nullptr,
+                                                                        MODE == 1 ? RS : nullptr, H); }
+  if (MODE == 2) {
+    LaunchScope _ls(K_DENSE_FWD, st);
+    nrm::head_fwd_kernel<<<dim3(cdiv(rows, 8), grid.y), 256, 0, st>>>(H, rows, N, params, P, ohw, ohb, A, Q);
+  }
+  return 0;
+}
+
 #include "pqn_rnn.cuh"
 
+// HH = H (64, 128, 256 or 512) as a constant for the one-thread-per-feature kernels
+#define PQN_H_DISPATCH(H_, ...)                                         \
+  switch (H_) {                                                         \
+    case 64: { constexpr int HH = 64; __VA_ARGS__; } break;             \
+    case 128: { constexpr int HH = 128; __VA_ARGS__; } break;           \
+    case 256: { constexpr int HH = 256; __VA_ARGS__; } break;           \
+    case 512: { constexpr int HH = 512; __VA_ARGS__; } break;           \
+    default: return set_error(PQN_E_UNSUPPORTED, "GRU hidden=%d", H_);  \
+  }
+
 static inline bool modular_net(const pqn_net_desc_t* d) { return d->norm_type != PQN_NORM_LAYER || d->norm_input != 0; }
+
+// The default MLP's hidden layers l >= 1 (K = N = H) run on the wgmma fp16-split GEMMs from H = 128 up; a 64-wide
+// layer would fill half of the GEMM's 128-wide N tile, so H = 64 stays on the FFMA kernels (64-wide N tiles).
+static inline bool mlp_hidden_tc(int H) { return g_use_tc == 2 && H >= 128; }
+// fp16 (hi, lo') planes of hidden layer l >= 1: its input h_{l-1} ([R][H] each) and its kernel ([S][H][H] each)
+static inline __half* mlp_h_planes(const Workspace& w, int64_t R, int H, int l) {
+  return reinterpret_cast<__half*>(w.m16_h0) + (int64_t)(l - 1) * 2 * R * H;
+}
+static inline __half* mlp_w_planes(const Workspace& w, int S, int H, int l) {
+  return reinterpret_cast<__half*>(w.m16_w) + (int64_t)(l - 1) * 2 * S * H * H;
+}
+// Z = h_{l-1} . W_l on wgmma (planes of both operands written here), then bias + LayerNorm + ReLU in place
+static int mlp_hidden_tc_fwd(const Workspace& w, const pqn_net_layout_t& L, const float* params, int64_t P, int H, int l, int S,
+                             int rows, float* xhat, float* rstd, int kid, cudaStream_t st) {
+  const int64_t R = (int64_t)S * rows;
+  const DenseOff o = dense_off(L, H, l);
+  __half* hp = mlp_h_planes(w, R, H, l);
+  __half* wp = mlp_w_planes(w, S, H, l);
+  split16_rows(w.h[l - 1], 0, R * H, 1, hp, hp + R * H, st);
+  split16_rows(params + o.w, P, (int64_t)H * H, S, wp, wp + (int64_t)S * H * H, st);
+  int rc = tc16_mm_store(hp, R * H, wp, (int64_t)S * H * H, w.h[l], S, rows, H, H, st, kid);
+  if (rc) return rc;
+  LaunchScope _ls(K_NORM_FWD, st);
+  const dim3 g(cdiv(rows, 8), S);
+  switch (H) {
+    case 128: nrm::ln_fwd_kernel<128><<<g, 256, 0, st>>>(w.h[l], rows, params, P, o.g, o.bi, xhat, rstd, w.h[l], o.b); break;
+    case 256: nrm::ln_fwd_kernel<256><<<g, 256, 0, st>>>(w.h[l], rows, params, P, o.g, o.bi, xhat, rstd, w.h[l], o.b); break;
+    case 512: nrm::ln_fwd_kernel<512><<<g, 256, 0, st>>>(w.h[l], rows, params, P, o.g, o.bi, xhat, rstd, w.h[l], o.b); break;
+    default: return set_error(PQN_E_UNSUPPORTED, "tensor-core hidden layer width %d", H);
+  }
+  return 0;
+}
 
 }  // namespace pqn
 
@@ -2870,7 +3015,7 @@ int pqn_rnn_step(const pqn_net_desc_t* d, const float* params, float* hs, const 
   make_layout(d, &L);
   rnn::RnnWs w;
   rnn::carve_rnn(d, S, E, (char*)workspace, &w);
-  rnn::rnn_trunk(d, L, params, obs, obs_rows_per_seed * d->in_c, S, E, false, w, st);
+  if ((rc = rnn::rnn_trunk(d, L, params, obs, obs_rows_per_seed * d->in_c, S, E, false, w, st))) return rc;
   if ((rc = rnn::rnn_scan_fwd<false>(d, L, params, last_action, last_done, hs, hs, S, 1, E, w, st))) return rc;
   { LaunchScope _ls(K_RNN_MISC, st);
     nrm::head_fwd_kernel<<<dim3(cdiv(E, 8), S), 256, 0, st>>>(w.y, E, d->hidden, params, L.total, L.head_w, L.head_b,
@@ -2899,7 +3044,7 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
     return check_launch("pqn_rnn_loss_grad(memset)");
   const int64_t gs = (int64_t)S * rows * H;
   // ---- forward over the window
-  rnn::rnn_trunk(d, L, params, obs, (int64_t)rows * D, S, rows, true, w, st);
+  if ((rc = rnn::rnn_trunk(d, L, params, obs, (int64_t)rows * D, S, rows, true, w, st))) return rc;
   if ((rc = rnn::rnn_scan_fwd<true>(d, L, params, last_action, last_done, hs0, w.dhl /*scratch carry out*/, S, T, B, w, st)))
     return rc;
   { LaunchScope _ls(K_RNN_MISC, st);
@@ -2911,8 +3056,7 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
                                                                     loss_sum, qsa_sum); }
   // ---- head backward
   { LaunchScope _ls(K_RNN_MISC, st);
-    if (H == 128) rnn::rnn_head_bwd_kernel<128><<<dim3(nrm::RED_BLOCKS, S), 128, 0, st>>>(w.y, w.dq, rows, A, params, P, L.head_w, w.dy, w.part);
-    else rnn::rnn_head_bwd_kernel<256><<<dim3(nrm::RED_BLOCKS, S), 256, 0, st>>>(w.y, w.dq, rows, A, params, P, L.head_w, w.dy, w.part); }
+    PQN_H_DISPATCH(H, rnn::rnn_head_bwd_kernel<HH><<<dim3(nrm::RED_BLOCKS, S), HH, 0, st>>>(w.y, w.dq, rows, A, params, P, L.head_w, w.dy, w.part)); }
   { LaunchScope _ls(K_RNN_MISC, st);
     rnn::rnn_head_bwd_final_kernel<<<S, 256, 0, st>>>(w.part, nrm::RED_BLOCKS, H, A, grads, P, L.head_w, L.head_b); }
   // ---- BPTT through the GRU
@@ -2921,14 +3065,12 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
     rnn::gru_transpose_kernel<<<dim3(32, S, 3), 256, 0, st>>>(params, P, L, H, w.wt, wts); }
   { LaunchScope _ls(K_RNN_SCAN, st);
     const dim3 grid(cdiv(B, rnn::RB), S);
-    if (H == 128) rnn::gru_scan_bwd_kernel<128><<<grid, 128, 0, st>>>(w.dy, last_done, w.h0, w.rg, w.zg, w.ng, w.hn, w.wt, wts, w.da, gs, w.dhn, T, B);
-    else rnn::gru_scan_bwd_kernel<256><<<grid, 256, 0, st>>>(w.dy, last_done, w.h0, w.rg, w.zg, w.ng, w.hn, w.wt, wts, w.da, gs, w.dhn, T, B); }
+    PQN_H_DISPATCH(H, rnn::gru_scan_bwd_kernel<HH><<<grid, HH, 0, st>>>(w.dy, last_done, w.h0, w.rg, w.zg, w.ng, w.hn, w.wt, wts, w.da, gs, w.dhn, T, B)); }
   // ---- weight gradients of the GRU (batched over the window)
   const float* xl = w.h[d->layers - 1];   // trunk output = first H columns of the GRU input
   const int64_t iw[3] = {L.gru_ir_w, L.gru_iz_w, L.gru_in_w}, ib[3] = {L.gru_ir_b, L.gru_iz_b, L.gru_in_b};
   const int64_t hw[3] = {L.gru_hr_w, L.gru_hz_w, L.gru_hn_w};
-  const int tiles = (H / 128) * (H / 128);
-  const int sp = wgrad_splits(tiles, S, rows);
+  const int sp = wgrad_splits(ffma_tiles(H, H), S, rows);
   nrm::NormWs nw = {};
   nw.part = w.part;
   for (int g = 0; g < 3; ++g) {
@@ -2938,28 +3080,28 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
     const float* dh = g == 2 ? w.dhn : da;                                                             // hn uses d(hn)
     run_wgrad_ffma(w.h0, (int64_t)rows * H, H, dh, (int64_t)rows * H, H, grads, P, hw[g], rows, H, S, sp, w.wgp, st);
     // d x_L (+)= da_g W_ig[:H]^T, masked by the trunk's ReLU
-    { LaunchScope _ls(K_DGRAD, st); dgrad_kernel<<<dim3(cdiv(rows, 128), H / 128, S), GT, 0, st>>>(da, (int64_t)rows * H, H, params, P, iw[g], xl, w.dx, (int64_t)rows * H, rows, H, g > 0 ? 1 : 0); }
+    launch_dgrad(da, (int64_t)rows * H, H, params, P, iw[g], xl, w.dx, (int64_t)rows * H, rows, H, g > 0 ? 1 : 0, S, st);
   }
   nrm::colsum2(w.dhn, w.dhn, S, rows, H, H, nw, w.sums, grads, P, L.gru_hn_b, -1, st);                 // d b_hn
   { LaunchScope _ls(K_RNN_MISC, st);
-    if (H == 128) rnn::rnn_onehot_grad_kernel<128><<<dim3(S, 3), 128, 0, st>>>(w.da, gs, last_action, rows, A, grads, P, L);
-    else rnn::rnn_onehot_grad_kernel<256><<<dim3(S, 3), 256, 0, st>>>(w.da, gs, last_action, rows, A, grads, P, L); }
+    PQN_H_DISPATCH(H, rnn::rnn_onehot_grad_kernel<HH><<<dim3(S, 3), HH, 0, st>>>(w.da, gs, last_action, rows, A, grads, P, L)); }
   // ---- trunk backward (LayerNorm backward -> weight gradient -> input gradient of the layer below)
   const dim3 rbg(conv_mma_ctas(S, rows, 4), S);
-  const int64_t offw[2] = {L.d0_w, L.d1_w}, offb[2] = {L.d0_b, L.d1_b}, offg[2] = {L.ln0_scale, L.ln1_scale},
-                offbi[2] = {L.ln0_bias, L.ln1_bias};
   float* dcur = w.dx;
   for (int l = d->layers - 1; l >= 0; --l) {
+    const DenseOff o = dense_off(L, H, l);
     if ((rc = run_row_bwd(H, false, rbg, A, st, nullptr, w.xh[l], w.rs[l], dcur, dcur, nullptr, nullptr, nullptr, 1.0f, params,
-                          grads, P, offg[l], offbi[l], offb[l], 0, 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr, w.rbp,
+                          grads, P, o.g, o.bi, o.b, 0, 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr, w.rbp,
                           rows))) return rc;
     const float* xprev = l == 0 ? obs : w.h[l - 1];
     const int kin = l == 0 ? D : H;
-    const int spl = wgrad_splits((kin + 127) / 128 * (H / 128), S, rows);
-    run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, dcur, (int64_t)rows * H, H, grads, P, offw[l], rows, kin, S, spl, w.wgp, st);
+    const int spl = wgrad_splits(ffma_tiles(kin, H), S, rows);
+    run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, dcur, (int64_t)rows * H, H, grads, P, o.w, rows, kin, S, spl, w.wgp, st);
     if (l > 0) {
-      { LaunchScope _ls(K_DGRAD, st); dgrad_kernel<<<dim3(cdiv(rows, 128), H / 128, S), GT, 0, st>>>(dcur, (int64_t)rows * H, H, params, P, offw[l], w.h[l - 1], w.dhl, (int64_t)rows * H, rows, H, 0); }
-      dcur = w.dhl;
+      // dh_{l-1} goes to the buffer dcur does not use (dx and dhl alternate): dgrad reads all of dz_l while it writes
+      float* dnext = dcur == w.dhl ? w.dx : w.dhl;
+      launch_dgrad(dcur, (int64_t)rows * H, H, params, P, o.w, w.h[l - 1], dnext, (int64_t)rows * H, rows, H, 0, S, st);
+      dcur = dnext;
     }
   }
   return check_launch("pqn_rnn_loss_grad");
@@ -2982,6 +3124,20 @@ int pqn_net_layout(const pqn_net_desc_t* d, pqn_net_layout_t* out) {
   if (rc) return rc;
   if (!out) return set_error(PQN_E_INVALID, "pqn_net_layout: out is NULL");
   make_layout(d, out);
+  return PQN_OK;
+}
+
+int pqn_net_dense_layer(const pqn_net_desc_t* d, int32_t layer, int64_t* offsets_host) {
+  int rc = check_desc(d, "pqn_net_dense_layer");
+  if (rc) return rc;
+  if (d->kind != PQN_NET_MLP && d->kind != PQN_NET_RNN)
+    return set_error(PQN_E_INVALID, "pqn_net_dense_layer: only the MLP and GRU networks have hidden dense layers");
+  if (!offsets_host || layer < 0 || layer >= d->layers)
+    return set_error(PQN_E_INVALID, "pqn_net_dense_layer: layer=%d out of [0,%d) or offsets NULL", layer, d->layers);
+  pqn_net_layout_t L;
+  make_layout(d, &L);
+  const DenseOff o = dense_off(L, d->hidden, layer);
+  offsets_host[0] = o.w; offsets_host[1] = o.b; offsets_host[2] = o.g; offsets_host[3] = o.bi;
   return PQN_OK;
 }
 
@@ -3027,9 +3183,9 @@ int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* 
       launch_split_w1(params, L.total, L.d0_w, w.w1_lo, S, st);
       if ((rc = tc_dense_fwd(tc::EPI_LN_HEAD, params, L.total, L, w, A, q, S, (int)rows, st))) return rc;
     } else {
-      launch_dense<2>(128, dim3(cdiv(rows, 128), S), st, w.h1, rows * FLAT_CNN, FLAT_CNN, params, L.total, L.d0_w,
+      if ((rc = launch_dense<2>(128, dim3(cdiv(rows, 128), S), st, w.h1, rows * FLAT_CNN, FLAT_CNN, params, L.total, L.d0_w,
                       L.d0_b, L.ln1_scale, L.ln1_bias, L.head_w, L.head_b, A, nullptr, nullptr, nullptr, q, (int)rows,
-                      FLAT_CNN);
+                      FLAT_CNN))) return rc;
     }
   } else {
     const int D = d->in_c, H = d->hidden;
@@ -3042,29 +3198,32 @@ int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* 
       xss = rows * D;
     }
     const int BM = (H == 128) ? 128 : 64;
-    if (d->layers == 1) {
-      launch_dense<2>(H, dim3(cdiv(rows, BM), S), st, x, xss, D, params, L.total, L.d0_w, L.d0_b, L.ln0_scale,
-                      L.ln0_bias, L.head_w, L.head_b, A, nullptr, nullptr, nullptr, q, (int)rows, D);
+    const dim3 grid(cdiv(rows, BM), S);
+    const int last = d->layers - 1;
+    if (last == 0) {
+      if ((rc = dense_ln_fwd<2>(H, grid, st, x, xss, D, params, L.total, dense_off(L, H, 0), L.head_w, L.head_b, A, w.h[0], nullptr,
+                      nullptr, q, (int)rows, D))) return rc;
     } else {
-      launch_dense<0>(H, dim3(cdiv(rows, BM), S), st, x, xss, D, params, L.total, L.d0_w, L.d0_b, L.ln0_scale,
-                      L.ln0_bias, 0, 0, A, w.h0, nullptr, nullptr, nullptr, (int)rows, D);
-      if (g_use_tc == 2) {
-        // hidden layer (K = N = H) on wgmma: fp16-split planes of h0 and of the Dense_1 kernel, raw product, then
-        // bias + LayerNorm + ReLU and the Q head in row kernels
-        const int64_t R = (int64_t)S * rows;
-        __half* hp = reinterpret_cast<__half*>(w.m16_h0);
-        __half* wp = reinterpret_cast<__half*>(w.m16_w);
-        split16_rows(w.h0, 0, R * H, 1, hp, hp + R * H, st);
-        split16_rows(params + L.d1_w, L.total, (int64_t)H * H, S, wp, wp + (int64_t)S * H * H, st);
-        if ((rc = tc16_mm_store(hp, R * H, wp, (int64_t)S * H * H, w.hh1, S, (int)rows, H, H, st, K_TC_FWD_HEAD))) return rc;
-        { LaunchScope _ls(K_NORM_FWD, st);
-          if (H == 128) nrm::ln_fwd_kernel<128><<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.hh1, rows, params, L.total, L.ln1_scale, L.ln1_bias, nullptr, nullptr, w.hh1, L.d1_b);
-          else nrm::ln_fwd_kernel<256><<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.hh1, rows, params, L.total, L.ln1_scale, L.ln1_bias, nullptr, nullptr, w.hh1, L.d1_b); }
-        { LaunchScope _ls(K_NORM_FWD, st);
-          nrm::head_fwd_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.hh1, (int)rows, H, params, L.total, L.head_w, L.head_b, A, q); }
-      } else
-      launch_dense<2>(H, dim3(cdiv(rows, BM), S), st, w.h0, rows * H, H, params, L.total, L.d1_w, L.d1_b, L.ln1_scale,
-                      L.ln1_bias, L.head_w, L.head_b, A, nullptr, nullptr, nullptr, q, (int)rows, H);
+      if ((rc = dense_ln_fwd<0>(H, grid, st, x, xss, D, params, L.total, dense_off(L, H, 0), 0, 0, A, w.h[0], nullptr, nullptr, nullptr,
+                      (int)rows, D))) return rc;
+      for (int l = 1; l <= last; ++l) {
+        if (mlp_hidden_tc(H)) {
+          // hidden layer (K = N = H) on wgmma: fp16-split planes of h_{l-1} and of the Dense_l kernel, raw product, then
+          // bias + LayerNorm + ReLU (and, after the last, the Q head) in row kernels
+          if ((rc = mlp_hidden_tc_fwd(w, L, params, L.total, H, l, S, (int)rows, nullptr, nullptr,
+                                      l == last ? K_TC_FWD_HEAD : K_TC_FWD, st))) return rc;
+          if (l == last) {
+            LaunchScope _ls(K_NORM_FWD, st);
+            nrm::head_fwd_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.h[l], (int)rows, H, params, L.total, L.head_w, L.head_b, A, q);
+          }
+        } else if (l == last) {
+          if ((rc = dense_ln_fwd<2>(H, grid, st, w.h[l - 1], rows * H, H, params, L.total, dense_off(L, H, l), L.head_w, L.head_b, A,
+                          w.h[l], nullptr, nullptr, q, (int)rows, H))) return rc;
+        } else {
+          if ((rc = dense_ln_fwd<0>(H, grid, st, w.h[l - 1], rows * H, H, params, L.total, dense_off(L, H, l), 0, 0, A, w.h[l], nullptr,
+                          nullptr, nullptr, (int)rows, H))) return rc;
+        }
+      }
     }
   }
   return check_launch("pqn_qnet_forward");
@@ -3115,8 +3274,8 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
       launch_split_w1(params, P, L.d0_w, w.w1_lo, S, st);
       if ((rc = tc_dense_fwd(tc::EPI_LN_TRAIN, params, P, L, w, A, nullptr, S, R, st))) return rc;
     } else {
-      launch_dense<1>(128, dim3(cdiv(rows, 128), S), st, w.h1, rows * FLAT_CNN, FLAT_CNN, params, P, L.d0_w, L.d0_b,
-                      L.ln1_scale, L.ln1_bias, 0, 0, A, w.h2, w.xhat2, w.rstd2, nullptr, R, FLAT_CNN);
+      if ((rc = launch_dense<1>(128, dim3(cdiv(rows, 128), S), st, w.h1, rows * FLAT_CNN, FLAT_CNN, params, P, L.d0_w, L.d0_b,
+                      L.ln1_scale, L.ln1_bias, 0, 0, A, w.h2, w.xhat2, w.rstd2, nullptr, R, FLAT_CNN))) return rc;
     }
     const dim3 rbg(conv_mma_ctas(S, R, 4), S);
     if ((rc = run_row_bwd(128, true, rbg, A, st, w.h2, w.xhat2, w.rstd2, nullptr, w.dz2, (use_tc && !f16) ? w.dz2_lo : nullptr,
@@ -3132,9 +3291,7 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
     } else {
       const int splits = wgrad_splits(FLAT_CNN / 128, S, R);
       run_wgrad_ffma(w.h1, rows * FLAT_CNN, FLAT_CNN, w.dz2, rows * HID_CNN, HID_CNN, grads, P, L.d0_w, R, FLAT_CNN, S, splits, w.wg_part, st);
-      { LaunchScope _ls(K_DGRAD, st); dgrad_kernel<<<dim3(cdiv(rows, 128), FLAT_CNN / 128, S), GT, 0, st>>>(w.dz2, rows * HID_CNN, HID_CNN, params, P,
-                                                                            L.d0_w, w.h1, w.h1, rows * FLAT_CNN, R,
-                                                                            FLAT_CNN); }
+      launch_dgrad(w.dz2, rows * HID_CNN, HID_CNN, params, P, L.d0_w, w.h1, w.h1, rows * FLAT_CNN, R, FLAT_CNN, 0, S, st);
     }
     dim3 cg(conv_bwd_ctas(S, R), S);
     if (g_conv_mma) {
@@ -3176,47 +3333,55 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
       nw.part = w.rb_part;
       nrm::colsum2(w.xg, w.xg, S, R, D, D, nw, bn_sums, nullptr, 0, -1, -1, st);
     }
-    launch_dense<1>(H, dim3(cdiv(rows, BM), S), st, w.xg, rows * D, D, params, P, L.d0_w, L.d0_b, L.ln0_scale,
-                    L.ln0_bias, 0, 0, A, w.h0, w.xhat0, w.rstd0, nullptr, R, D);
-    const dim3 rbg(conv_mma_ctas(S, R, 4), S);
-    if (d->layers == 2 && g_use_tc == 2) {
-      // hidden layer on wgmma (fp16-split planes): forward product, weight gradient and input gradient
-      const int64_t RR = (int64_t)S * rows;
-      __half* hp = reinterpret_cast<__half*>(w.m16_h0);
-      __half* wp = reinterpret_cast<__half*>(w.m16_w);
-      __half* zp = reinterpret_cast<__half*>(w.m16_dz);
-      const float gscale = grad_scale(rows);
-      split16_rows(w.h0, 0, RR * H, 1, hp, hp + RR * H, st);
-      split16_rows(params + L.d1_w, P, (int64_t)H * H, S, wp, wp + (int64_t)S * H * H, st);
-      if ((rc = tc16_mm_store(hp, RR * H, wp, (int64_t)S * H * H, w.hh1, S, R, H, H, st, K_TC_FWD))) return rc;
-      { LaunchScope _ls(K_NORM_FWD, st);
-        if (H == 128) nrm::ln_fwd_kernel<128><<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.hh1, rows, params, P, L.ln1_scale, L.ln1_bias, w.xhat1, w.rstd1, w.hh1, L.d1_b);
-        else nrm::ln_fwd_kernel<256><<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.hh1, rows, params, P, L.ln1_scale, L.ln1_bias, w.xhat1, w.rstd1, w.hh1, L.d1_b); }
-      if ((rc = run_row_bwd(H, true, rbg, A, st, w.hh1, w.xhat1, w.rstd1, nullptr, w.dzl, nullptr, zp, zp + RR * H, gscale, params, grads, P, L.ln1_scale, L.ln1_bias, L.d1_b, L.head_w, L.head_b,
-                            gather, action, target, tr_rows_per_seed, loss_sum, qsa_sum, w.rb_part, R))) return rc;
-      if ((rc = tc16_mm_wgrad(hp, RR * H, zp, RR * H, grads + L.d1_w, P, S, R, H, H, 1.0f / gscale, w.wg_part, st))) return rc;
-      if ((rc = tc16_mm_dgrad(zp, RR * H, wp, (int64_t)S * H * H, w.h0, w.dh0, S, R, H, H, 1.0f / gscale, st))) return rc;
-      if ((rc = run_row_bwd(H, false, rbg, A, st, nullptr, w.xhat0, w.rstd0, w.dh0, w.dh0, nullptr, nullptr, nullptr, 1.0f, params, grads, P, L.ln0_scale, L.ln0_bias, L.d0_b, 0, 0,
-                            nullptr, nullptr, nullptr, 0, nullptr, nullptr, w.rb_part, R))) return rc;
-      run_wgrad_first(w.xg, w.dh0, grads, P, L.d0_w, S, R, D, H, w.rb_part, w.wg_part, st);
-    } else if (d->layers == 2) {
-      launch_dense<1>(H, dim3(cdiv(rows, BM), S), st, w.h0, rows * H, H, params, P, L.d1_w, L.d1_b, L.ln1_scale,
-                      L.ln1_bias, 0, 0, A, w.hh1, w.xhat1, w.rstd1, nullptr, R, H);
-      if ((rc = run_row_bwd(H, true, rbg, A, st, w.hh1, w.xhat1, w.rstd1, nullptr, w.dzl, nullptr, nullptr, nullptr, 1.0f, params, grads, P, L.ln1_scale, L.ln1_bias, L.d1_b, L.head_w, L.head_b,
-                            gather, action, target, tr_rows_per_seed, loss_sum, qsa_sum, w.rb_part, R))) return rc;
-      const int tiles = (H / 128) * (H / 128);
-      const int splits = wgrad_splits(tiles, S, R);
-      run_wgrad_ffma(w.h0, rows * H, H, w.dzl, rows * H, H, grads, P, L.d1_w, R, H, S, splits, w.wg_part, st);
-      { LaunchScope _ls(K_DGRAD, st); dgrad_kernel<<<dim3(cdiv(rows, 128), H / 128, S), GT, 0, st>>>(w.dzl, rows * H, H, params, P, L.d1_w, w.h0,
-                                                                     w.dh0, rows * H, R, H); }
-      if ((rc = run_row_bwd(H, false, rbg, A, st, nullptr, w.xhat0, w.rstd0, w.dh0, w.dh0, nullptr, nullptr, nullptr, 1.0f, params, grads, P, L.ln0_scale, L.ln0_bias, L.d0_b, 0, 0,
-                            nullptr, nullptr, nullptr, 0, nullptr, nullptr, w.rb_part, R))) return rc;
-      run_wgrad_first(w.xg, w.dh0, grads, P, L.d0_w, S, R, D, H, w.rb_part, w.wg_part, st);
-    } else {
-      if ((rc = run_row_bwd(H, true, rbg, A, st, w.h0, w.xhat0, w.rstd0, nullptr, w.dzl, nullptr, nullptr, nullptr, 1.0f, params, grads, P, L.ln0_scale, L.ln0_bias, L.d0_b, L.head_w, L.head_b,
-                            gather, action, target, tr_rows_per_seed, loss_sum, qsa_sum, w.rb_part, R))) return rc;
-      run_wgrad_first(w.xg, w.dzl, grads, P, L.d0_w, S, R, D, H, w.rb_part, w.wg_part, st);
+    const dim3 grid(cdiv(rows, BM), S);
+    const int last = d->layers - 1;
+    const bool tcl = mlp_hidden_tc(H);
+    const int64_t RR = (int64_t)S * rows;
+    // ---- forward, keeping every layer's h, xhat and rstd
+    if ((rc = dense_ln_fwd<1>(H, grid, st, w.xg, rows * D, D, params, P, dense_off(L, H, 0), 0, 0, A, w.h[0], w.xhat[0], w.rstd[0],
+                    nullptr, R, D))) return rc;
+    for (int l = 1; l <= last; ++l) {
+      if (tcl) {
+        if ((rc = mlp_hidden_tc_fwd(w, L, params, P, H, l, S, R, w.xhat[l], w.rstd[l], K_TC_FWD, st))) return rc;
+      } else {
+        if ((rc = dense_ln_fwd<1>(H, grid, st, w.h[l - 1], rows * H, H, params, P, dense_off(L, H, l), 0, 0, A, w.h[l], w.xhat[l],
+                        w.rstd[l], nullptr, R, H))) return rc;
+      }
     }
+    // ---- backward, last layer first.  For l >= 1, row_bwd turns dh_l (the head's, or dh0 from the layer above) into
+    // dz_l: fp16 planes pre-scaled by gscale for the wgmma layers, fp32 dzl otherwise; then dW_l and dh_{l-1} (into
+    // dh0, ReLU-masked by h_{l-1}).  Layer 0's dz is fp32 (in place in dh0, or dzl when it is the only layer).
+    const dim3 rbg(conv_mma_ctas(S, R, 4), S);
+    __half* zp = reinterpret_cast<__half*>(w.m16_dz);
+    const float gscale = grad_scale(rows);
+    for (int l = last; l >= 1; --l) {
+      const DenseOff o = dense_off(L, H, l);
+      const bool head = l == last;
+      if ((rc = run_row_bwd(H, head, rbg, A, st, w.h[l], w.xhat[l], w.rstd[l], head ? nullptr : w.dh0, w.dzl, nullptr,
+                            tcl ? zp : nullptr, tcl ? zp + RR * H : nullptr, tcl ? gscale : 1.0f, params, grads, P, o.g,
+                            o.bi, o.b, head ? L.head_w : 0, head ? L.head_b : 0, head ? gather : nullptr,
+                            head ? action : nullptr, head ? target : nullptr, head ? tr_rows_per_seed : 0,
+                            head ? loss_sum : nullptr, head ? qsa_sum : nullptr, w.rb_part, R))) return rc;
+      if (tcl) {
+        __half* hp = mlp_h_planes(w, RR, H, l);
+        __half* wp = mlp_w_planes(w, S, H, l);
+        if ((rc = tc16_mm_wgrad(hp, RR * H, zp, RR * H, grads + o.w, P, S, R, H, H, 1.0f / gscale, w.wg_part, st))) return rc;
+        if ((rc = tc16_mm_dgrad(zp, RR * H, wp, (int64_t)S * H * H, w.h[l - 1], w.dh0, S, R, H, H, 1.0f / gscale, st))) return rc;
+      } else {
+        run_wgrad_ffma(w.h[l - 1], rows * H, H, w.dzl, rows * H, H, grads, P, o.w, R, H, S,
+                       wgrad_splits(ffma_tiles(H, H), S, R), w.wg_part, st);
+        launch_dgrad(w.dzl, rows * H, H, params, P, o.w, w.h[l - 1], w.dh0, rows * H, R, H, 0, S, st);
+      }
+    }
+    const DenseOff o0 = dense_off(L, H, 0);
+    float* dz0 = last == 0 ? w.dzl : w.dh0;
+    const bool head = last == 0;
+    if ((rc = run_row_bwd(H, head, rbg, A, st, w.h[0], w.xhat[0], w.rstd[0], head ? nullptr : w.dh0, dz0, nullptr, nullptr,
+                          nullptr, 1.0f, params, grads, P, o0.g, o0.bi, o0.b, head ? L.head_w : 0, head ? L.head_b : 0,
+                          head ? gather : nullptr, head ? action : nullptr, head ? target : nullptr,
+                          head ? tr_rows_per_seed : 0, head ? loss_sum : nullptr, head ? qsa_sum : nullptr, w.rb_part, R)))
+      return rc;
+    run_wgrad_first(w.xg, dz0, grads, P, o0.w, S, R, D, H, w.rb_part, w.wg_part, st);
   }
   return check_launch("pqn_qnet_loss_grad");
 }

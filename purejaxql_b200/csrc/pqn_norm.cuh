@@ -25,7 +25,7 @@ constexpr int RED_BLOCKS = 64;   // row chunks per seed of the two-stage reducti
 // ---------------------------------------------------------------------------------------------------------------
 // two-stage per-channel reduction over [S][rows][ncols] (channel = col % G):  out[s][0][g] = sum A,
 // out[s][1][g] = sum A*B.   A == B gives (sum x, sum x^2); (dy, xhat) gives (d beta, d gamma); (dz, dz)[0] = d bias.
-// Requires 256 % G == 0 or G == ncols <= 256 handled by the generic path below.
+// Requires 256 % G == 0, G == 512 (two channels per thread), or G == ncols <= 16 (the generic path below).
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) colsum2_partial_kernel(const float* __restrict__ A, const float* __restrict__ B,
                                                               int rows, int ncols, int G, float* __restrict__ part) {
@@ -52,6 +52,17 @@ __global__ void __launch_bounds__(256) colsum2_partial_kernel(const float* __res
       float* o = part + (((int64_t)seed * nb + b) * 2) * G;
       o[t] = v0; o[G + t] = v1;
     }
+  } else if (G == 512) {
+    // 512 channels (ncols % 512 == 0): thread t owns channels t and t + 256 of every 512-wide row segment
+    const int64_t e0 = (int64_t)r0 * ncols, e1 = (int64_t)r1 * ncols;
+    float s2 = 0.f, ss2 = 0.f;
+    for (int64_t e = e0 + t; e < e1; e += 512) {
+      const float x = a[e], y = a[e + 256];
+      s += x; ss = fmaf(x, bb[e], ss);
+      s2 += y; ss2 = fmaf(y, bb[e + 256], ss2);
+    }
+    float* o = part + (((int64_t)seed * nb + b) * 2) * G;
+    o[t] = s; o[256 + t] = s2; o[G + t] = ss; o[G + 256 + t] = ss2;
   } else {
     // small G that does not divide 256 (MLP input features, ncols == G <= 16): thread = row, G register accumulators,
     // then a fixed-order tree per channel (warp shuffles, warps in order)
@@ -157,8 +168,8 @@ __global__ void norm_elem_fwd_kernel(const float* __restrict__ Z, int64_t n_per_
   H[(int64_t)seed * n_per_seed + i] = MODE == 0 ? fmaxf(y, 0.f) : y;
 }
 
-// LayerNorm over groups of G consecutive values + ReLU: one warp per group for G >= 128 (lane-strided), one thread
-// per group for G == 16.  rstd[S][groups]
+// LayerNorm over groups of G consecutive values + ReLU: one warp per group for G in {64, 128, 256, 512} (lane-strided),
+// one thread per group for G == 16.  rstd[S][groups]
 template <int G>
 __global__ void ln_fwd_kernel(const float* Z, int64_t groups_per_seed, const float* __restrict__ params,
                               int64_t P, int64_t off_g, int64_t off_b, float* XH, float* RS, float* H,
@@ -299,7 +310,7 @@ __global__ void relu_mask_kernel(const float* DY, const float* __restrict__ Hh, 
 // Q head: q = h @ Wh + bh (forward), and its loss backward:
 //   dy[row][n] = dq_row * Wh[n][a_row] * (h[row][n] > 0)       dq_row = (q_sa - target) / rows
 //   per-block partials of loss, mean q_sa, d bh[A], d Wh[N][A]  ->  head_bwd_final_kernel adds them in order.
-// One thread per feature n (N <= 256), the block walks its chunk of rows.
+// One thread per feature n (blockDim = max(N, 256)), the block walks its chunk of rows.
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void head_fwd_kernel(const float* __restrict__ Hh, int rows, int N, const float* __restrict__ params,
                                 int64_t P, int64_t off_w, int64_t off_b, int A, float* __restrict__ Q) {
@@ -318,7 +329,7 @@ __global__ void head_fwd_kernel(const float* __restrict__ Hh, int rows, int N, c
 }
 
 constexpr int HEAD_MAX_A = 32;
-__global__ void __launch_bounds__(256) head_bwd_kernel(
+__global__ void __launch_bounds__(512) head_bwd_kernel(
     const float* __restrict__ Hh, const float* __restrict__ Q, int rows, int N, const float* __restrict__ params,
     int64_t P, int64_t off_w, int A, const int32_t* __restrict__ gather, const int32_t* __restrict__ action,
     const float* __restrict__ target, int64_t tr_rows_per_seed, float* __restrict__ DY, float* __restrict__ part) {
@@ -657,19 +668,25 @@ __global__ void in_xhat_kernel(const float* __restrict__ X, int64_t n_per_seed, 
 // host side
 // ---------------------------------------------------------------------------------------------------------------
 struct NormWs {
-  // shared small buffers
-  float *part, *sums, *dg, *mr[3], *aff, *weff, *beff, *cntp, *q;
+  // shared small buffers; mr[l]: (mean, rstd) of hidden norm l, mr_in: of the MLP's input BatchNorm
+  float *part, *sums, *dg, *mr[PQN_MAX_LAYERS], *mr_in, *aff, *weff, *beff, *cntp, *q;
   float* wgp;   // per-split partials of the FFMA weight gradient (run_wgrad_ffma)
   // CNN
   float *z1, *xh1, *h1, *rs1, *z2, *xh2, *h2, *rs2, *d2, *d1;
   // MLP
-  float *xg, *xn, *xhin, *dxn, *z[2], *xh[2], *h[2], *rs[2], *d[2];
+  float *xg, *xn, *xhin, *dxn, *z[PQN_MAX_LAYERS], *xh[PQN_MAX_LAYERS], *h[PQN_MAX_LAYERS], *rs[PQN_MAX_LAYERS],
+      *d[PQN_MAX_LAYERS];
 };
+
+// channels per seed of the (sum, sum of squares) / (mean, rstd) tables: every per-channel reduction of the network
+static int64_t chan_floats(const pqn_net_desc_t* d) {
+  return 2 * (int64_t)(d->kind != PQN_NET_MINATAR_CNN && d->hidden > 256 ? d->hidden : 256);
+}
 
 static int64_t part_floats(const pqn_net_desc_t* d) {
   const int A = d->num_actions;
   const int N = d->kind == PQN_NET_MINATAR_CNN ? HID_CNN : d->hidden;
-  int64_t m = 2 * 256;
+  int64_t m = chan_floats(d);
   if (2 + A + (int64_t)N * A > m) m = 2 + A + (int64_t)N * A;
   if (d->kind == PQN_NET_MINATAR_CNN && 9 * d->in_c * CONV_O > m) m = 9 * d->in_c * CONV_O;
   return m * RED_BLOCKS;
@@ -688,9 +705,11 @@ static int64_t carve_norm(const pqn_net_desc_t* d, int32_t S, int64_t rows, char
   const int A = d->num_actions;
   ww->part = take((int64_t)S * part_floats(d));
   ww->wgp = take(wgrad_split_tiles() * 128 * 128);
-  ww->sums = take((int64_t)S * 2 * 256);
-  ww->dg = take((int64_t)S * 2 * 256);
-  for (int i = 0; i < 3; ++i) ww->mr[i] = take((int64_t)S * 2 * 256);
+  const int nl = d->kind != PQN_NET_MINATAR_CNN && d->layers > 2 ? d->layers : 2;   // hidden norms (CNN: 2)
+  ww->sums = take((int64_t)S * chan_floats(d));
+  ww->dg = take((int64_t)S * chan_floats(d));
+  ww->mr_in = take((int64_t)S * chan_floats(d));
+  for (int l = 0; l < nl; ++l) ww->mr[l] = take((int64_t)S * chan_floats(d));
   ww->q = take(R * A);
   if (d->kind == PQN_NET_MINATAR_CNN) {
     const int C = d->in_c;
@@ -704,7 +723,7 @@ static int64_t carve_norm(const pqn_net_desc_t* d, int32_t S, int64_t rows, char
   } else {
     const int D = d->in_c, H = d->hidden;
     ww->xg = take(R * D); ww->xn = take(R * D); ww->xhin = take(R * D); ww->dxn = take(R * D);
-    for (int l = 0; l < 2; ++l) {
+    for (int l = 0; l < nl; ++l) {
       ww->z[l] = take(R * H); ww->xh[l] = take(R * H); ww->h[l] = take(R * H); ww->rs[l] = take(R); ww->d[l] = take(R * H);
     }
   }
@@ -721,10 +740,11 @@ static int64_t stats_floats(const pqn_net_desc_t* d) {
   }
   return n;
 }
-static int64_t stats_off(const pqn_net_desc_t* d, int layer /*0,1*/) {
-  int64_t n = 2 * d->in_c;
-  if (layer == 0) return n;
-  return n + (d->kind == PQN_NET_MINATAR_CNN ? 2 * CONV_O : 2 * (int64_t)d->hidden);
+// offset of hidden BatchNorm `layer` (CNN: 0 or 1; MLP: 0 .. NUM_LAYERS-1) in the batch_stats block
+static int64_t stats_off(const pqn_net_desc_t* d, int layer) {
+  const int64_t n = 2 * d->in_c;
+  if (d->kind == PQN_NET_MINATAR_CNN) return layer == 0 ? n : n + 2 * CONV_O;
+  return n + 2 * (int64_t)d->hidden * layer;
 }
 
 static inline void colsum2(const float* A, const float* B, int S, int rows, int ncols, int G, NormWs& w, float* out,
@@ -743,6 +763,8 @@ static int norm_layer_fwd(int norm, const float* Z, int S, int rows, int ncols, 
     const int64_t groups = n / G;
     LaunchScope _ls(K_NORM_FWD, st);
     if (G == 16) ln_fwd_kernel<16><<<dim3(cdiv(groups, 256), S), 256, 0, st>>>(Z, groups, params, P, off_g, off_b, XH, RS, H);
+    else if (G == 64) ln_fwd_kernel<64><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(Z, groups, params, P, off_g, off_b, XH, RS, H);
+    else if (G == 512) ln_fwd_kernel<512><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(Z, groups, params, P, off_g, off_b, XH, RS, H);
     else if (G == 128) ln_fwd_kernel<128><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(Z, groups, params, P, off_g, off_b, XH, RS, H);
     else if (G == 256) ln_fwd_kernel<256><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(Z, groups, params, P, off_g, off_b, XH, RS, H);
     else return set_error(PQN_E_UNSUPPORTED, "LayerNorm width %d", G);
@@ -768,8 +790,11 @@ static int norm_layer_bwd(int norm, float* D, const float* XH, const float* RS, 
     const int64_t groups = n / G;
     LaunchScope _ls(K_NORM_BWD, st);
     if (G == 16) ln_bwd_kernel<16><<<dim3(cdiv(groups, 256), S), 256, 0, st>>>(D, XH, RS, groups, params, P, off_g, D);
+    else if (G == 64) ln_bwd_kernel<64><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(D, XH, RS, groups, params, P, off_g, D);
     else if (G == 128) ln_bwd_kernel<128><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(D, XH, RS, groups, params, P, off_g, D);
-    else ln_bwd_kernel<256><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(D, XH, RS, groups, params, P, off_g, D);
+    else if (G == 256) ln_bwd_kernel<256><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(D, XH, RS, groups, params, P, off_g, D);
+    else if (G == 512) ln_bwd_kernel<512><<<dim3(cdiv(groups, 8), S), 256, 0, st>>>(D, XH, RS, groups, params, P, off_g, D);
+    else return set_error(PQN_E_UNSUPPORTED, "LayerNorm width %d", G);
   } else if (norm == NORM_BN) {
     LaunchScope _ls(K_NORM_BWD, st);
     bn_bwd_kernel<<<dim3(cdiv(n, 256), S), 256, 0, st>>>(D, XH, n, ncols, G, mr, w.dg, (float)(1.0 / ((double)rows * (ncols / G))),
@@ -830,8 +855,8 @@ static int norm_forward(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
     float* run1 = norm == NORM_BN ? batch_stats + stats_off(d, 1) : nullptr;
     if ((rc = norm_layer_fwd(norm, w.z1, S, rows, FLAT_CNN, CONV_O, params, P, L.ln0_scale, L.ln0_bias, run0, sstride, train,
                              w, w.mr[0], norm == NORM_NONE ? nullptr : w.xh1, w.rs1, w.h1, st))) return rc;
-    launch_dense<3>(128, dim3(cdiv(rows, 128), S), st, w.h1, (int64_t)rows * FLAT_CNN, FLAT_CNN, params, P, L.d0_w, L.d0_b,
-                    0, 0, 0, 0, A, w.z2, nullptr, nullptr, nullptr, rows, FLAT_CNN);
+    if ((rc = launch_dense<3>(128, dim3(cdiv(rows, 128), S), st, w.h1, (int64_t)rows * FLAT_CNN, FLAT_CNN, params, P, L.d0_w, L.d0_b,
+                    0, 0, 0, 0, A, w.z2, nullptr, nullptr, nullptr, rows, FLAT_CNN))) return rc;
     if ((rc = norm_layer_fwd(norm, w.z2, S, rows, HID_CNN, HID_CNN, params, P, L.ln1_scale, L.ln1_bias, run1, sstride, train,
                              w, w.mr[1], norm == NORM_NONE ? nullptr : w.xh2, w.rs2, w.h2, st))) return rc;
     { LaunchScope _ls(K_NORM_FWD, st); head_fwd_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.h2, rows, HID_CNN, params, P, L.head_w, L.head_b, A, q); }
@@ -854,23 +879,22 @@ static int norm_forward(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
         if (bn_sums) cudaMemcpyAsync(bn_sums, w.sums, (size_t)S * 2 * D * sizeof(float), cudaMemcpyDeviceToDevice, st);
       }
       // running statistics of the input BatchNorm are updated by pqn_bn_stats_update (engine) from bn_sums
-      { LaunchScope _ls(K_NORM_FWD, st); bn_prepare_kernel<<<S, 256, 0, st>>>(w.sums, (float)rows, train ? nullptr : batch_stats, sstride, D, train, 0.99f, w.mr[2]); }
+      { LaunchScope _ls(K_NORM_FWD, st); bn_prepare_kernel<<<S, 256, 0, st>>>(w.sums, (float)rows, train ? nullptr : batch_stats, sstride, D, train, 0.99f, w.mr_in); }
     }
     const float* xin = x;
     if (d->norm_input) {
-      { LaunchScope _ls(K_NORM_FWD, st); norm_elem_fwd_kernel<2><<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(x, (int64_t)rows * D, D, D, w.mr[2], params, P, L.bn_scale, L.bn_bias, nullptr, w.xn); }
+      { LaunchScope _ls(K_NORM_FWD, st); norm_elem_fwd_kernel<2><<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(x, (int64_t)rows * D, D, D, w.mr_in, params, P, L.bn_scale, L.bn_bias, nullptr, w.xn); }
       xin = w.xn;
     }
     const int BM = (H == 128) ? 128 : 64;
-    const int64_t offw[2] = {L.d0_w, L.d1_w}, offb[2] = {L.d0_b, L.d1_b}, offg[2] = {L.ln0_scale, L.ln1_scale},
-                  offbi[2] = {L.ln0_bias, L.ln1_bias};
     const float* cur = xin;
     int kin = D;
     for (int l = 0; l < d->layers; ++l) {
-      launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, (int64_t)rows * kin, kin, params, P, offw[l], offb[l], 0, 0, 0, 0, A,
-                      w.z[l], nullptr, nullptr, nullptr, rows, kin);
+      const DenseOff o = dense_off(L, H, l);
+      if ((rc = launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, (int64_t)rows * kin, kin, params, P, o.w, o.b, 0, 0, 0, 0, A,
+                      w.z[l], nullptr, nullptr, nullptr, rows, kin))) return rc;
       float* run = norm == NORM_BN ? batch_stats + stats_off(d, l) : nullptr;
-      if ((rc = norm_layer_fwd(norm, w.z[l], S, rows, H, H, params, P, offg[l], offbi[l], run, sstride, train, w, w.mr[l],
+      if ((rc = norm_layer_fwd(norm, w.z[l], S, rows, H, H, params, P, o.g, o.bi, run, sstride, train, w, w.mr[l],
                                norm == NORM_NONE ? nullptr : w.xh[l], w.rs[l], w.h[l], st))) return rc;
       cur = w.h[l];
       kin = H;
@@ -893,37 +917,34 @@ static int norm_loss_grad(const pqn_net_desc_t* d, const pqn_net_layout_t& L, co
   const int last = cnn ? 1 : d->layers - 1;
   float* hl = cnn ? w.h2 : w.h[last];
   float* dl = cnn ? w.d2 : w.d[last];
-  { LaunchScope _ls(K_ROW_BWD, st); head_bwd_kernel<<<dim3(RED_BLOCKS, S), 256, 0, st>>>(hl, w.q, rows, N, params, P, L.head_w, A, gather, action, target, trps, dl, w.part); }
+  { LaunchScope _ls(K_ROW_BWD, st); head_bwd_kernel<<<dim3(RED_BLOCKS, S), N > 256 ? N : 256, 0, st>>>(hl, w.q, rows, N, params, P, L.head_w, A, gather, action, target, trps, dl, w.part); }
   { LaunchScope _ls(K_GRAD_FINAL, st); head_bwd_final_kernel<<<S, 256, 0, st>>>(w.part, RED_BLOCKS, N, A, grads, P, L.head_w, L.head_b, loss_sum, qsa_sum); }
   if (cnn) {
     if ((rc = norm_layer_bwd(norm, w.d2, w.xh2, w.rs2, S, rows, HID_CNN, HID_CNN, params, grads, P, L.ln1_scale, L.ln1_bias,
                              L.d0_b, w, w.mr[1], st))) return rc;
     const int splits = wgrad_splits(FLAT_CNN / 128, S, rows);
     run_wgrad_ffma(w.h1, (int64_t)rows * FLAT_CNN, FLAT_CNN, w.d2, (int64_t)rows * HID_CNN, HID_CNN, grads, P, L.d0_w, rows, FLAT_CNN, S, splits, w.wgp, st);
-    { LaunchScope _ls(K_DGRAD, st); dgrad_kernel<<<dim3(cdiv(rows, 128), FLAT_CNN / 128, S), GT, 0, st>>>(w.d2, (int64_t)rows * HID_CNN, HID_CNN, params, P, L.d0_w, w.h1, w.d1, (int64_t)rows * FLAT_CNN, rows, FLAT_CNN); }
+    launch_dgrad(w.d2, (int64_t)rows * HID_CNN, HID_CNN, params, P, L.d0_w, w.h1, w.d1, (int64_t)rows * FLAT_CNN, rows, FLAT_CNN, 0, S, st);
     if ((rc = norm_layer_bwd(norm, w.d1, w.xh1, w.rs1, S, rows, FLAT_CNN, CONV_O, params, grads, P, L.ln0_scale, L.ln0_bias,
                              -1, w, w.mr[0], st))) return rc;
     PQN_C_DISPATCH(d->in_c, rc = cnn_norm_conv_bwd<CC>(d, L, params, (const uint32_t*)obs, orps, gather, S, rows, grads, w, st));
     if (rc) return rc;
   } else {
     const int D = d->in_c, H = d->hidden;
-    const int64_t offw[2] = {L.d0_w, L.d1_w}, offb[2] = {L.d0_b, L.d1_b}, offg[2] = {L.ln0_scale, L.ln1_scale},
-                  offbi[2] = {L.ln0_bias, L.ln1_bias};
     const float* xin = d->norm_input ? w.xn : w.xg;
     for (int l = last; l >= 0; --l) {
-      if ((rc = norm_layer_bwd(norm, w.d[l], w.xh[l], w.rs[l], S, rows, H, H, params, grads, P, offg[l], offbi[l], offb[l], w,
+      const DenseOff o = dense_off(L, H, l);
+      if ((rc = norm_layer_bwd(norm, w.d[l], w.xh[l], w.rs[l], S, rows, H, H, params, grads, P, o.g, o.bi, o.b, w,
                                w.mr[l], st))) return rc;
       const float* xprev = l == 0 ? xin : w.h[l - 1];
       const int kin = l == 0 ? D : H;
-      const int sp = wgrad_splits((kin + 127) / 128 * (H / 128), S, rows);
-      run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, w.d[l], (int64_t)rows * H, H, grads, P, offw[l], rows, kin, S, sp, w.wgp, st);
-      if (l > 0) {
-        { LaunchScope _ls(K_DGRAD, st); dgrad_kernel<<<dim3(cdiv(rows, 128), H / 128, S), GT, 0, st>>>(w.d[l], (int64_t)rows * H, H, params, P, offw[l], w.h[l - 1], w.d[l - 1], (int64_t)rows * H, rows, H); }
-      }
+      const int sp = wgrad_splits(ffma_tiles(kin, H), S, rows);
+      run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, w.d[l], (int64_t)rows * H, H, grads, P, o.w, rows, kin, S, sp, w.wgp, st);
+      if (l > 0) launch_dgrad(w.d[l], (int64_t)rows * H, H, params, P, o.w, w.h[l - 1], w.d[l - 1], (int64_t)rows * H, rows, H, 0, S, st);
     }
     if (d->norm_input) {   // the input BatchNorm is on the path: gradients of its scale / bias
       { LaunchScope _ls(K_DGRAD, st); dgrad_small_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.d[0], rows, H, params, P, L.d0_w, D, w.dxn); }
-      { LaunchScope _ls(K_NORM_BWD, st); in_xhat_kernel<<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(w.xg, (int64_t)rows * D, D, w.mr[2], w.xhin); }
+      { LaunchScope _ls(K_NORM_BWD, st); in_xhat_kernel<<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(w.xg, (int64_t)rows * D, D, w.mr_in, w.xhin); }
       colsum2(w.dxn, w.xhin, S, rows, D, D, w, w.dg, grads, P, L.bn_bias, L.bn_scale, st);
     }
   }

@@ -123,14 +123,17 @@ __global__ void bn_update_kernel(float* __restrict__ batch_stats, float* __restr
 // Draws are counter-based (threefry block (element, attempt) under a per-tensor key derived from the seed key)
 // with Box-Muller + rejection: deterministic in the seed key, same distribution as flax, not the same draws
 // (flax folds module paths into the key).
+// Entry t < MAX_INIT draws under split(seed key, MAX_INIT)[t]; the split's width enters every value, so it stays 16 and
+// the entries past it (deep networks only) draw under split(split(seed key, 2)[1], MAX_INIT)[t - MAX_INIT].
 struct InitEntry {
   long long off, n;
   float std;   // > 0: truncated normal * std ; 0: zeros ; < 0: ones
 };
 constexpr int MAX_INIT = 16;
+constexpr int MAX_INIT_ENTRIES = 2 * MAX_INIT;
 struct InitTable {
   int count;
-  InitEntry e[MAX_INIT];
+  InitEntry e[MAX_INIT_ENTRIES];
 };
 
 __global__ void net_init_kernel(const uint32_t* __restrict__ keys, float* __restrict__ params, int64_t P, InitTable tab) {
@@ -138,7 +141,8 @@ __global__ void net_init_kernel(const uint32_t* __restrict__ keys, float* __rest
   const Key sk{keys[2 * seed], keys[2 * seed + 1]};
   for (int t = 0; t < tab.count; ++t) {
     const InitEntry en = tab.e[t];
-    const Key kt = split_at(sk, (uint32_t)MAX_INIT, (uint32_t)t, 0);
+    const Key kt = t < MAX_INIT ? split_at(sk, (uint32_t)MAX_INIT, (uint32_t)t, 0)
+                                : split_at(split_at(sk, 2u, 1u, 0), (uint32_t)MAX_INIT, (uint32_t)(t - MAX_INIT), 0);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < en.n; i += (long long)gridDim.x * blockDim.x) {
       float v;
       if (en.std == 0.f) v = 0.f;
@@ -189,13 +193,15 @@ int pqn_net_init(const pqn_net_desc_t* d, const uint32_t* keys, float* params, i
   if (!keys || !params || S <= 0 || S > 65535) return set_error(PQN_E_INVALID, "pqn_net_init: bad argument");
   InitTable tab;
   tab.count = 0;
+  bool overflow = false;
   auto add = [&](int64_t off, int64_t n, float std) {
-    if (off >= 0 && tab.count < MAX_INIT) tab.e[tab.count++] = InitEntry{(long long)off, (long long)n, std};
+    if (off < 0) return;
+    if (tab.count == MAX_INIT_ENTRIES) { overflow = true; return; }
+    tab.e[tab.count++] = InitEntry{(long long)off, (long long)n, std};
   };
   auto tn = [](double scale, double fan_in) { return (float)(sqrt(scale / fan_in) / 0.87962566103423978); };
   const int A = d->num_actions;
   cudaStream_t st = (cudaStream_t)stream;
-  if (cudaMemsetAsync(params, 0, (size_t)S * L.total * sizeof(float), st) != cudaSuccess) return check_launch("pqn_net_init(memset)");
   if (d->kind == PQN_NET_MINATAR_CNN) {
     const int C = d->in_c;
     add(L.bn_scale, C, -1.f);
@@ -209,9 +215,11 @@ int pqn_net_init(const pqn_net_desc_t* d, const uint32_t* keys, float* params, i
     add(L.bn_scale, D, -1.f);
     add(L.d0_w, (int64_t)D * H, tn(1.0, D));
     add(L.ln0_scale, H, -1.f);
-    if (d->layers == 2) {
-      add(L.d1_w, (int64_t)H * H, tn(1.0, H));
-      add(L.ln1_scale, H, -1.f);
+    for (int l = 1; l < d->layers; ++l) {
+      int64_t o[4];
+      if ((rc = pqn_net_dense_layer(d, l, o))) return rc;
+      add(o[0], (int64_t)H * H, tn(1.0, H));
+      add(o[2], H, -1.f);
     }
     if (d->kind == PQN_NET_RNN) {   // GRUCell input denses: lecun_normal over fan_in = H + A; the orthogonal recurrent
       add(L.gru_ir_w, (int64_t)(H + A) * H, tn(1.0, H + A));   // kernels are drawn on the host (networks.py)
@@ -220,6 +228,8 @@ int pqn_net_init(const pqn_net_desc_t* d, const uint32_t* keys, float* params, i
     }
     add(L.head_w, (int64_t)H * A, tn(1.0, H));
   }
+  if (overflow) return set_error(PQN_E_UNSUPPORTED, "pqn_net_init: more than %d initialised tensors", MAX_INIT_ENTRIES);
+  if (cudaMemsetAsync(params, 0, (size_t)S * L.total * sizeof(float), st) != cudaSuccess) return check_launch("pqn_net_init(memset)");
   { LaunchScope _ls(K_NET_INIT, st); net_init_kernel<<<dim3(64, S), 256, 0, st>>>(keys, params, L.total, tab); }
   return check_launch("pqn_net_init");
 }

@@ -298,7 +298,7 @@ __global__ void __launch_bounds__(H) rnn_onehot_grad_kernel(const float* __restr
 // host side
 // ---------------------------------------------------------------------------------------------------------------
 struct RnnWs {
-  float *h[2], *xh[2], *rs[2], *ai, *y, *h0, *rg, *zg, *ng, *hn, *q, *dq, *dy, *da, *dhn, *dx, *dhl, *wt, *part, *sums, *rbp, *wgp;
+  float *h[PQN_MAX_LAYERS], *xh[PQN_MAX_LAYERS], *rs[PQN_MAX_LAYERS], *ai, *y, *h0, *rg, *zg, *ng, *hn, *q, *dq, *dy, *da, *dhn, *dx, *dhl, *wt, *part, *sums, *rbp, *wgp;
 };
 
 static int64_t carve_rnn(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* base, RnnWs* w) {
@@ -312,15 +312,17 @@ static int64_t carve_rnn(const pqn_net_desc_t* d, int32_t S, int64_t rows, char*
   RnnWs* ww = w ? w : &tmp;
   const int64_t R = (int64_t)S * rows;
   const int H = d->hidden, A = d->num_actions;
-  for (int l = 0; l < 2; ++l) { ww->h[l] = take(R * H); ww->xh[l] = take(R * H); ww->rs[l] = take(R); }
+  const int nl = d->layers > 2 ? d->layers : 2;
+  for (int l = 0; l < nl; ++l) { ww->h[l] = take(R * H); ww->xh[l] = take(R * H); ww->rs[l] = take(R); }
   ww->ai = take(3 * R * H);
   ww->y = take(R * H); ww->h0 = take(R * H); ww->rg = take(R * H); ww->zg = take(R * H); ww->ng = take(R * H);
   ww->hn = take(R * H);
   ww->q = take(R * A); ww->dq = take(R * A);
   ww->dy = take(R * H); ww->da = take(3 * R * H); ww->dhn = take(R * H); ww->dx = take(R * H); ww->dhl = take(R * H);
   ww->wt = take(3 * (int64_t)S * H * H);
-  ww->part = take((int64_t)S * nrm::RED_BLOCKS * (2 * 256 > A + H * A ? 2 * 256 : A + H * A));
-  ww->sums = take((int64_t)S * 2 * 256);
+  const int64_t chan = nrm::chan_floats(d);   // the colsum2 tables of the GRU biases (H channels)
+  ww->part = take((int64_t)S * nrm::RED_BLOCKS * (chan > A + H * A ? chan : A + H * A));
+  ww->sums = take((int64_t)S * chan);
   ww->wgp = take(wgrad_split_tiles() * 128 * 128);   // per-split partials of the FFMA weight gradient
   ww->rbp = take(part_ctas(S) * row_bwd_part_floats(H, A));
   return off;
@@ -334,28 +336,31 @@ static int check_rnn(const pqn_net_desc_t* d, const char* who) {
 }
 
 // trunk (NUM_LAYERS x Dense -> LayerNorm -> ReLU) + input-side gate products over `rows` rows per seed
-static void rnn_trunk(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const float* params, const float* x, int64_t xss,
+static int rnn_trunk(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const float* params, const float* x, int64_t xss,
                       int S, int rows, bool train, RnnWs& w, cudaStream_t st) {
   const int D = d->in_c, H = d->hidden, A = d->num_actions;
   const int64_t P = L.total;
   const int BM = (H == 128) ? 128 : 64;
-  const int64_t offw[2] = {L.d0_w, L.d1_w}, offb[2] = {L.d0_b, L.d1_b}, offg[2] = {L.ln0_scale, L.ln1_scale},
-                offbi[2] = {L.ln0_bias, L.ln1_bias};
   const float* cur = x;
   int64_t css = xss;
   int kin = D;
   for (int l = 0; l < d->layers; ++l) {
-    if (train) launch_dense<1>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, offw[l], offb[l], offg[l], offbi[l], 0, 0,
-                               A, w.h[l], w.xh[l], w.rs[l], nullptr, rows, kin);
-    else launch_dense<0>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, offw[l], offb[l], offg[l], offbi[l], 0, 0, A,
-                         w.h[l], nullptr, nullptr, nullptr, rows, kin);
+    const DenseOff o = dense_off(L, H, l);
+    const int rc = train ? dense_ln_fwd<1>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o, 0, 0, A, w.h[l],
+                                           w.xh[l], w.rs[l], nullptr, rows, kin)
+                         : dense_ln_fwd<0>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o, 0, 0, A, w.h[l],
+                                           nullptr, nullptr, nullptr, rows, kin);
+    if (rc) return rc;
     cur = w.h[l]; css = (int64_t)rows * H; kin = H;
   }
   const int64_t gs = (int64_t)S * rows * H;
   const int64_t iw[3] = {L.gru_ir_w, L.gru_iz_w, L.gru_in_w}, ib[3] = {L.gru_ir_b, L.gru_iz_b, L.gru_in_b};
-  for (int g = 0; g < 3; ++g)
-    launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, css, H, params, P, iw[g], ib[g], 0, 0, 0, 0, A, w.ai + g * gs, nullptr,
-                    nullptr, nullptr, rows, H);
+  for (int g = 0; g < 3; ++g) {
+    const int rc = launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, css, H, params, P, iw[g], ib[g], 0, 0, 0, 0, A,
+                                   w.ai + g * gs, nullptr, nullptr, nullptr, rows, H);
+    if (rc) return rc;
+  }
+  return 0;
 }
 
 template <bool TRAIN>
@@ -366,13 +371,17 @@ static int rnn_scan_fwd(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
   const int64_t gs = (int64_t)S * T * B * H;
   const dim3 grid(cdiv(B, RB), S);
   LaunchScope _ls(K_RNN_SCAN, st);
-  if (H == 128)
-    gru_scan_fwd_kernel<128, TRAIN><<<grid, 128, 0, st>>>(w.ai, gs, la, reset, hs_in, hs_out, params, L.total, L, A, w.y, w.h0,
-                                                         w.rg, w.zg, w.ng, w.hn, T, B);
-  else if (H == 256)
-    gru_scan_fwd_kernel<256, TRAIN><<<grid, 256, 0, st>>>(w.ai, gs, la, reset, hs_in, hs_out, params, L.total, L, A, w.y, w.h0,
-                                                         w.rg, w.zg, w.ng, w.hn, T, B);
-  else return set_error(PQN_E_UNSUPPORTED, "GRU hidden=%d (128 or 256 built)", H);
+#define PQN_GRU_FWD(HH)                                                                                                     \
+  gru_scan_fwd_kernel<HH, TRAIN><<<grid, HH, 0, st>>>(w.ai, gs, la, reset, hs_in, hs_out, params, L.total, L, A, w.y, w.h0, \
+                                                      w.rg, w.zg, w.ng, w.hn, T, B)
+  switch (H) {
+    case 64: PQN_GRU_FWD(64); break;
+    case 128: PQN_GRU_FWD(128); break;
+    case 256: PQN_GRU_FWD(256); break;
+    case 512: PQN_GRU_FWD(512); break;
+    default: return set_error(PQN_E_UNSUPPORTED, "GRU hidden=%d (64, 128, 256 or 512 built)", H);
+  }
+#undef PQN_GRU_FWD
   return 0;
 }
 

@@ -14,6 +14,7 @@ the network has no normalisation parameters at all.
 """
 from __future__ import annotations
 
+import ctypes
 import math
 
 import numpy as np
@@ -70,14 +71,11 @@ class QNetworkSpec:
         else:
             D, H = self.in_c, self.hidden
             e += [(("BatchNorm_0", "scale"), L.bn_scale, (D,), "ones"),
-                  (("BatchNorm_0", "bias"), L.bn_bias, (D,), "zeros"),
-                  (("Dense_0", "kernel"), L.d0_w, (D, H), "lecun"),
-                  (("Dense_0", "bias"), L.d0_b, (H,), "zeros")]
-            e += norm((), 0, L.ln0_scale, L.ln0_bias, H)
-            if self.layers == 2:
-                e += [(("Dense_1", "kernel"), L.d1_w, (H, H), "lecun"),
-                      (("Dense_1", "bias"), L.d1_b, (H,), "zeros")]
-                e += norm((), 1, L.ln1_scale, L.ln1_bias, H)
+                  (("BatchNorm_0", "bias"), L.bn_bias, (D,), "zeros")]
+            for layer, (off_w, off_b, off_s, off_bi) in enumerate(self.dense_layers()):
+                e += [((f"Dense_{layer}", "kernel"), off_w, (D if layer == 0 else H, H), "lecun"),
+                      ((f"Dense_{layer}", "bias"), off_b, (H,), "zeros")]
+                e += norm((), layer, off_s, off_bi, H)
             if self.kind == NET_RNN:
                 # flax.linen.GRUCell: input denses ir/iz/in (bias, lecun_normal), recurrent hr/hz (no bias) and hn
                 # (bias), orthogonal recurrent kernels
@@ -91,6 +89,15 @@ class QNetworkSpec:
             e += [((f"Dense_{self.layers}", "kernel"), L.head_w, (H, A), "lecun"),
                   ((f"Dense_{self.layers}", "bias"), L.head_b, (A,), "zeros")]
         return e
+
+    def dense_layers(self):
+        """(kernel, bias, norm scale, norm bias) offsets of every hidden layer (``pqn_net_dense_layer``; -1: none)."""
+        out = []
+        for layer in range(self.layers):
+            off = (ctypes.c_int64 * 4)()
+            _lib.check(_lib.lib().pqn_net_dense_layer(self.desc, layer, off), "pqn_net_dense_layer")
+            out.append(tuple(int(v) for v in off))
+        return out
 
     # ------------------------------------------------------------------ #
     def stats_entries(self):
