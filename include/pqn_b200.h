@@ -258,6 +258,24 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* desc_host, const float* params, cons
                       const uint8_t* last_done, const int32_t* last_action, const int32_t* action, const float* reward,
                       const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum, int32_t S, int32_t T, int32_t B,
                       float gamma, float lambda, void* workspace, void* stream);
+/* pqn_rnn_step / pqn_rnn_loss_grad take only the default network (norm_type layer_norm, norm_input 0).  These two take
+ * every norm_type x norm_input (:65-76) and the running statistics batch_stats float32[S][pqn_net_stats_floats]
+ * (layout as for pqn_qnet_forward; BatchNorm_0 first, then the hidden BatchNorm_1..L).
+ *  - step_stats: train=False, the running statistics normalise; batch_stats is only read.
+ *  - loss_grad_stats: train=True; every BatchNorm, the input one included (also when its output is discarded), uses
+ *    the statistics of all T*B rows of the window and updates its running statistics in place
+ *    (0.99 old + 0.01 batch, fast biased variance; :330-337,362-369) from the forward at the given params.
+ * batch_stats may be NULL only for the default network; then both give exactly what the entries above give.  With a
+ * non-NULL batch_stats the default network's BatchNorm_0 statistics are updated by loss_grad_stats (its output stays
+ * discarded).  The input BatchNorm is built for in_c <= 16 or in_c dividing 256 (PQN_E_UNSUPPORTED otherwise). */
+int pqn_rnn_step_stats(const pqn_net_desc_t* desc_host, const float* params, const float* batch_stats, float* hs,
+                       const float* obs, int64_t obs_rows_per_seed, const uint8_t* last_done, const int32_t* last_action,
+                       float* q, int32_t S, int32_t E, void* workspace, void* stream);
+int pqn_rnn_loss_grad_stats(const pqn_net_desc_t* desc_host, const float* params, float* batch_stats, const float* hs0,
+                            const float* obs, const uint8_t* last_done, const int32_t* last_action,
+                            const int32_t* action, const float* reward, const uint8_t* done, float* grads,
+                            float* loss_sum, float* qsa_sum, int32_t S, int32_t T, int32_t B, float gamma, float lambda,
+                            void* workspace, void* stream);
 
 /* optax.chain(clip_by_global_norm(max_norm), radam(lr_t)) + apply_updates
  * (pqn_minatar.py:159-162,292).  sched: float32[num_steps][4] per optimizer step

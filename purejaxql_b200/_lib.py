@@ -87,6 +87,11 @@ _SIGS = {
     "pqn_rnn_loss_grad": (c_int, [POINTER(NetDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_float, c_float,
                                   c_void_p, c_void_p]),
+    "pqn_rnn_step_stats": (c_int, [POINTER(NetDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                   c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
+    "pqn_rnn_loss_grad_stats": (c_int, [POINTER(NetDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
+                                        c_int32, c_float, c_float, c_void_p, c_void_p]),
     "pqn_radam_clip_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
                                     c_int64, c_float, c_float, c_float, c_float, c_void_p]),
     "pqn_bn_stats_update": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int64, c_float, c_float, c_void_p]),

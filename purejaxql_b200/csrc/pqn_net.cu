@@ -2991,48 +2991,36 @@ static int mlp_hidden_tc_fwd(const Workspace& w, const pqn_net_layout_t& L, cons
   return 0;
 }
 
-}  // namespace pqn
-
-using namespace pqn;
-
-extern "C" {
-
-int64_t pqn_net_stats_floats(const pqn_net_desc_t* d) {
-  if (check_desc(d, "pqn_net_stats_floats")) return -1;
-  return nrm::stats_floats(d);
-}
-
-int pqn_rnn_step(const pqn_net_desc_t* d, const float* params, float* hs, const float* obs, int64_t obs_rows_per_seed,
-                 const uint8_t* last_done, const int32_t* last_action, float* q, int32_t S, int32_t E, void* workspace,
-                 void* stream) {
-  int rc = check_desc(d, "pqn_rnn_step");
-  if (rc) return rc;
-  if ((rc = rnn::check_rnn(d, "pqn_rnn_step"))) return rc;
+// pqn_rnn_step / pqn_rnn_step_stats after their descriptor checks (batch_stats read-only: train=False)
+static int rnn_step(const pqn_net_desc_t* d, const float* params, const float* batch_stats, float* hs, const float* obs,
+                    int64_t obs_rows_per_seed, const uint8_t* last_done, const int32_t* last_action, float* q, int32_t S,
+                    int32_t E, void* workspace, void* stream, const char* who) {
+  int rc;
   if (!params || !hs || !obs || !last_done || !last_action || !q || !workspace || S <= 0 || E <= 0 || S > 65535)
-    return set_error(PQN_E_INVALID, "pqn_rnn_step: bad argument");
+    return set_error(PQN_E_INVALID, "%s: bad argument", who);
   cudaStream_t st = (cudaStream_t)stream;
   pqn_net_layout_t L;
   make_layout(d, &L);
   rnn::RnnWs w;
   rnn::carve_rnn(d, S, E, (char*)workspace, &w);
-  if ((rc = rnn::rnn_trunk(d, L, params, obs, obs_rows_per_seed * d->in_c, S, E, false, w, st))) return rc;
+  if ((rc = rnn::rnn_trunk(d, L, params, const_cast<float*>(batch_stats), obs, obs_rows_per_seed, S, E, false, w, st)))
+    return rc;
   if ((rc = rnn::rnn_scan_fwd<false>(d, L, params, last_action, last_done, hs, hs, S, 1, E, w, st))) return rc;
   { LaunchScope _ls(K_RNN_MISC, st);
     nrm::head_fwd_kernel<<<dim3(cdiv(E, 8), S), 256, 0, st>>>(w.y, E, d->hidden, params, L.total, L.head_w, L.head_b,
                                                                d->num_actions, q); }
-  return check_launch("pqn_rnn_step");
+  return check_launch(who);
 }
 
-int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float* hs0, const float* obs,
-                      const uint8_t* last_done, const int32_t* last_action, const int32_t* action, const float* reward,
-                      const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum, int32_t S, int32_t T, int32_t B,
-                      float gamma, float lambda, void* workspace, void* stream) {
-  int rc = check_desc(d, "pqn_rnn_loss_grad");
-  if (rc) return rc;
-  if ((rc = rnn::check_rnn(d, "pqn_rnn_loss_grad"))) return rc;
+// pqn_rnn_loss_grad / pqn_rnn_loss_grad_stats after their descriptor checks (batch_stats updated in place)
+static int rnn_loss_grad(const pqn_net_desc_t* d, const float* params, float* batch_stats, const float* hs0,
+                         const float* obs, const uint8_t* last_done, const int32_t* last_action, const int32_t* action,
+                         const float* reward, const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum, int32_t S,
+                         int32_t T, int32_t B, float gamma, float lambda, void* workspace, void* stream, const char* who) {
+  int rc;
   if (!params || !hs0 || !obs || !last_done || !last_action || !action || !reward || !done || !grads || !loss_sum ||
       !qsa_sum || !workspace || S <= 0 || T < 2 || B <= 0 || B > 1024 || S > 65535)
-    return set_error(PQN_E_INVALID, "pqn_rnn_loss_grad: bad argument (T >= 2, B <= 1024)");
+    return set_error(PQN_E_INVALID, "%s: bad argument (T >= 2, B <= 1024)", who);
   cudaStream_t st = (cudaStream_t)stream;
   pqn_net_layout_t L;
   make_layout(d, &L);
@@ -3041,10 +3029,10 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
   rnn::RnnWs w;
   rnn::carve_rnn(d, S, rows, (char*)workspace, &w);
   if (cudaMemsetAsync(grads, 0, (size_t)S * P * sizeof(float), st) != cudaSuccess)
-    return check_launch("pqn_rnn_loss_grad(memset)");
+    return check_launch(who);
   const int64_t gs = (int64_t)S * rows * H;
   // ---- forward over the window
-  if ((rc = rnn::rnn_trunk(d, L, params, obs, (int64_t)rows * D, S, rows, true, w, st))) return rc;
+  if ((rc = rnn::rnn_trunk(d, L, params, batch_stats, obs, rows, S, rows, true, w, st))) return rc;
   if ((rc = rnn::rnn_scan_fwd<true>(d, L, params, last_action, last_done, hs0, w.dhl /*scratch carry out*/, S, T, B, w, st)))
     return rc;
   { LaunchScope _ls(K_RNN_MISC, st);
@@ -3085,6 +3073,10 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
   nrm::colsum2(w.dhn, w.dhn, S, rows, H, H, nw, w.sums, grads, P, L.gru_hn_b, -1, st);                 // d b_hn
   { LaunchScope _ls(K_RNN_MISC, st);
     PQN_H_DISPATCH(H, rnn::rnn_onehot_grad_kernel<HH><<<dim3(S, 3), HH, 0, st>>>(w.da, gs, last_action, rows, A, grads, P, L)); }
+  if (rnn::modular_rnn(d)) {
+    if ((rc = rnn::rnn_trunk_bwd_modular(d, L, params, obs, grads, S, rows, w, st))) return rc;
+    return check_launch(who);
+  }
   // ---- trunk backward (LayerNorm backward -> weight gradient -> input gradient of the layer below)
   const dim3 rbg(conv_mma_ctas(S, rows, 4), S);
   float* dcur = w.dx;
@@ -3104,7 +3096,60 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
       dcur = dnext;
     }
   }
-  return check_launch("pqn_rnn_loss_grad");
+  return check_launch(who);
+}
+
+}  // namespace pqn
+
+using namespace pqn;
+
+extern "C" {
+
+int64_t pqn_net_stats_floats(const pqn_net_desc_t* d) {
+  if (check_desc(d, "pqn_net_stats_floats")) return -1;
+  return nrm::stats_floats(d);
+}
+
+int pqn_rnn_step(const pqn_net_desc_t* d, const float* params, float* hs, const float* obs, int64_t obs_rows_per_seed,
+                 const uint8_t* last_done, const int32_t* last_action, float* q, int32_t S, int32_t E, void* workspace,
+                 void* stream) {
+  int rc = check_desc(d, "pqn_rnn_step");
+  if (rc) return rc;
+  if ((rc = rnn::check_rnn(d, "pqn_rnn_step"))) return rc;
+  return rnn_step(d, params, nullptr, hs, obs, obs_rows_per_seed, last_done, last_action, q, S, E, workspace, stream,
+                  "pqn_rnn_step");
+}
+
+int pqn_rnn_step_stats(const pqn_net_desc_t* d, const float* params, const float* batch_stats, float* hs, const float* obs,
+                       int64_t obs_rows_per_seed, const uint8_t* last_done, const int32_t* last_action, float* q, int32_t S,
+                       int32_t E, void* workspace, void* stream) {
+  int rc = check_desc(d, "pqn_rnn_step_stats");
+  if (rc) return rc;
+  if ((rc = rnn::check_rnn_stats(d, batch_stats, "pqn_rnn_step_stats"))) return rc;
+  return rnn_step(d, params, batch_stats, hs, obs, obs_rows_per_seed, last_done, last_action, q, S, E, workspace, stream,
+                  "pqn_rnn_step_stats");
+}
+
+int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float* hs0, const float* obs,
+                      const uint8_t* last_done, const int32_t* last_action, const int32_t* action, const float* reward,
+                      const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum, int32_t S, int32_t T, int32_t B,
+                      float gamma, float lambda, void* workspace, void* stream) {
+  int rc = check_desc(d, "pqn_rnn_loss_grad");
+  if (rc) return rc;
+  if ((rc = rnn::check_rnn(d, "pqn_rnn_loss_grad"))) return rc;
+  return rnn_loss_grad(d, params, nullptr, hs0, obs, last_done, last_action, action, reward, done, grads, loss_sum, qsa_sum,
+                       S, T, B, gamma, lambda, workspace, stream, "pqn_rnn_loss_grad");
+}
+
+int pqn_rnn_loss_grad_stats(const pqn_net_desc_t* d, const float* params, float* batch_stats, const float* hs0,
+                            const float* obs, const uint8_t* last_done, const int32_t* last_action, const int32_t* action,
+                            const float* reward, const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum,
+                            int32_t S, int32_t T, int32_t B, float gamma, float lambda, void* workspace, void* stream) {
+  int rc = check_desc(d, "pqn_rnn_loss_grad_stats");
+  if (rc) return rc;
+  if ((rc = rnn::check_rnn_stats(d, batch_stats, "pqn_rnn_loss_grad_stats"))) return rc;
+  return rnn_loss_grad(d, params, batch_stats, hs0, obs, last_done, last_action, action, reward, done, grads, loss_sum,
+                       qsa_sum, S, T, B, gamma, lambda, workspace, stream, "pqn_rnn_loss_grad_stats");
 }
 
 int pqn_set_conv_mma_path(int on) {

@@ -6,7 +6,10 @@
 // flax.linen.GRUCell (restated from its published source; the test-side NumPy restatement pins it against
 // torch.nn.GRUCell):   r = sigmoid(x W_ir + b_ir + h W_hr)      z = sigmoid(x W_iz + b_iz + h W_hz)
 //                      n = tanh(x W_in + b_in + r * (h W_hn + b_hn))       h' = (1 - z) n + z h
-// Layer-norm networks only (the shipped pqn_rnn_*.yaml), NORM_INPUT=False.
+// NORM_TYPE in {layer_norm, batch_norm, none} x NORM_INPUT (:65-76).  The default (layer_norm, NORM_INPUT=False, the
+// shipped pqn_rnn_*.yaml) runs its trunk on the fused dense + LayerNorm kernels; every other combination runs the
+// modular trunk of pqn_norm.cuh (raw dense, then one normalisation kernel per layer), whose BatchNorms reduce over
+// every row of the [T][B] window and keep running statistics in the caller's batch_stats block.
 //
 // Structure (fp32 CUDA cores; these runs are small and launch-bound: 32 envs x 64 steps per update in the shipped
 // preset): the time-independent parts (trunk MLP, input-side gate products x W_i*, Q head, all weight gradients) are
@@ -299,7 +302,12 @@ __global__ void __launch_bounds__(H) rnn_onehot_grad_kernel(const float* __restr
 // ---------------------------------------------------------------------------------------------------------------
 struct RnnWs {
   float *h[PQN_MAX_LAYERS], *xh[PQN_MAX_LAYERS], *rs[PQN_MAX_LAYERS], *ai, *y, *h0, *rg, *zg, *ng, *hn, *q, *dq, *dy, *da, *dhn, *dx, *dhl, *wt, *part, *sums, *rbp, *wgp;
+  // modular trunk only: (mean, rstd) of hidden BatchNorm l and of the input BatchNorm, (d beta, d gamma) sums, the
+  // dense obs rows, the normalised input, its xhat and its gradient
+  float *mr[PQN_MAX_LAYERS], *mr_in, *dg, *xg, *xn, *xhin, *dxn;
 };
+
+static inline bool modular_rnn(const pqn_net_desc_t* d) { return d->norm_type != PQN_NORM_LAYER || d->norm_input != 0; }
 
 static int64_t carve_rnn(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* base, RnnWs* w) {
   int64_t off = 0;
@@ -325,33 +333,102 @@ static int64_t carve_rnn(const pqn_net_desc_t* d, int32_t S, int64_t rows, char*
   ww->sums = take((int64_t)S * chan);
   ww->wgp = take(wgrad_split_tiles() * 128 * 128);   // per-split partials of the FFMA weight gradient
   ww->rbp = take(part_ctas(S) * row_bwd_part_floats(H, A));
+  if (modular_rnn(d)) {   // appended, so the default network's workspace does not change
+    const int D = d->in_c;
+    for (int l = 0; l < d->layers; ++l) ww->mr[l] = take((int64_t)S * chan);
+    ww->mr_in = take((int64_t)S * chan);
+    ww->dg = take((int64_t)S * chan);
+    ww->xg = take(R * D); ww->xn = take(R * D); ww->xhin = take(R * D); ww->dxn = take(R * D);
+  }
   return off;
 }
 
 static int check_rnn(const pqn_net_desc_t* d, const char* who) {
   if (d->kind != PQN_NET_RNN) return set_error(PQN_E_INVALID, "%s: not an RNN descriptor", who);
-  if (d->norm_type != PQN_NORM_LAYER || d->norm_input)
-    return set_error(PQN_E_UNSUPPORTED, "%s: the GRU network is built for NORM_TYPE=layer_norm, NORM_INPUT=False", who);
+  if (modular_rnn(d))
+    return set_error(PQN_E_UNSUPPORTED, "%s: the GRU network is built for NORM_TYPE=layer_norm, NORM_INPUT=False here; "
+                     "the other NORM_TYPE / NORM_INPUT take batch_stats (pqn_rnn_step_stats / pqn_rnn_loss_grad_stats)", who);
   return PQN_OK;
 }
 
-// trunk (NUM_LAYERS x Dense -> LayerNorm -> ReLU) + input-side gate products over `rows` rows per seed
-static int rnn_trunk(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const float* params, const float* x, int64_t xss,
-                      int S, int rows, bool train, RnnWs& w, cudaStream_t st) {
+// the *_stats entry points: every NORM_TYPE / NORM_INPUT; batch_stats may be NULL only for the default network.  The
+// input BatchNorm's statistics are column sums over D <= 16 features (colsum2's per-row path) or D dividing 256.
+static int check_rnn_stats(const pqn_net_desc_t* d, const float* batch_stats, const char* who) {
+  if (d->kind != PQN_NET_RNN) return set_error(PQN_E_INVALID, "%s: not an RNN descriptor", who);
+  if (modular_rnn(d) && !batch_stats)
+    return set_error(PQN_E_INVALID, "%s: NORM_TYPE=%s, NORM_INPUT=%d needs the batch_stats block (NULL given)", who,
+                     d->norm_type == PQN_NORM_BATCH ? "batch_norm" : (d->norm_type == PQN_NORM_LAYER ? "layer_norm" : "none"),
+                     d->norm_input);
+  if (batch_stats && d->in_c > 16 && 256 % d->in_c != 0)
+    return set_error(PQN_E_UNSUPPORTED, "%s: input BatchNorm over %d features (at most 16, or a divisor of 256, built)",
+                     who, d->in_c);
+  return PQN_OK;
+}
+
+// trunk (NUM_LAYERS x Dense -> normalize -> ReLU) + input-side gate products over `rows` rows per seed.
+//   x: float obs rows, row r of seed s at s * orps + r.  batch_stats: running statistics (NULL for the default network).
+//   train: the modular trunk's BatchNorms use the batch statistics of the rows and update batch_stats in place; the
+//   input BatchNorm's statistics are updated whenever batch_stats is given (also for the default network, whose
+//   fused trunk does not read them).  Eval: the running statistics normalise.
+static int rnn_trunk(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const float* params, float* batch_stats,
+                     const float* x, int64_t orps, int S, int rows, bool train, RnnWs& w, cudaStream_t st) {
   const int D = d->in_c, H = d->hidden, A = d->num_actions;
   const int64_t P = L.total;
   const int BM = (H == 128) ? 128 : 64;
   const float* cur = x;
-  int64_t css = xss;
+  int64_t css = orps * D;
   int kin = D;
-  for (int l = 0; l < d->layers; ++l) {
-    const DenseOff o = dense_off(L, H, l);
-    const int rc = train ? dense_ln_fwd<1>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o, 0, 0, A, w.h[l],
-                                           w.xh[l], w.rs[l], nullptr, rows, kin)
-                         : dense_ln_fwd<0>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o, 0, 0, A, w.h[l],
-                                           nullptr, nullptr, nullptr, rows, kin);
-    if (rc) return rc;
-    cur = w.h[l]; css = (int64_t)rows * H; kin = H;
+  nrm::NormWs nw = {};
+  nw.part = w.part; nw.sums = w.sums; nw.dg = w.dg;
+  if (!modular_rnn(d)) {
+    if (train && batch_stats) {
+      // BatchNorm_0 is applied and its output discarded (:75-76); train mode still moves its running statistics.
+      // bn_prepare turns the sums into (mean, rstd) in place: each thread reads its two sums before it writes them.
+      nrm::colsum2(x, x, S, rows, D, D, nw, w.sums, nullptr, 0, -1, -1, st);
+      LaunchScope _ls(K_NORM_FWD, st);
+      nrm::bn_prepare_kernel<<<S, 256, 0, st>>>(w.sums, (float)rows, batch_stats, nrm::stats_floats(d), D, 1, 0.99f, w.sums);
+    }
+    for (int l = 0; l < d->layers; ++l) {
+      const DenseOff o = dense_off(L, H, l);
+      const int rc = train ? dense_ln_fwd<1>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o, 0, 0, A, w.h[l],
+                                             w.xh[l], w.rs[l], nullptr, rows, kin)
+                           : dense_ln_fwd<0>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o, 0, 0, A, w.h[l],
+                                             nullptr, nullptr, nullptr, rows, kin);
+      if (rc) return rc;
+      cur = w.h[l]; css = (int64_t)rows * H; kin = H;
+    }
+  } else {
+    const int norm = d->norm_type;
+    const int64_t sstride = nrm::stats_floats(d);
+    if (orps != rows) {   // strided rollout rows: make them dense for the column sums and the elementwise kernels
+      LaunchScope _ls(K_GATHER_ROWS, st);
+      gather_rows_kernel<<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(x, orps, nullptr, w.xg, rows, D);
+      cur = w.xg; css = (int64_t)rows * D;
+    }
+    const float* xd = cur;
+    if (train || d->norm_input) {
+      if (train) nrm::colsum2(xd, xd, S, rows, D, D, nw, w.sums, nullptr, 0, -1, -1, st);
+      LaunchScope _ls(K_NORM_FWD, st);
+      nrm::bn_prepare_kernel<<<S, 256, 0, st>>>(w.sums, (float)rows, batch_stats, sstride, D, train, 0.99f, w.mr_in);
+    }
+    if (d->norm_input) {
+      LaunchScope _ls(K_NORM_FWD, st);
+      nrm::norm_elem_fwd_kernel<2><<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(
+          xd, (int64_t)rows * D, D, D, w.mr_in, params, P, L.bn_scale, L.bn_bias, nullptr, w.xn);
+      cur = w.xn;
+    }
+    for (int l = 0; l < d->layers; ++l) {
+      const DenseOff o = dense_off(L, H, l);
+      // raw pre-activation into h[l], normalised + ReLU in place
+      int rc = launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, css, kin, params, P, o.w, o.b, 0, 0, 0, 0, A, w.h[l],
+                               nullptr, nullptr, nullptr, rows, kin);
+      if (rc) return rc;
+      float* run = norm == nrm::NORM_BN ? batch_stats + nrm::stats_off(d, l) : nullptr;
+      if ((rc = nrm::norm_layer_fwd(norm, w.h[l], S, rows, H, H, params, P, o.g, o.bi, run, sstride, train, nw, w.mr[l],
+                                    train && norm != nrm::NORM_NONE ? w.xh[l] : nullptr, train ? w.rs[l] : nullptr, w.h[l],
+                                    st))) return rc;
+      cur = w.h[l]; css = (int64_t)rows * H; kin = H;
+    }
   }
   const int64_t gs = (int64_t)S * rows * H;
   const int64_t iw[3] = {L.gru_ir_w, L.gru_iz_w, L.gru_in_w}, ib[3] = {L.gru_ir_b, L.gru_iz_b, L.gru_in_b};
@@ -359,6 +436,44 @@ static int rnn_trunk(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const f
     const int rc = launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, css, H, params, P, iw[g], ib[g], 0, 0, 0, 0, A,
                                    w.ai + g * gs, nullptr, nullptr, nullptr, rows, H);
     if (rc) return rc;
+  }
+  return 0;
+}
+
+// Backward of the modular trunk.  On entry w.dx holds d x_L, the gate input-gradients under the trunk's ReLU mask.
+// Per layer, last first: normalisation backward (LN / BN with the batch statistics' terms / none) with d scale, d bias
+// of the norm and of the dense, the FFMA weight gradient, the masked input gradient of the layer below.  With
+// NORM_INPUT, d scale / d bias of BatchNorm_0 from the input gradient of Dense_0 (nrm::norm_loss_grad's recipe).
+//   x: the dense float obs rows [S][rows][D] of the forward.
+static int rnn_trunk_bwd_modular(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const float* params, const float* x,
+                                 float* grads, int S, int rows, RnnWs& w, cudaStream_t st) {
+  const int D = d->in_c, H = d->hidden;
+  const int64_t P = L.total;
+  nrm::NormWs nw = {};
+  nw.part = w.part; nw.sums = w.sums; nw.dg = w.dg;
+  const float* xin = d->norm_input ? w.xn : x;
+  float* dcur = w.dx;
+  for (int l = d->layers - 1; l >= 0; --l) {
+    const DenseOff o = dense_off(L, H, l);
+    int rc = nrm::norm_layer_bwd(d->norm_type, dcur, w.xh[l], w.rs[l], S, rows, H, H, params, grads, P, o.g, o.bi, o.b, nw,
+                                 w.mr[l], st);
+    if (rc) return rc;
+    const float* xprev = l == 0 ? xin : w.h[l - 1];
+    const int kin = l == 0 ? D : H;
+    run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, dcur, (int64_t)rows * H, H, grads, P, o.w, rows, kin, S,
+                   wgrad_splits(ffma_tiles(kin, H), S, rows), w.wgp, st);
+    if (l > 0) {
+      float* dnext = dcur == w.dhl ? w.dx : w.dhl;   // dgrad reads all of dz_l while it writes dh_{l-1}
+      launch_dgrad(dcur, (int64_t)rows * H, H, params, P, o.w, w.h[l - 1], dnext, (int64_t)rows * H, rows, H, 0, S, st);
+      dcur = dnext;
+    }
+  }
+  if (d->norm_input) {
+    { LaunchScope _ls(K_DGRAD, st);
+      nrm::dgrad_small_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(dcur, rows, H, params, P, L.d0_w, D, w.dxn); }
+    { LaunchScope _ls(K_NORM_BWD, st);
+      nrm::in_xhat_kernel<<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(x, (int64_t)rows * D, D, w.mr_in, w.xhin); }
+    nrm::colsum2(w.dxn, w.xhin, S, rows, D, D, nw, w.dg, grads, P, L.bn_bias, L.bn_scale, st);
   }
   return 0;
 }

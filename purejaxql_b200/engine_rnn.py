@@ -3,7 +3,10 @@ purejaxql/pqn_rnn_gymnax.py:117-560 with the seed axis taken natively.
 
 All compute is libpqn_b200 kernels: ``pqn_rnn_step`` (one step of the recurrent Q-network for the rollout, the memory
 warm-up and the evaluation), ``pqn_rollout_act_step`` (eps-greedy + env step + LogWrapper, shared with the feed-forward
-engine), ``pqn_rnn_loss_grad`` (window forward, in-loss Q(lambda) targets, BPTT) and ``pqn_radam_clip_step``.  This
+engine), ``pqn_rnn_loss_grad`` (window forward, in-loss Q(lambda) targets, BPTT) and ``pqn_radam_clip_step``.  The
+NORM_TYPE / NORM_INPUT variants other than (layer_norm, False) call ``pqn_rnn_step_stats`` / ``pqn_rnn_loss_grad_stats``
+with a static ``batch_stats`` buffer: the loss updates the running statistics in place (:362-369), the steps read them
+(train=False), so the update stays capturable in a CUDA graph.  This
 module owns the buffers, walks the reference's PRNG key chain — including its re-bindings of ``rng`` to the final
 carry of the rollout scans (:222-228, :531-537) — and keeps the memory of the last MEMORY_WINDOW + NUM_STEPS
 transitions.  Minibatches are whole env trajectories: ``jax.random.permutation(rng, x, axis=1)`` (:368-379).
@@ -27,9 +30,6 @@ class PQNRnnEngine:
         if self.device.type != "cuda" or not torch.cuda.is_available():
             raise _lib.PqnError("purejaxql_b200 needs a CUDA device: there is no CPU fallback")
         _lib.lib()
-        if c.get("NORM_TYPE", "layer_norm") != "layer_norm" or c.get("NORM_INPUT", False):
-            raise NotImplementedError("the GRU network is built for NORM_TYPE=layer_norm, NORM_INPUT=False "
-                                      "(the shipped pqn_rnn_cartpole.yaml)")
         self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
         self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=True, rng_mode=self.rng_mode)
         if env_params is not None:                                   # e.g. MemoryChain's memory_length (:134-136)
@@ -42,7 +42,11 @@ class PQNRnnEngine:
         self.W = int(c["MEMORY_WINDOW"])
         self.A, self.D = self.env.num_actions, self.env.obs_dim
         self.H = int(c.get("HIDDEN_SIZE", 128))
-        self.spec = QNetworkSpec(NET_RNN, self.D, self.A, self.H, int(c.get("NUM_LAYERS", 2)))
+        self.spec = QNetworkSpec(NET_RNN, self.D, self.A, self.H, int(c.get("NUM_LAYERS", 2)),
+                                 norm_type=c.get("NORM_TYPE", "layer_norm"), norm_input=bool(c.get("NORM_INPUT", False)))
+        # the default network keeps the entry points without running statistics (its BatchNorm_0 output is discarded)
+        self.with_stats = self.spec.norm_type != "layer_norm" or self.spec.norm_input
+        self.batch_stats = None                                      # [S][stats_total] running statistics (with_stats)
         self.nmb, self.epochs = int(c["NUM_MINIBATCHES"]), int(c["NUM_EPOCHS"])
         assert self.E % self.nmb == 0, "NUM_MINIBATCHES must divide NUM_ENVS (minibatches are whole env trajectories)"
         self.Bm = self.E // self.nmb
@@ -59,10 +63,16 @@ class PQNRnnEngine:
         return self._ws
 
     def step(self, params, hs, obs, last_done, last_action, q, S, N):
-        """network.apply(params, hs, obs[None], done[None], last_action[None], train=False) for S x N envs; hs in place."""
-        _lib.check(_lib.lib().pqn_rnn_step(self.spec.desc, _lib.p(params), _lib.p(hs), _lib.p(obs), N, _lib.p(last_done),
-                                           _lib.p(last_action), _lib.p(q), S, N, _lib.p(self._workspace(S, N)),
-                                           _lib.stream_ptr()), "pqn_rnn_step")
+        """network.apply(params, hs, obs[None], done[None], last_action[None], train=False) for S x N envs; hs in place.
+        The BatchNorm variants normalise with ``self.batch_stats``."""
+        L, ws = _lib.lib(), self._workspace(S, N)
+        if self.with_stats:
+            _lib.check(L.pqn_rnn_step_stats(self.spec.desc, _lib.p(params), _lib.p(self.batch_stats), _lib.p(hs),
+                                            _lib.p(obs), N, _lib.p(last_done), _lib.p(last_action), _lib.p(q), S, N,
+                                            _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_step_stats")
+        else:
+            _lib.check(L.pqn_rnn_step(self.spec.desc, _lib.p(params), _lib.p(hs), _lib.p(obs), N, _lib.p(last_done),
+                                      _lib.p(last_action), _lib.p(q), S, N, _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_step")
 
     def _act_step(self, S, N, step_keys, q, eps, state, obs_next, action, reward, done, maxq, sums, done_only, rew_scale):
         L = _lib.lib()
@@ -102,6 +112,7 @@ class PQNRnnEngine:
         k = jr.split(keys, 2, mode)
         rng = k[:, 0].contiguous()                                   # :255  rng, _rng = split(rng)
         params = spec.init(rng, dev)                                 # :256  create_agent(rng)  (the CARRIED key)
+        self.batch_stats = spec.init_stats(S, dev) if self.with_stats else None   # mean 0, var 1
         mu, nu, grads = torch.zeros_like(params), torch.zeros_like(params), torch.zeros_like(params)
         step_counter = torch.zeros(1, dtype=torch.int32, device=dev)
         gnorm = torch.zeros(S * 64, device=dev)
@@ -201,10 +212,17 @@ class PQNRnnEngine:
                     obs_mb = mem.obs.gather(2, i3[..., None].expand(S, Tm, Bm, D)).contiguous()
                     hs0 = mem.hs[:, 0].gather(1, idx[:, :, None].expand(S, Bm, H)).contiguous()
                     ld, la, ac, rw, dn = g3(mem.last_done), g3(mem.last_action), g3(mem.action), g3(mem.reward), g3(mem.done)
-                    _lib.check(L.pqn_rnn_loss_grad(spec.desc, _lib.p(params), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
-                                                   _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads),
-                                                   _lib.p(loss_sum), _lib.p(qsa_sum), S, Tm, Bm, self.gamma, self.lam,
-                                                   _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_loss_grad")
+                    if self.with_stats:                              # batch_stats = updates["batch_stats"] (:362-369)
+                        _lib.check(L.pqn_rnn_loss_grad_stats(
+                            spec.desc, _lib.p(params), _lib.p(self.batch_stats), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
+                            _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads), _lib.p(loss_sum),
+                            _lib.p(qsa_sum), S, Tm, Bm, self.gamma, self.lam, _lib.p(ws), _lib.stream_ptr()),
+                            "pqn_rnn_loss_grad_stats")
+                    else:
+                        _lib.check(L.pqn_rnn_loss_grad(spec.desc, _lib.p(params), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
+                                                       _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads),
+                                                       _lib.p(loss_sum), _lib.p(qsa_sum), S, Tm, Bm, self.gamma, self.lam,
+                                                       _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_loss_grad")
                     _lib.check(L.pqn_radam_clip_step(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu), _lib.p(sched),
                                                      _lib.p(step_counter), _lib.p(gnorm), S, P, float(c["MAX_GRAD_NORM"]),
                                                      0.9, 0.999, 1e-8, _lib.stream_ptr()), "pqn_radam_clip_step")
@@ -253,7 +271,7 @@ class PQNRnnEngine:
             for j, kk in enumerate(INFO_KEYS):
                 metrics[kk][:, col] = m_cur[:, 2 + j]
             if on_update_end is not None:
-                on_update_end(n_updates, dict(mem=mem, params=params, rng=rng_buf))
+                on_update_end(n_updates, dict(mem=mem, params=params, rng=rng_buf, batch_stats=self.batch_stats))
             if self.test:                                            # :398-408
                 if test_every > 0 and (n_updates + 1) % test_every == 0:
                     test_metrics = self.get_test_metrics(params, kT_buf.clone())
@@ -266,7 +284,7 @@ class PQNRnnEngine:
         if self.test:
             out_metrics.update({f"test/{kk}": v[:, :NU].float() for kk, v in test_hist.items()})
         F = spec.in_c
-        bs = spec.init_stats(S, dev)
+        bs = self.batch_stats if self.with_stats else spec.init_stats(S, dev)
         train_state = TrainState(
             params=spec.unflatten(params), params_flat=params, batch_stats=spec.unflatten_stats(bs), batch_stats_flat=bs,
             opt_state=SimpleNamespace(mu=mu, nu=nu, count=grad_steps),
