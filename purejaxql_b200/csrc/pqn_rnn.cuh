@@ -181,7 +181,7 @@ __global__ void rnn_targets_kernel(const float* __restrict__ q, const int32_t* _
                                    const float* __restrict__ reward, const uint8_t* __restrict__ done, int T, int B, int A,
                                    float gamma, float lam, float* __restrict__ dq, float* __restrict__ loss_sum,
                                    float* __restrict__ qsa_sum) {
-  extern __shared__ float red[];   // [2][blockDim]
+  extern __shared__ float red[];   // [2][32] warp sums (blockDim is a multiple of 32, so at least 64 floats)
   const int seed = blockIdx.x, b = threadIdx.x;
   float l_acc = 0.f, q_acc = 0.f;
   const float inv = 1.0f / (float)((T - 1) * B);
@@ -221,11 +221,19 @@ __global__ void rnn_targets_kernel(const float* __restrict__ q, const int32_t* _
       emit(t, lr);
     }
   }
-  red[b] = l_acc; red[blockDim.x + b] = q_acc;
+  // deterministic reduction over the columns: a butterfly within each warp, then thread 0 adds the warp sums in order.
+  // (a serial sum over the columns drifts with B: ~8 fp32 ulps at B = 1024).  For B <= 2 the result is the serial
+  // sum's, bit for bit: the other lanes add zeros.
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    l_acc += __shfl_xor_sync(0xffffffffu, l_acc, o);
+    q_acc += __shfl_xor_sync(0xffffffffu, q_acc, o);
+  }
+  if ((b & 31) == 0) { red[b >> 5] = l_acc; red[32 + (b >> 5)] = q_acc; }
   __syncthreads();
   if (b == 0) {
     float l = 0.f, qs = 0.f;
-    for (int i = 0; i < B; ++i) { l += red[i]; qs += red[blockDim.x + i]; }
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { l += red[i]; qs += red[32 + i]; }
     loss_sum[seed] += l;
     qsa_sum[seed] += qs;
   }

@@ -26,6 +26,15 @@ def make_train(config):
             raise ValueError(f"MemoryChain-bsuite needs ENV_KWARGS.memory_length to be a positive int, "
                              f"got {memory_length!r}")
         env_params = envs.EnvParams(env_params.max_steps_in_episode, memory_length=memory_length)
+    # the window loss (pqn_rnn_loss_grad) takes at most 1024 trajectories per minibatch and needs two steps of window
+    # (one loss step plus its bootstrap); refuse other shapes here rather than after the warm-up and the first rollout
+    traj = config["NUM_ENVS"] // config["NUM_MINIBATCHES"]
+    if traj > 1024:
+        raise ValueError(f"NUM_ENVS / NUM_MINIBATCHES = {traj} trajectories per minibatch; the recurrent loss takes at "
+                         f"most 1024")
+    window = config.get("MEMORY_WINDOW", 0) + config["NUM_STEPS"]
+    if window < 2:
+        raise ValueError(f"MEMORY_WINDOW + NUM_STEPS = {window}; the recurrent loss needs a window of at least 2 steps")
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=True)    # :119-132,140
     engine = PQNRnnEngine(config, env_params=env_params)
 
