@@ -169,6 +169,13 @@ int pqn_qlambda(const float* reward, const uint8_t* done, const float* maxq, con
 #define PQN_NET_MINATAR_CNN 0
 #define PQN_NET_MLP 1
 #define PQN_NET_RNN 2   /* RNNQNetwork (GRU) of pqn_rnn_gymnax.py:57-105: MLP trunk + one-hot last action + scanned GRU + head */
+/* The MLP QNetwork of pqn_gymnax.py on a MinAtar env behind FlattenObservationWrapper: in_c = D = 100 * C (400, 600 or
+ * 700) {0,1} features, fed as the env's packed rows (packed_obs_words uint32 per row; bit f = element f of the flattened
+ * (10,10,C) observation, which multiplies row f of Dense_0/kernel).  Parameter layout, flax names, hidden / layer /
+ * action limits and batch_stats are those of PQN_NET_MLP with in_c inputs; obs / gather / obs_rows_per_seed mean what
+ * they mean for the CNN.  Tensor-core path 2 runs Dense_0 (forward and weight gradient) on fp16 mma.sync straight from
+ * the packed bits; any other path expands the gathered bits into fp32 rows and runs the PQN_NET_MLP kernels. */
+#define PQN_NET_MLP_BITS 3
 
 typedef struct pqn_net_desc_t {
   int32_t kind;        /* PQN_NET_* */
@@ -220,7 +227,7 @@ int64_t pqn_net_workspace_bytes(const pqn_net_desc_t* desc_host, int32_t S, int6
 int pqn_net_init(const pqn_net_desc_t* desc_host, const uint32_t* keys, float* params, int32_t S, void* stream);
 
 /* q[S][rows][A] = network.apply(params, obs, train=False) — pqn_minatar.py:184-191,227-234.
- *  obs: packed uint32[S][rows_total][packed_words] (CNN) or float32[S][rows_total][D] (MLP);
+ *  obs: packed uint32[S][rows_total][packed_words] (CNN, MLP_BITS) or float32[S][rows_total][D] (MLP);
  *  gather (may be NULL): int32[S][rows] row indices into the seed's obs rows
  *  (minibatch gather of preprocess_transition, :299-307); obs_rows_per_seed is
  *  the stride of the obs buffer in rows.  batch_stats: float32[S][pqn_net_stats_floats] running statistics, read by

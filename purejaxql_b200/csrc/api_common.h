@@ -18,7 +18,8 @@ enum KernelId : int {
   K_NORM_FWD, K_NORM_BWD, K_NORM_REDUCE /* modular NORM_TYPE / NORM_INPUT path (pqn_norm.cuh) */,
   K_RNN_SCAN, K_RNN_MISC /* GRU network (pqn_rnn.cuh) */,
   K_GRAD_FINAL /* fixed-order second stage of the deterministic gradient reductions */,
-  K_PERM /* jax.random.permutation bucket + rank sort (pqn_perm.cu) */, K_COUNT
+  K_PERM /* jax.random.permutation bucket + rank sort (pqn_perm.cu) */,
+  K_BITS_FWD, K_BITS_WGRAD /* Dense_0 of the MLP on packed MinAtar bits (pqn_bits.cuh) */, K_COUNT
 };
 
 // SM count of the CURRENT device (cached per device ordinal, not per process)

@@ -53,7 +53,7 @@ static int make_layout(const pqn_net_desc_t* d, pqn_net_layout_t* L) {
     L->d0_w = take((int64_t)FLAT_CNN * HID_CNN); L->d0_b = take(HID_CNN);
     if (has_norm) { L->ln1_scale = take(HID_CNN); L->ln1_bias = take(HID_CNN); }
     L->head_w = take((int64_t)HID_CNN * A); L->head_b = take(A);
-  } else if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN) {
+  } else if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN || d->kind == PQN_NET_MLP_BITS) {
     const int D = d->in_c, H = d->hidden;
     L->bn_scale = take(D); L->bn_bias = take(D);
     L->d0_w = take((int64_t)D * H); L->d0_b = take(H);
@@ -98,7 +98,7 @@ static int check_desc(const pqn_net_desc_t* d, const char* who) {
   if (d->num_actions < 1 || d->num_actions > 32) return set_error(PQN_E_INVALID, "%s: num_actions=%d out of [1,32]", who, d->num_actions);
   if (d->norm_type < 0 || d->norm_type > 2 || d->norm_input < 0 || d->norm_input > 1)
     return set_error(PQN_E_INVALID, "%s: norm_type=%d norm_input=%d", who, d->norm_type, d->norm_input);
-  if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN) {
+  if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN || d->kind == PQN_NET_MLP_BITS) {
     const int H = d->hidden;
     if (H != 64 && H != 128 && H != 256 && H != 512)
       return set_error(PQN_E_UNSUPPORTED, "%s: hidden=%d (64, 128, 256 or 512 built)", who, H);
@@ -116,6 +116,12 @@ static int check_desc(const pqn_net_desc_t* d, const char* who) {
   if (d->kind == PQN_NET_MINATAR_CNN) {
     if (d->in_c != 4 && d->in_c != 6 && d->in_c != 7 && d->in_c != 10)
       return set_error(PQN_E_UNSUPPORTED, "%s: CNN in_c=%d (MinAtar uses 4/6/7/10)", who, d->in_c);
+    return PQN_OK;
+  }
+  if (d->kind == PQN_NET_MLP_BITS) {
+    if (d->in_c != 400 && d->in_c != 600 && d->in_c != 700)
+      return set_error(PQN_E_UNSUPPORTED, "%s: MLP on packed MinAtar observations with in_c=%d (100 * C: 400, 600 or 700 "
+                       "built)", who, d->in_c);
     return PQN_OK;
   }
   if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN) {
@@ -2446,6 +2452,8 @@ static void launch_dgrad(const float* DZ, int64_t dz_seed_stride, int N, const f
     dgrad_kernel<64><<<grid, GT, 0, st>>>(DZ, dz_seed_stride, N, params, P, off_w, HPREV, OUT, h_seed_stride, rows, Kprev, accumulate);
 }
 
+#include "pqn_bits.cuh"
+
 static int64_t carve(const pqn_net_desc_t* d, int32_t S, int64_t rows, char* base, Workspace* w) {
   int64_t off = 0;
   auto take = [&](int64_t nfloats) -> float* {
@@ -2991,6 +2999,28 @@ static int mlp_hidden_tc_fwd(const Workspace& w, const pqn_net_layout_t& L, cons
   return 0;
 }
 
+// Layer 0 of the default MLP on packed bits (PQN_NET_MLP_BITS, tensor-core path 2): w.h[0] = ReLU(LayerNorm(bits . W0 +
+// b0)), with xhat / rstd for the backward when given
+static int bits_layer0_ln(const pqn_net_desc_t* d, const pqn_net_layout_t& L, const float* params, const uint32_t* obs,
+                          int64_t orps, const int32_t* gather, int S, int rows, const Workspace& w, const bits::BitsWs& bw,
+                          float* xhat, float* rstd, cudaStream_t st) {
+  const int D = d->in_c, H = d->hidden;
+  const int64_t P = L.total;
+  bits::launch_wfrag(params, P, L.d0_w, nullptr, nullptr, D, H, S, bw.wf, st);
+  int rc = bits::launch_fwd(obs, orps, gather, rows, D, H, bw.wf, params + L.d0_b, P, nullptr, w.h[0], S, st);
+  if (rc) return rc;
+  LaunchScope _ls(K_NORM_FWD, st);
+  const dim3 g(cdiv(rows, 8), S);
+  switch (H) {
+    case 64: nrm::ln_fwd_kernel<64><<<g, 256, 0, st>>>(w.h[0], rows, params, P, L.ln0_scale, L.ln0_bias, xhat, rstd, w.h[0]); break;
+    case 128: nrm::ln_fwd_kernel<128><<<g, 256, 0, st>>>(w.h[0], rows, params, P, L.ln0_scale, L.ln0_bias, xhat, rstd, w.h[0]); break;
+    case 256: nrm::ln_fwd_kernel<256><<<g, 256, 0, st>>>(w.h[0], rows, params, P, L.ln0_scale, L.ln0_bias, xhat, rstd, w.h[0]); break;
+    case 512: nrm::ln_fwd_kernel<512><<<g, 256, 0, st>>>(w.h[0], rows, params, P, L.ln0_scale, L.ln0_bias, xhat, rstd, w.h[0]); break;
+    default: return set_error(PQN_E_UNSUPPORTED, "hidden=%d", H);
+  }
+  return 0;
+}
+
 // pqn_rnn_step / pqn_rnn_step_stats after their descriptor checks (batch_stats read-only: train=False)
 static int rnn_step(const pqn_net_desc_t* d, const float* params, const float* batch_stats, float* hs, const float* obs,
                     int64_t obs_rows_per_seed, const uint8_t* last_done, const int32_t* last_action, float* q, int32_t S,
@@ -3175,7 +3205,7 @@ int pqn_net_layout(const pqn_net_desc_t* d, pqn_net_layout_t* out) {
 int pqn_net_dense_layer(const pqn_net_desc_t* d, int32_t layer, int64_t* offsets_host) {
   int rc = check_desc(d, "pqn_net_dense_layer");
   if (rc) return rc;
-  if (d->kind != PQN_NET_MLP && d->kind != PQN_NET_RNN)
+  if (d->kind != PQN_NET_MLP && d->kind != PQN_NET_RNN && d->kind != PQN_NET_MLP_BITS)
     return set_error(PQN_E_INVALID, "pqn_net_dense_layer: only the MLP and GRU networks have hidden dense layers");
   if (!offsets_host || layer < 0 || layer >= d->layers)
     return set_error(PQN_E_INVALID, "pqn_net_dense_layer: layer=%d out of [0,%d) or offsets NULL", layer, d->layers);
@@ -3190,7 +3220,8 @@ int64_t pqn_net_workspace_bytes(const pqn_net_desc_t* d, int32_t S, int64_t rows
   if (check_desc(d, "pqn_net_workspace_bytes")) return -1;
   if (d->kind == PQN_NET_RNN) return rnn::carve_rnn(d, S, rows, nullptr, nullptr);
   if (modular_net(d)) return nrm::carve_norm(d, S, rows, nullptr, nullptr);
-  return carve(d, S, rows, nullptr, nullptr);
+  return carve(d, S, rows, nullptr, nullptr) +
+         (d->kind == PQN_NET_MLP_BITS ? bits::carve_bits(d, S, rows, nullptr, nullptr) : 0);
 }
 
 int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* batch_stats, const void* obs,
@@ -3234,9 +3265,14 @@ int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* 
     }
   } else {
     const int D = d->in_c, H = d->hidden;
+    const bool bits = d->kind == PQN_NET_MLP_BITS, bits_tc = bits && g_use_tc == 2;
     const float* x = (const float*)obs;
     int64_t xss = obs_rows_per_seed * D;
-    if (gather) {
+    if (bits && !bits_tc) {   // packed bits with the tensor-core path off: gathered fp32 rows for the FFMA kernels
+      bits::launch_expand((const uint32_t*)obs, obs_rows_per_seed, gather, (int)rows, D, w.xg, S, st);
+      x = w.xg;
+      xss = rows * D;
+    } else if (gather && !bits) {
       { LaunchScope _ls(K_GATHER_ROWS, st); gather_rows_kernel<<<dim3(cdiv(rows * D, 256), S), 256, 0, st>>>(x, obs_rows_per_seed, gather, w.xg,
                                                                       (int)rows, D); }
       x = w.xg;
@@ -3245,12 +3281,23 @@ int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* 
     const int BM = (H == 128) ? 128 : 64;
     const dim3 grid(cdiv(rows, BM), S);
     const int last = d->layers - 1;
-    if (last == 0) {
+    if (bits_tc) {
+      bits::BitsWs bw;
+      bits::carve_bits(d, S, rows, (char*)workspace + carve(d, S, rows, nullptr, nullptr), &bw);
+      if ((rc = bits_layer0_ln(d, L, params, (const uint32_t*)obs, obs_rows_per_seed, gather, S, (int)rows, w, bw, nullptr,
+                               nullptr, st))) return rc;
+      if (last == 0) {
+        LaunchScope _ls(K_NORM_FWD, st);
+        nrm::head_fwd_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.h[0], (int)rows, H, params, L.total, L.head_w, L.head_b, A, q);
+      }
+    } else if (last == 0) {
       if ((rc = dense_ln_fwd<2>(H, grid, st, x, xss, D, params, L.total, dense_off(L, H, 0), L.head_w, L.head_b, A, w.h[0], nullptr,
                       nullptr, q, (int)rows, D))) return rc;
     } else {
       if ((rc = dense_ln_fwd<0>(H, grid, st, x, xss, D, params, L.total, dense_off(L, H, 0), 0, 0, A, w.h[0], nullptr, nullptr, nullptr,
                       (int)rows, D))) return rc;
+    }
+    {
       for (int l = 1; l <= last; ++l) {
         if (mlp_hidden_tc(H)) {
           // hidden layer (K = N = H) on wgmma: fp16-split planes of h_{l-1} and of the Dense_l kernel, raw product, then
@@ -3370,8 +3417,19 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
   } else {
     const int D = d->in_c, H = d->hidden;
     const int BM = (H == 128) ? 128 : 64;
-    { LaunchScope _ls(K_GATHER_ROWS, st); gather_rows_kernel<<<dim3(cdiv(rows * D, 256), S), 256, 0, st>>>((const float*)obs, obs_rows_per_seed, gather, w.xg, R, D); }
-    if (bn_sums) {
+    const bool bits = d->kind == PQN_NET_MLP_BITS, bits_tc = bits && g_use_tc == 2;
+    const uint32_t* ob = (const uint32_t*)obs;
+    bits::BitsWs bw = {};
+    if (bits) bits::carve_bits(d, S, rows, (char*)workspace + carve(d, S, rows, nullptr, nullptr), &bw);
+    if (bits && !bits_tc) {   // packed bits with the tensor-core path off: gathered fp32 rows for the FFMA kernels
+      bits::launch_expand(ob, obs_rows_per_seed, gather, R, D, w.xg, S, st);
+    } else if (!bits) {
+      LaunchScope _ls(K_GATHER_ROWS, st); gather_rows_kernel<<<dim3(cdiv(rows * D, 256), S), 256, 0, st>>>((const float*)obs, obs_rows_per_seed, gather, w.xg, R, D);
+    }
+    if (bn_sums && bits) {
+      // BatchNorm_0 statistics of {0,1} inputs: sum x = sum x^2 = the per-feature popcount of the minibatch
+      bits::launch_counts(ob, obs_rows_per_seed, gather, R, D, bw, nullptr, bn_sums, S, st);
+    } else if (bn_sums) {
       // input BatchNorm statistics (sum x, sum x^2 per feature): deterministic two-stage column sums of the gathered
       // rows (the per-element float atomics this replaces were 18 % of an Acrobot update at 65,536 envs)
       nrm::NormWs nw = {};
@@ -3383,8 +3441,10 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
     const bool tcl = mlp_hidden_tc(H);
     const int64_t RR = (int64_t)S * rows;
     // ---- forward, keeping every layer's h, xhat and rstd
-    if ((rc = dense_ln_fwd<1>(H, grid, st, w.xg, rows * D, D, params, P, dense_off(L, H, 0), 0, 0, A, w.h[0], w.xhat[0], w.rstd[0],
-                    nullptr, R, D))) return rc;
+    if (bits_tc) {
+      if ((rc = bits_layer0_ln(d, L, params, ob, obs_rows_per_seed, gather, S, R, w, bw, w.xhat[0], w.rstd[0], st))) return rc;
+    } else if ((rc = dense_ln_fwd<1>(H, grid, st, w.xg, rows * D, D, params, P, dense_off(L, H, 0), 0, 0, A, w.h[0], w.xhat[0],
+                                     w.rstd[0], nullptr, R, D))) return rc;
     for (int l = 1; l <= last; ++l) {
       if (tcl) {
         if ((rc = mlp_hidden_tc_fwd(w, L, params, P, H, l, S, R, w.xhat[l], w.rstd[l], K_TC_FWD, st))) return rc;
@@ -3426,7 +3486,8 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
                           head ? gather : nullptr, head ? action : nullptr, head ? target : nullptr,
                           head ? tr_rows_per_seed : 0, head ? loss_sum : nullptr, head ? qsa_sum : nullptr, w.rb_part, R)))
       return rc;
-    run_wgrad_first(w.xg, dz0, grads, P, o0.w, S, R, D, H, w.rb_part, w.wg_part, st);
+    if (bits_tc) bits::launch_wgrad(ob, obs_rows_per_seed, gather, R, D, H, dz0, gscale, nullptr, grads + o0.w, P, bw, S, st);
+    else run_wgrad_first(w.xg, dz0, grads, P, o0.w, S, R, D, H, w.rb_part, w.wg_part, st);
   }
   return check_launch("pqn_qnet_loss_grad");
 }

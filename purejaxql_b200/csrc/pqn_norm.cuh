@@ -25,7 +25,7 @@ constexpr int RED_BLOCKS = 64;   // row chunks per seed of the two-stage reducti
 // ---------------------------------------------------------------------------------------------------------------
 // two-stage per-channel reduction over [S][rows][ncols] (channel = col % G):  out[s][0][g] = sum A,
 // out[s][1][g] = sum A*B.   A == B gives (sum x, sum x^2); (dy, xhat) gives (d beta, d gamma); (dz, dz)[0] = d bias.
-// Requires 256 % G == 0, G == 512 (two channels per thread), or G == ncols <= 16 (the generic path below).
+// Requires 256 % G == 0, G == 512 (two channels per thread), or G == ncols <= 16 or <= 1024 (the generic paths below).
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) colsum2_partial_kernel(const float* __restrict__ A, const float* __restrict__ B,
                                                               int rows, int ncols, int G, float* __restrict__ part) {
@@ -63,6 +63,27 @@ __global__ void __launch_bounds__(256) colsum2_partial_kernel(const float* __res
     }
     float* o = part + (((int64_t)seed * nb + b) * 2) * G;
     o[t] = s; o[256 + t] = s2; o[G + t] = ss; o[G + 256 + t] = ss2;
+  } else if (G > 16) {
+    // wide G that does not divide 256 (the packed-bits MLP's input features, ncols == G <= 1024): thread t owns
+    // channels t, t + 256, ..., rows in order
+    float a0[4] = {0.f, 0.f, 0.f, 0.f}, a1[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int r = r0; r < r1; ++r) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int c = t + 256 * k;
+        if (c < G) {
+          const float x = a[(int64_t)r * ncols + c];
+          a0[k] += x;
+          a1[k] = fmaf(x, bb[(int64_t)r * ncols + c], a1[k]);
+        }
+      }
+    }
+    float* o = part + (((int64_t)seed * nb + b) * 2) * G;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int c = t + 256 * k;
+      if (c < G) { o[c] = a0[k]; o[G + c] = a1[k]; }
+    }
   } else {
     // small G that does not divide 256 (MLP input features, ncols == G <= 16): thread = row, G register accumulators,
     // then a fixed-order tree per channel (warp shuffles, warps in order)
@@ -671,6 +692,7 @@ struct NormWs {
   // shared small buffers; mr[l]: (mean, rstd) of hidden norm l, mr_in: of the MLP's input BatchNorm
   float *part, *sums, *dg, *mr[PQN_MAX_LAYERS], *mr_in, *aff, *weff, *beff, *cntp, *q;
   float* wgp;   // per-split partials of the FFMA weight gradient (run_wgrad_ffma)
+  bits::BitsWs bw;   // PQN_NET_MLP_BITS: Dense_0 on packed bits
   // CNN
   float *z1, *xh1, *h1, *rs1, *z2, *xh2, *h2, *rs2, *d2, *d1;
   // MLP
@@ -680,7 +702,9 @@ struct NormWs {
 
 // channels per seed of the (sum, sum of squares) / (mean, rstd) tables: every per-channel reduction of the network
 static int64_t chan_floats(const pqn_net_desc_t* d) {
-  return 2 * (int64_t)(d->kind != PQN_NET_MINATAR_CNN && d->hidden > 256 ? d->hidden : 256);
+  int64_t m = d->kind != PQN_NET_MINATAR_CNN && d->hidden > 256 ? d->hidden : 256;
+  if (d->kind == PQN_NET_MLP_BITS && d->in_c > m) m = d->in_c;   // the input features' statistics
+  return 2 * m;
 }
 
 static int64_t part_floats(const pqn_net_desc_t* d) {
@@ -726,6 +750,7 @@ static int64_t carve_norm(const pqn_net_desc_t* d, int32_t S, int64_t rows, char
     for (int l = 0; l < nl; ++l) {
       ww->z[l] = take(R * H); ww->xh[l] = take(R * H); ww->h[l] = take(R * H); ww->rs[l] = take(R); ww->d[l] = take(R * H);
     }
+    if (d->kind == PQN_NET_MLP_BITS) off += bits::carve_bits(d, S, rows, base ? base + off : nullptr, &ww->bw);
   }
   return off;
 }
@@ -862,9 +887,17 @@ static int norm_forward(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
     { LaunchScope _ls(K_NORM_FWD, st); head_fwd_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.h2, rows, HID_CNN, params, P, L.head_w, L.head_b, A, q); }
   } else {
     const int D = d->in_c, H = d->hidden;
+    const bool bits = d->kind == PQN_NET_MLP_BITS, bits_tc = bits && g_use_tc == 2;
+    const uint32_t* ob = (const uint32_t*)obs;
     const float* x = (const float*)obs;
     int64_t xss = orps * D;
-    if (gather || train) {   // training also needs the input sums for the (dummy or real) input BatchNorm
+    if (bits) {
+      if (!bits_tc) {   // tensor-core path off: the gathered bits as fp32 rows, then the fp32 MLP path below
+        bits::launch_expand(ob, orps, gather, rows, D, w.xg, S, st);
+        x = w.xg;
+      }
+      xss = (int64_t)rows * D;
+    } else if (gather || train) {   // training also needs the input sums for the (dummy or real) input BatchNorm
       { LaunchScope _ls(K_GATHER_ROWS, st); gather_rows_kernel<<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(x, orps, gather, w.xg, rows, D); }
       x = w.xg;
       xss = (int64_t)rows * D;
@@ -874,7 +907,9 @@ static int norm_forward(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
       x = w.xg;
     }
     if (train || d->norm_input) {
-      if (train) {
+      if (train && bits_tc) {
+        bits::launch_counts(ob, orps, gather, rows, D, w.bw, w.sums, bn_sums, S, st);
+      } else if (train) {
         colsum2(x, x, S, rows, D, D, w, w.sums, nullptr, 0, -1, -1, st);
         if (bn_sums) cudaMemcpyAsync(bn_sums, w.sums, (size_t)S * 2 * D * sizeof(float), cudaMemcpyDeviceToDevice, st);
       }
@@ -882,7 +917,23 @@ static int norm_forward(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
       { LaunchScope _ls(K_NORM_FWD, st); bn_prepare_kernel<<<S, 256, 0, st>>>(w.sums, (float)rows, train ? nullptr : batch_stats, sstride, D, train, 0.99f, w.mr_in); }
     }
     const float* xin = x;
-    if (d->norm_input) {
+    const float* b0 = params + L.d0_b;   // bits_tc: Dense_0's bias, per seed at stride b0_stride
+    int64_t b0_stride = P;
+    const uint32_t* fl = nullptr;   // NORM_INPUT: features folded around 1 (bits flipped)
+    if (bits_tc) {
+      // NORM_INPUT: BN(x_f) = a0_f + bit * d_f folded into Dense_0' = diag(d) W0 and b0' = b0 + a0^T W0 per call
+      const float* dv = nullptr;
+      if (d->norm_input) {
+        { LaunchScope _ls(K_NORM_FWD, st);
+          bits::eff_kernel<<<dim3(cdiv(H, 128), S), 128, 0, st>>>(params, P, L.bn_scale, L.bn_bias, L.d0_w, L.d0_b, w.mr_in, D, H,
+                                                                  w.bw.aff, w.bw.flip, w.bw.beff); }
+        dv = w.bw.aff;
+        fl = w.bw.flip;
+        b0 = w.bw.beff;
+        b0_stride = H;
+      }
+      bits::launch_wfrag(params, P, L.d0_w, dv, fl, D, H, S, w.bw.wf, st);
+    } else if (d->norm_input) {
       { LaunchScope _ls(K_NORM_FWD, st); norm_elem_fwd_kernel<2><<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(x, (int64_t)rows * D, D, D, w.mr_in, params, P, L.bn_scale, L.bn_bias, nullptr, w.xn); }
       xin = w.xn;
     }
@@ -891,8 +942,10 @@ static int norm_forward(const pqn_net_desc_t* d, const pqn_net_layout_t& L, cons
     int kin = D;
     for (int l = 0; l < d->layers; ++l) {
       const DenseOff o = dense_off(L, H, l);
-      if ((rc = launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, (int64_t)rows * kin, kin, params, P, o.w, o.b, 0, 0, 0, 0, A,
-                      w.z[l], nullptr, nullptr, nullptr, rows, kin))) return rc;
+      if (l == 0 && bits_tc) {
+        if ((rc = bits::launch_fwd(ob, orps, gather, rows, D, H, w.bw.wf, b0, b0_stride, fl, w.z[0], S, st))) return rc;
+      } else if ((rc = launch_dense<3>(H, dim3(cdiv(rows, BM), S), st, cur, (int64_t)rows * kin, kin, params, P, o.w, o.b, 0, 0, 0, 0,
+                                       A, w.z[l], nullptr, nullptr, nullptr, rows, kin))) return rc;
       float* run = norm == NORM_BN ? batch_stats + stats_off(d, l) : nullptr;
       if ((rc = norm_layer_fwd(norm, w.z[l], S, rows, H, H, params, P, o.g, o.bi, run, sstride, train, w, w.mr[l],
                                norm == NORM_NONE ? nullptr : w.xh[l], w.rs[l], w.h[l], st))) return rc;
@@ -931,6 +984,8 @@ static int norm_loss_grad(const pqn_net_desc_t* d, const pqn_net_layout_t& L, co
     if (rc) return rc;
   } else {
     const int D = d->in_c, H = d->hidden;
+    const bool bits_tc = d->kind == PQN_NET_MLP_BITS && g_use_tc == 2;
+    const uint32_t* ob = (const uint32_t*)obs;
     const float* xin = d->norm_input ? w.xn : w.xg;
     for (int l = last; l >= 0; --l) {
       const DenseOff o = dense_off(L, H, l);
@@ -938,11 +993,24 @@ static int norm_loss_grad(const pqn_net_desc_t* d, const pqn_net_layout_t& L, co
                                w.mr[l], st))) return rc;
       const float* xprev = l == 0 ? xin : w.h[l - 1];
       const int kin = l == 0 ? D : H;
-      const int sp = wgrad_splits(ffma_tiles(kin, H), S, rows);
-      run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, w.d[l], (int64_t)rows * H, H, grads, P, o.w, rows, kin, S, sp, w.wgp, st);
+      // dz of a batch-normalised layer carries rstd (up to ~316): one sixteenth of the dense gradient scale keeps it far
+      // below the fp16 maximum
+      const float gs = grad_scale(rows) * (1.0f / 16.0f);
+      if (l == 0 && bits_tc && !d->norm_input) {
+        bits::launch_wgrad(ob, orps, gather, rows, D, H, w.d[0], gs, nullptr, grads + o.w, P, w.bw, S, st);
+      } else if (l == 0 && bits_tc) {
+        // G = bits^T dz0, then every NORM_INPUT gradient from G and sum_r dz0 (w.sums, left by norm_layer_bwd)
+        bits::launch_wgrad(ob, orps, gather, rows, D, H, w.d[0], gs, w.bw.flip, w.bw.G, (int64_t)D * H, w.bw, S, st);
+        LaunchScope _ls(K_NORM_BWD, st);
+        bits::grad_finish_kernel<<<dim3(cdiv(D, 8), S), 256, 0, st>>>(w.bw.G, w.sums, 2 * (int64_t)H, w.bw.aff, w.bw.flip, w.mr_in, params, P,
+                                                                      o.w, L.bn_scale, L.bn_bias, D, H, grads);
+      } else {
+        const int sp = wgrad_splits(ffma_tiles(kin, H), S, rows);
+        run_wgrad_ffma(xprev, (int64_t)rows * kin, kin, w.d[l], (int64_t)rows * H, H, grads, P, o.w, rows, kin, S, sp, w.wgp, st);
+      }
       if (l > 0) launch_dgrad(w.d[l], (int64_t)rows * H, H, params, P, o.w, w.h[l - 1], w.d[l - 1], (int64_t)rows * H, rows, H, 0, S, st);
     }
-    if (d->norm_input) {   // the input BatchNorm is on the path: gradients of its scale / bias
+    if (d->norm_input && !bits_tc) {   // the input BatchNorm is on the path: gradients of its scale / bias
       { LaunchScope _ls(K_DGRAD, st); dgrad_small_kernel<<<dim3(cdiv(rows, 8), S), 256, 0, st>>>(w.d[0], rows, H, params, P, L.d0_w, D, w.dxn); }
       { LaunchScope _ls(K_NORM_BWD, st); in_xhat_kernel<<<dim3(cdiv((int64_t)rows * D, 256), S), 256, 0, st>>>(w.xg, (int64_t)rows * D, D, w.mr_in, w.xhin); }
       colsum2(w.dxn, w.xhin, S, rows, D, D, w, w.dg, grads, P, L.bn_bias, L.bn_scale, st);

@@ -25,7 +25,7 @@ import numpy as np
 import torch
 
 from . import _lib, envs, jaxrandom as jr
-from .networks import NET_CNN, NET_MLP, QNetworkSpec
+from .networks import NET_CNN, NET_MLP, NET_MLP_BITS, QNetworkSpec
 
 INFO_KEYS = ("returned_episode_returns", "returned_episode_lengths", "timestep", "returned_episode", "discount")
 
@@ -73,6 +73,25 @@ class TrainState(SimpleNamespace):
     and the optimizer moments."""
 
 
+def network_spec(env, network: str, c: dict):
+    """(QNetworkSpec, int32/float32 words per stored obs row, their torch dtype) of the engine's Q-network on `env`
+    (host-side: allocates nothing).  "cnn": the MinAtar CNN on packed rows; "mlp": the MLP QNetwork, on float rows for
+    classic control / bsuite and on the packed rows of a MinAtar env behind FlattenObservationWrapper
+    (PQN_NET_MLP_BITS)."""
+    norm_type, norm_input = c.get("NORM_TYPE", "layer_norm"), bool(c.get("NORM_INPUT", False))
+    if network == "cnn":
+        if not env.binary_obs:
+            raise ValueError("the MinAtar CNN needs a (10,10,C) binary-observation env")
+        spec = QNetworkSpec(NET_CNN, env.info.obs_shape[2], env.num_actions, norm_type=norm_type, norm_input=norm_input)
+        return spec, env.packed_obs_words, torch.int32
+    kind = NET_MLP_BITS if env.binary_obs else NET_MLP
+    spec = QNetworkSpec(kind, env.obs_dim, env.num_actions, int(c.get("HIDDEN_SIZE", 128)), int(c.get("NUM_LAYERS", 2)),
+                        norm_type=norm_type, norm_input=norm_input)
+    if env.binary_obs:
+        return spec, env.packed_obs_words, torch.int32
+    return spec, env.obs_dim, torch.float32
+
+
 class PQNEngine:
     def __init__(self, config: dict, network: str, flatten_obs: bool, device=None):
         self.cfg = config
@@ -81,7 +100,6 @@ class PQNEngine:
             raise _lib.PqnError("purejaxql_b200 needs a CUDA device: there is no CPU fallback")
         _lib.lib()
         c = config
-        norm_type, norm_input = c.get("NORM_TYPE", "layer_norm"), bool(c.get("NORM_INPUT", False))
         self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
         self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=flatten_obs, rng_mode=self.rng_mode)
         self.max_steps = int(self.env_params.max_steps_in_episode)
@@ -91,20 +109,7 @@ class PQNEngine:
         self.A = self.env.num_actions
         self.binary = self.env.binary_obs
         self.network = network
-        if network == "cnn":
-            if not self.binary:
-                raise ValueError("the MinAtar CNN needs a (10,10,C) binary-observation env")
-            self.spec = QNetworkSpec(NET_CNN, self.env.info.obs_shape[2], self.A, norm_type=norm_type,
-                                     norm_input=norm_input)
-            self.row_words = self.env.packed_obs_words          # int32 words per obs row
-            self.obs_dtype = torch.int32
-        else:
-            self.spec = QNetworkSpec(NET_MLP, self.env.obs_dim, self.A, int(c.get("HIDDEN_SIZE", 128)),
-                                     int(c.get("NUM_LAYERS", 2)), norm_type=norm_type, norm_input=norm_input)
-            if self.binary:
-                raise NotImplementedError("MLP on packed MinAtar observations is not built")
-            self.row_words = self.env.obs_dim
-            self.obs_dtype = torch.float32
+        self.spec, self.row_words, self.obs_dtype = network_spec(self.env, network, c)
         self.nmb = int(c["NUM_MINIBATCHES"])
         self.epochs = int(c["NUM_EPOCHS"])
         self.mb = self.T * self.E // self.nmb
@@ -235,7 +240,7 @@ class PQNEngine:
         ws = self._workspace(S, max(mb, E))
         perm_ws = jr.permutation_workspace(T * E, S, dev)
         denom = float(self.epochs * self.nmb)
-        bn_count = float(mb * world * (100 if self.binary else 1))
+        bn_count = float(mb * world * (100 if self.network == "cnn" else 1))   # CNN: per channel over 10x10 pixels
 
         def allreduce_(t, avg):
             if world > 1:

@@ -27,16 +27,16 @@ class PQNRnnEngine:
     def __init__(self, config: dict, device=None, env_params: envs.EnvParams | None = None):
         self.cfg = c = config
         self.device = torch.device(device or "cuda")
+        self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
+        self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=True, rng_mode=self.rng_mode)
+        if self.env.binary_obs:   # its memory buffer stores float observation rows
+            raise NotImplementedError("the recurrent script is built for the float-observation envs "
+                                      "(classic control, MemoryChain-bsuite)")
         if self.device.type != "cuda" or not torch.cuda.is_available():
             raise _lib.PqnError("purejaxql_b200 needs a CUDA device: there is no CPU fallback")
         _lib.lib()
-        self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
-        self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=True, rng_mode=self.rng_mode)
         if env_params is not None:                                   # e.g. MemoryChain's memory_length (:134-136)
             self.env_params = env_params
-        if self.env.binary_obs:
-            raise NotImplementedError("the recurrent script is built for the float-observation envs "
-                                      "(classic control, MemoryChain-bsuite)")
         self.max_steps = int(self.env_params.max_steps_in_episode)
         self.T, self.E, self.NU = int(c["NUM_STEPS"]), int(c["NUM_ENVS"]), int(c["NUM_UPDATES"])
         self.W = int(c["MEMORY_WINDOW"])

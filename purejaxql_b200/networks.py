@@ -25,6 +25,7 @@ from . import _lib
 NET_CNN = 0
 NET_MLP = 1
 NET_RNN = 2     # RNNQNetwork (GRU) of pqn_rnn_gymnax.py:57-105
+NET_MLP_BITS = 3   # the MLP QNetwork fed a MinAtar env's packed {0,1} observation rows (D = 100 * C inputs)
 
 
 class QNetworkSpec:

@@ -2,6 +2,10 @@
 purejaxql/pqn_gymnax.py.
 
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole NUM_SEEDS=8
+    python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=Breakout-MinAtar
+
+On a MinAtar game the flattened (10,10,C) observation feeds the MLP as in the reference; the rollout keeps it as
+packed bits and Dense_0 reads those directly (PQN_NET_MLP_BITS).
 
 Differences from pqn_minatar (as in the reference, pqn_gymnax.py:29-58,92-97):
 MLP ``QNetwork(HIDDEN_SIZE, NUM_LAYERS)`` without the /255, the observation is
