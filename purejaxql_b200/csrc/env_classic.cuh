@@ -180,4 +180,55 @@ struct AcrobotEnv {
   }
 };
 
+// gymnax classic_control/mountain_car.py (MountainCar-v0).  Restated from recollection of gymnax 0.0.6: the EnvParams
+// defaults below, the uniform(-0.6, -0.4) reset, the step order and the wall rule
+// `velocity *= 1 - (position == min_position) * (velocity < 0)`, which gives -0.0 for a negative velocity.
+struct MountainCarEnv {
+  static constexpr int ID = ENV_MOUNTAIN_CAR;
+  static constexpr int CORE_WORDS = 3;
+  static constexpr int STATE_WORDS = CORE_WORDS + LOG_WORDS;
+  static constexpr int NUM_ACTIONS = 3;
+  static constexpr int OBS_DIM = 2;
+  static constexpr bool BINARY_OBS = false;
+  static constexpr bool OBS_IN_REGS = false;
+  static constexpr int OBS_WORDS = 1, OBS_WORDS_PAD = 1;
+  static constexpr int DEFAULT_MAX_STEPS = 200;
+
+  struct State {
+    float position, velocity;
+    int time;
+  };
+
+  template <typename W>
+  PQN_HD static void load(State& s, const W* __restrict__ st, int64_t N, int64_t i) {
+    s.position = u2f(st[i]); s.velocity = u2f(st[N + i]); s.time = (int)st[2 * N + i];
+  }
+  PQN_HD static void store(const State& s, uint32_t* __restrict__ st, int64_t N, int64_t i) {
+    st[i] = f2u(s.position); st[N + i] = f2u(s.velocity); st[2 * N + i] = (uint32_t)s.time;
+  }
+
+  PQN_HD static void reset_env(Key key, int part, int /*max_steps*/, State& s) {
+    // jax.random.uniform(key, shape=(), minval=-0.6, maxval=-0.4)
+    s.position = uniform_from_bits(bits_scalar(key, part), -0.6f, -0.4f);
+    s.velocity = 0.f;
+    s.time = 0;
+  }
+
+  PQN_HD static void step_env(Key /*key*/, int /*part*/, int max_steps, State& s, int action, float& reward,
+                              bool& done) {
+    const float min_position = -1.2f, max_position = 0.6f, max_speed = 0.07f;
+    const float goal_position = 0.5f, goal_velocity = 0.0f, force = 0.001f, gravity = 0.0025f;
+    float velocity = s.velocity + (float)(action - 1) * force - cosf(3.0f * s.position) * gravity;
+    velocity = fminf(fmaxf(velocity, -max_speed), max_speed);
+    float position = s.position + velocity;
+    position = fminf(fmaxf(position, min_position), max_position);
+    velocity = velocity * (float)(1 - ((position == min_position && velocity < 0.f) ? 1 : 0));
+    reward = -1.0f;
+    s.position = position; s.velocity = velocity; s.time = s.time + 1;
+    done = (position >= goal_position && velocity >= goal_velocity) || s.time >= max_steps;
+  }
+
+  PQN_HD static void obs_float(const State& s, float (&o)[OBS_DIM]) { o[0] = s.position; o[1] = s.velocity; }
+};
+
 }  // namespace pqn

@@ -27,7 +27,9 @@ enum EnvId : int {
   ENV_SEAQUEST = 4,
   ENV_CARTPOLE = 16,
   ENV_ACROBOT = 17,
+  ENV_MOUNTAIN_CAR = 18,
   ENV_MEMORY_CHAIN = 32,
+  ENV_CATCH = 33,
 };
 
 constexpr int LOG_WORDS = 5;

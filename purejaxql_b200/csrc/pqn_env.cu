@@ -12,6 +12,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <type_traits>
 
 #include "../../include/pqn_b200.h"
 #include "api_common.h"
@@ -335,6 +336,17 @@ __global__ void threefry_kernel(const uint32_t* __restrict__ kp, const uint32_t*
 // ---------------------------------------------------------------------------
 // host-side dispatch
 // ---------------------------------------------------------------------------
+// gymnax's unflattened observation shape of a float-observation env: a vector of OBS_DIM, or the (OBS_ROWS, OBS_COLS)
+// board of an env that defines them (Catch-bsuite)
+template <class Env, class = void>
+struct FloatObsShape {
+  static constexpr int ROWS = Env::OBS_DIM, COLS = 1;
+};
+template <class Env>
+struct FloatObsShape<Env, std::void_t<decltype(Env::OBS_ROWS)>> {
+  static constexpr int ROWS = Env::OBS_ROWS, COLS = Env::OBS_COLS;
+};
+
 template <class Env>
 static void fill_info(pqn_env_info_t* o) {
   o->state_words = Env::STATE_WORDS;
@@ -346,7 +358,7 @@ static void fill_info(pqn_env_info_t* o) {
     o->obs_shape[0] = Env::OBS_H; o->obs_shape[1] = Env::OBS_W; o->obs_shape[2] = Env::OBS_C;
     o->packed_obs_words = Env::OBS_WORDS_PAD;
   } else {
-    o->obs_shape[0] = Env::OBS_DIM; o->obs_shape[1] = 1; o->obs_shape[2] = 1;
+    o->obs_shape[0] = FloatObsShape<Env>::ROWS; o->obs_shape[1] = FloatObsShape<Env>::COLS; o->obs_shape[2] = 1;
     o->packed_obs_words = 0;
   }
 }
@@ -359,7 +371,9 @@ static void fill_info(pqn_env_info_t* o) {
     case ENV_SPACE_INVADERS: { using EnvT = SpaceInvadersEnv; __VA_ARGS__; } break; \
     case ENV_CARTPOLE: { using EnvT = CartPoleEnv; __VA_ARGS__; } break;        \
     case ENV_ACROBOT: { using EnvT = AcrobotEnv; __VA_ARGS__; } break;          \
+    case ENV_MOUNTAIN_CAR: { using EnvT = MountainCarEnv; __VA_ARGS__; } break; \
     case ENV_MEMORY_CHAIN: { using EnvT = MemoryChainEnv; __VA_ARGS__; } break; \
+    case ENV_CATCH: { using EnvT = CatchEnv; __VA_ARGS__; } break;              \
     default: return set_error(PQN_E_UNSUPPORTED, "env id %d is not built into libpqn_b200", env_id); \
   }
 

@@ -658,7 +658,8 @@ __global__ void conv_grad_finish_kernel(const float* __restrict__ dw_part, int n
   }
 }
 
-// MLP input: d x_n[row][j] = sum_n dz0[row][n] * W0[j][n]   (D <= 16 input features), one warp per row
+// MLP / GRU input: d x_n[row][j] = sum_n dz0[row][n] * W0[j][n], one warp per row and the D input features in turn.
+// Built for narrow inputs (classic control, bsuite: D <= 50); any D runs, at D shuffle reductions per row.
 __global__ void dgrad_small_kernel(const float* __restrict__ DZ, int rows, int H, const float* __restrict__ params,
                                    int64_t P, int64_t off_w, int D, float* __restrict__ DX) {
   const int seed = blockIdx.y, lane = threadIdx.x & 31;
@@ -703,7 +704,8 @@ struct NormWs {
 // channels per seed of the (sum, sum of squares) / (mean, rstd) tables: every per-channel reduction of the network
 static int64_t chan_floats(const pqn_net_desc_t* d) {
   int64_t m = d->kind != PQN_NET_MINATAR_CNN && d->hidden > 256 ? d->hidden : 256;
-  if (d->kind == PQN_NET_MLP_BITS && d->in_c > m) m = d->in_c;   // the input features' statistics
+  // the input features' statistics
+  if ((d->kind == PQN_NET_MLP_BITS || d->kind == PQN_NET_RNN) && d->in_c > m) m = d->in_c;
   return 2 * m;
 }
 

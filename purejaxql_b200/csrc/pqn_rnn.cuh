@@ -360,16 +360,16 @@ static int check_rnn(const pqn_net_desc_t* d, const char* who) {
 }
 
 // the *_stats entry points: every NORM_TYPE / NORM_INPUT; batch_stats may be NULL only for the default network.  The
-// input BatchNorm's statistics are column sums over D <= 16 features (colsum2's per-row path) or D dividing 256.
+// input BatchNorm's statistics are colsum2 column sums over G == D features, which it builds for D <= 1024; the
+// per-channel tables (nrm::chan_floats) grow with D beyond 256.
 static int check_rnn_stats(const pqn_net_desc_t* d, const float* batch_stats, const char* who) {
   if (d->kind != PQN_NET_RNN) return set_error(PQN_E_INVALID, "%s: not an RNN descriptor", who);
   if (modular_rnn(d) && !batch_stats)
     return set_error(PQN_E_INVALID, "%s: NORM_TYPE=%s, NORM_INPUT=%d needs the batch_stats block (NULL given)", who,
                      d->norm_type == PQN_NORM_BATCH ? "batch_norm" : (d->norm_type == PQN_NORM_LAYER ? "layer_norm" : "none"),
                      d->norm_input);
-  if (batch_stats && d->in_c > 16 && 256 % d->in_c != 0)
-    return set_error(PQN_E_UNSUPPORTED, "%s: input BatchNorm over %d features (at most 16, or a divisor of 256, built)",
-                     who, d->in_c);
+  if (batch_stats && d->in_c > 1024)
+    return set_error(PQN_E_UNSUPPORTED, "%s: input BatchNorm over %d features (at most 1024 built)", who, d->in_c);
   return PQN_OK;
 }
 

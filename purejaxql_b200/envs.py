@@ -31,7 +31,9 @@ ENV_IDS = {
     "Freeway-MinAtar": 3,
     "CartPole-v1": 16,
     "Acrobot-v1": 17,
+    "MountainCar-v0": 18,
     "MemoryChain-bsuite": 32,
+    "Catch-bsuite": 33,
 }
 # PQN_ENV_SEAQUEST (4) is reserved in include/pqn_b200.h but not built: gymnax 0.0.6 (the reference's pin) does not
 # register "Seaquest-MinAtar" in gymnax.make either (DESIGN.md section 8), so the reference cannot run it.
@@ -143,6 +145,20 @@ def state_to_fields(env_name: str, state: torch.Tensor) -> dict:
             f[k] = _u2f(st[j])
         f["time"] = st[4]
         core = 5
+    elif env_name == "MountainCar-v0":
+        f["position"] = _u2f(st[0])
+        f["velocity"] = _u2f(st[1])
+        f["time"] = st[2]
+        core = 3
+    elif env_name == "Catch-bsuite":
+        w = st[0]
+        f["ball_x"] = w & 15
+        f["ball_y"] = (w >> 4) & 15
+        f["paddle_x"] = (w >> 8) & 15
+        f["paddle_y"] = (w >> 12) & 15
+        f["prev_done"] = ((w >> 16) & 1).bool()
+        f["time"] = st[1]
+        core = 2
     elif env_name == "MemoryChain-bsuite":
         f["context"] = (st[0] != 0).unsqueeze(1)                           # [N, num_bits = 1]
         for j, k in enumerate(("query", "total_perfect", "total_regret", "time", "memory_length"), 1):
@@ -218,6 +234,11 @@ def fields_to_state(env_name: str, f: dict) -> torch.Tensor:
     elif env_name == "Acrobot-v1":
         core = [_f2u(torch.as_tensor(f[k])) for k in
                 ("joint_angle1", "joint_angle2", "velocity_1", "velocity_2")] + [i32(f["time"])]
+    elif env_name == "MountainCar-v0":
+        core = [_f2u(torch.as_tensor(f[k])) for k in ("position", "velocity")] + [i32(f["time"])]
+    elif env_name == "Catch-bsuite":
+        core = [i32(f["ball_x"]) | (i32(f["ball_y"]) << 4) | (i32(f["paddle_x"]) << 8) | (i32(f["paddle_y"]) << 12)
+                | (i32(f["prev_done"]) << 16), i32(f["time"])]
     elif env_name == "MemoryChain-bsuite":
         ctx = i32(f["context"])
         core = [ctx.reshape(ctx.shape[0], -1)[:, 0]] + [i32(f[k]) for k in
@@ -274,7 +295,10 @@ class BatchedEnv:
         self.binary_obs = bool(info.binary_obs)
         self.packed_obs_words = info.packed_obs_words
         self.num_actions = info.num_actions
-        shape = tuple(info.obs_shape) if self.binary_obs else (info.obs_dim,)
+        if self.binary_obs:
+            shape = tuple(info.obs_shape)
+        else:   # a vector, or a 2-D board (Catch-bsuite's (10, 5)): gymnax's unflattened shape
+            shape = (info.obs_shape[0], info.obs_shape[1]) if info.obs_shape[1] > 1 else (info.obs_dim,)
         self._obs_shape = (info.obs_dim,) if flatten_obs else shape
         self.default_params = EnvParams(max_steps_in_episode=info.max_steps)
         self.rng_mode = rng_mode

@@ -1,7 +1,12 @@
-"""Recurrent (GRU) PQN on gymnax classic control and MemoryChain-bsuite — drop-in for purejaxql/pqn_rnn_gymnax.py.
+"""Recurrent (GRU) PQN on the float-observation gymnax envs — drop-in for purejaxql/pqn_rnn_gymnax.py.
 
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole NUM_SEEDS=4
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_memory_chain
+    python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=MountainCar-v0
+    python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=Catch-bsuite
+
+The envs are CartPole-v1, Acrobot-v1, MountainCar-v0, MemoryChain-bsuite and Catch-bsuite (50 inputs: every
+NORM_TYPE / NORM_INPUT runs on it).  The MinAtar games are refused: the memory stores float observation rows.
 
 ``make_train(config)`` keeps the reference's contract (pqn_rnn_gymnax.py:117-560): config mutation (NUM_UPDATES,
 NUM_UPDATES_DECAY, TEST_NUM_STEPS), ``RNNQNetwork`` (MLP trunk -> one-hot last action -> scanned GRU with done-resets ->
