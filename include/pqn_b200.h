@@ -46,13 +46,17 @@ extern "C" {
 #define PQN_ENV_MOUNTAIN_CAR 18   /* "MountainCar-v0" */
 #define PQN_ENV_MEMORY_CHAIN 32   /* "MemoryChain-bsuite" */
 #define PQN_ENV_CATCH 33          /* "Catch-bsuite" */
+#define PQN_ENV_DEEP_SEA 34       /* "DeepSea-bsuite" */
+#define PQN_ENV_UMBRELLA_CHAIN 35 /* "UmbrellaChain-bsuite" */
+#define PQN_ENV_DISCOUNTING_CHAIN 36 /* "DiscountingChain-bsuite" */
 
 typedef struct pqn_env_info_t {
   int32_t state_words;      /* uint32 words per env in the SoA state block (incl. 5 LogWrapper words) */
   int32_t obs_dim;          /* flattened observation length (400 Breakout, 4 CartPole, 6 Acrobot, 2 MountainCar,
-                               3 MemoryChain, 50 Catch) */
-  int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control and MemoryChain, (10, 5, 1) for
-                               Catch's board; obs buffers hold the obs_dim floats of an env contiguously either way */
+                               3 MemoryChain, 50 Catch, 64 DeepSea, 3 UmbrellaChain, 2 DiscountingChain) */
+  int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control, MemoryChain, UmbrellaChain and
+                               DiscountingChain, (10, 5, 1) for Catch's board and (8, 8, 1) for DeepSea's; obs buffers
+                               hold the obs_dim floats of an env contiguously either way */
   int32_t num_actions;      /* env.action_space(params).n  — pqn_minatar.py:151 */
   int32_t max_steps;        /* env_params.max_steps_in_episode default — pqn_minatar.py:105 */
   int32_t binary_obs;       /* 1: obs are {0,1}; the rollout buffer stores them bit-packed */

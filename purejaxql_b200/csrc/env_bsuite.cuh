@@ -149,4 +149,228 @@ struct CatchEnv {
   }
 };
 
+// gymnax bsuite/deep_sea.py (DeepSea-bsuite) with the constructor's size 8 and the default EnvParams
+// (deterministic = True, unscaled_move_cost = 0.01).  Restated from recollection of gymnax 0.0.6:
+//   reset_env:  row = column = 0, bad_episode = False, total_bad_episodes = denoised_return = 0,
+//               optimal_no_cost = 1.0, optimal_return = optimal_no_cost - unscaled_move_cost, time = 0;
+//               action_mapping = ones((8, 8)) under deterministic = True (a per-env bernoulli draw otherwise)
+//   step_env:   right = action == action_mapping[row, column];
+//               reward = 0.0 + (right & row == 7 & column == 7) - right * unscaled_move_cost / 8;
+//               a left move at row == column sets bad_episode; column = clip(column +- 1, 0, 7); row += 1;
+//               total_bad_episodes += bad_episode at row == 8; time += 1;
+//               done = row == 8 || time >= max_steps_in_episode, so an episode lasts 8 steps
+//   get_obs:    the (8, 8) one-hot of (row, column), all zeros once row == 8
+// gymnax's step_env also draws a uniform (a right move succeeds when it exceeds 1 / size, or under deterministic) and
+// a normal (reward noise, multiplied by 1 - deterministic) from its key.  At deterministic = True the uniform's
+// condition is or-ed with True, and the noise term is 0 * finite = +-0.0 (jax.random.normal is finite: it maps a
+// uniform in (-1, 1) through erfinv).  Adding +-0.0 to a reward that starts as +0.0 + bool leaves it bit for bit as
+// it is (+0 + -0 = +0 in round-to-nearest), so neither draw can reach an output and this step does not make them.
+// Integer work plus fp32 constants: bit-exact.
+struct DeepSeaEnv {
+  static constexpr int ID = ENV_DEEP_SEA;
+  static constexpr int SIZE = 8;
+  static constexpr int CORE_WORDS = 8;
+  static constexpr int STATE_WORDS = CORE_WORDS + LOG_WORDS;
+  static constexpr int NUM_ACTIONS = 2;
+  static constexpr int OBS_DIM = SIZE * SIZE;
+  static constexpr int OBS_ROWS = SIZE, OBS_COLS = SIZE;  // gymnax's (8, 8) board, unflattened
+  static constexpr bool BINARY_OBS = false;
+  static constexpr bool OBS_IN_REGS = false;
+  static constexpr int OBS_WORDS = 1, OBS_WORDS_PAD = 1;
+  static constexpr int DEFAULT_MAX_STEPS = 2000;  // EnvParams.max_steps_in_episode; episodes end on the last row
+  static constexpr float UNSCALED_MOVE_COST = 0.01f;
+  static constexpr float MOVE_COST = UNSCALED_MOVE_COST / SIZE;  // exact: a power-of-two divisor
+
+  // word 0: row | column << 8 | bad_episode << 16;  1: total_bad_episodes;  2: denoised_return;
+  // 3, 4: optimal_return, optimal_no_cost (fp32 bits);  5, 6: action_mapping, bit 8 * row + column;  7: time
+  struct State {
+    int row, column, bad_episode, total_bad_episodes, denoised_return;
+    float optimal_return, optimal_no_cost;
+    uint32_t map_lo, map_hi;
+    int time;
+  };
+
+  template <typename W>
+  PQN_HD static void load(State& s, const W* __restrict__ st, int64_t N, int64_t i) {
+    const uint32_t w = (uint32_t)st[i];
+    s.row = (int)(w & 255u); s.column = (int)((w >> 8) & 255u); s.bad_episode = (int)((w >> 16) & 1u);
+    s.total_bad_episodes = (int)st[N + i]; s.denoised_return = (int)st[2 * N + i];
+    s.optimal_return = u2f((uint32_t)st[3 * N + i]); s.optimal_no_cost = u2f((uint32_t)st[4 * N + i]);
+    s.map_lo = (uint32_t)st[5 * N + i]; s.map_hi = (uint32_t)st[6 * N + i]; s.time = (int)st[7 * N + i];
+  }
+  PQN_HD static void store(const State& s, uint32_t* __restrict__ st, int64_t N, int64_t i) {
+    st[i] = (uint32_t)s.row | ((uint32_t)s.column << 8) | ((uint32_t)s.bad_episode << 16);
+    st[N + i] = (uint32_t)s.total_bad_episodes; st[2 * N + i] = (uint32_t)s.denoised_return;
+    st[3 * N + i] = f2u(s.optimal_return); st[4 * N + i] = f2u(s.optimal_no_cost);
+    st[5 * N + i] = s.map_lo; st[6 * N + i] = s.map_hi; st[7 * N + i] = (uint32_t)s.time;
+  }
+
+  PQN_HD static void reset_env(Key /*key*/, int /*part*/, int /*max_steps*/, State& s) {
+    s.row = 0; s.column = 0; s.bad_episode = 0; s.total_bad_episodes = 0; s.denoised_return = 0;
+    s.optimal_no_cost = 1.0f;
+    s.optimal_return = s.optimal_no_cost - UNSCALED_MOVE_COST;
+    s.map_lo = 0xFFFFFFFFu; s.map_hi = 0xFFFFFFFFu;  // ones((8, 8)): deterministic = True
+    s.time = 0;
+  }
+
+  PQN_HD static void step_env(Key /*key*/, int /*part*/, int max_steps, State& s, int action, float& reward,
+                              bool& done) {
+    const int bit = s.row * SIZE + s.column;
+    const uint32_t map_word = bit < 32 ? s.map_lo : s.map_hi;
+    const bool right = action == (int)((map_word >> (bit & 31)) & 1u);
+    const bool treasure = right && s.row == SIZE - 1 && s.column == SIZE - 1;
+    reward = (treasure ? 1.f : 0.f) - (right ? MOVE_COST : 0.f);
+    s.denoised_return += treasure ? 1 : 0;
+    if (!right && s.row == s.column) s.bad_episode = 1;
+    s.column = right ? (s.column + 1 > SIZE - 1 ? SIZE - 1 : s.column + 1) : (s.column - 1 < 0 ? 0 : s.column - 1);
+    s.row = s.row + 1;
+    if (s.row == SIZE) s.total_bad_episodes += s.bad_episode;
+    s.time = s.time + 1;
+    done = s.row == SIZE || s.time >= max_steps;
+  }
+
+  // compares instead of an indexed write, so that `o` stays in registers
+  PQN_HD static void obs_float(const State& s, float (&o)[OBS_DIM]) {
+    const int hot = s.row < SIZE ? s.row * SIZE + s.column : -1;
+#pragma unroll
+    for (int j = 0; j < OBS_DIM; ++j) o[j] = j == hot ? 1.f : 0.f;
+  }
+};
+
+// gymnax bsuite/umbrella_chain.py (UmbrellaChain-bsuite) with n_distractor = 0, as `gymnax.make` builds it, and
+// chain_length = 10.  Restated from recollection of gymnax 0.0.6:
+//   reset_env:  k_need, k_has, k_obs = split(key, 3); need_umbrella = bernoulli(k_need, 0.5, ()),
+//               has_umbrella = bernoulli(k_has, 0.5, ()), total_regret = 0, time = 0 (k_obs feeds the distractors)
+//   step_env:   k_reward, k_obs = split(key); has_umbrella = action if time == 0;
+//               chain_full = time + 1 == chain_length;
+//               reward = +-1 by has_umbrella == need_umbrella if chain_full, else 2 * bernoulli(k_reward, 0.5, ()) - 1;
+//               total_regret += 2 * (chain_full & !match); time += 1;
+//               done = time == chain_length || time >= max_steps_in_episode, so an episode lasts 10 steps
+//   get_obs:    [need_umbrella, has_umbrella, 1 - time / chain_length]
+// Integer logic plus one fp32 division: bit-exact.
+struct UmbrellaChainEnv {
+  static constexpr int ID = ENV_UMBRELLA_CHAIN;
+  static constexpr int CHAIN_LENGTH = 10;
+  static constexpr int CORE_WORDS = 4;
+  static constexpr int STATE_WORDS = CORE_WORDS + LOG_WORDS;
+  static constexpr int NUM_ACTIONS = 2;
+  static constexpr int OBS_DIM = 3;  // 3 + n_distractor, flattened from (1, 3)
+  static constexpr bool BINARY_OBS = false;
+  static constexpr bool OBS_IN_REGS = false;
+  static constexpr int OBS_WORDS = 1, OBS_WORDS_PAD = 1;
+  static constexpr int DEFAULT_MAX_STEPS = 100;  // EnvParams.max_steps_in_episode; episodes end on chain_length
+
+  // words: need_umbrella, has_umbrella, total_regret, time
+  struct State {
+    int need_umbrella, has_umbrella, total_regret, time;
+  };
+
+  template <typename W>
+  PQN_HD static void load(State& s, const W* __restrict__ st, int64_t N, int64_t i) {
+    s.need_umbrella = (int)st[i]; s.has_umbrella = (int)st[N + i]; s.total_regret = (int)st[2 * N + i];
+    s.time = (int)st[3 * N + i];
+  }
+  PQN_HD static void store(const State& s, uint32_t* __restrict__ st, int64_t N, int64_t i) {
+    st[i] = (uint32_t)s.need_umbrella; st[N + i] = (uint32_t)s.has_umbrella;
+    st[2 * N + i] = (uint32_t)s.total_regret; st[3 * N + i] = (uint32_t)s.time;
+  }
+
+  PQN_HD static int coin(Key k, int part) { return uniform_scalar(k, part) < 0.5f ? 1 : 0; }  // bernoulli(k, 0.5, ())
+
+  PQN_HD static void reset_env(Key key, int part, int /*max_steps*/, State& s) {
+    Key k_need, k_has, k_obs;
+    split3(key, part, k_need, k_has, k_obs);
+    s.need_umbrella = coin(k_need, part);
+    s.has_umbrella = coin(k_has, part);
+    s.total_regret = 0; s.time = 0;
+  }
+
+  PQN_HD static void step_env(Key key, int part, int max_steps, State& s, int action, float& reward, bool& done) {
+    if (s.time == 0) s.has_umbrella = action;
+    const bool chain_full = s.time + 1 == CHAIN_LENGTH;
+    const bool match = s.has_umbrella == s.need_umbrella;
+    if (chain_full) {
+      reward = match ? 1.f : -1.f;
+    } else {
+      Key k_reward, k_obs;
+      split2(key, part, k_reward, k_obs);
+      reward = (float)(2 * coin(k_reward, part) - 1);
+    }
+    s.total_regret += (chain_full && !match) ? 2 : 0;
+    s.time = s.time + 1;
+    done = s.time == CHAIN_LENGTH || s.time >= max_steps;
+  }
+
+  // fp32 IEEE division (this TU is built with -fmad=false and the division is not fast-math)
+  PQN_HD static void obs_float(const State& s, float (&o)[OBS_DIM]) {
+    o[0] = (float)s.need_umbrella;
+    o[1] = (float)s.has_umbrella;
+    o[2] = 1.0f - (float)s.time / (float)CHAIN_LENGTH;
+  }
+};
+
+// gymnax bsuite/discounting_chain.py (DiscountingChain-bsuite) with mapping_seed = None, as `gymnax.make` builds it.
+// Restated from recollection of gymnax 0.0.6:
+//   reset_env:  context = -1, time = 0; rewards = ones(5).at[randint(key, (), 0, 5)].set(1.1)
+//   step_env:   context = action if time == 0; time += 1;
+//               reward = rewards[context] if time == reward_timestep[context] else 0.0,
+//               reward_timestep = [1, 3, 10, 30, 100]; done = time >= max_steps_in_episode (100)
+//   get_obs:    [context, time / max_steps_in_episode]
+// The state keeps the index of the 1.1 reward (mapped_action) rather than the five rewards, so a mapping fixed by
+// mapping_seed fits the same word.  It also keeps max_steps_in_episode, the observation's divisor: the reset kernels
+// pass it to reset_env, and the auto-reset inside a step passes the same value.  Integer logic plus one fp32 division:
+// bit-exact.
+struct DiscountingChainEnv {
+  static constexpr int ID = ENV_DISCOUNTING_CHAIN;
+  static constexpr int CORE_WORDS = 4;
+  static constexpr int STATE_WORDS = CORE_WORDS + LOG_WORDS;
+  static constexpr int NUM_ACTIONS = 5;
+  static constexpr int OBS_DIM = 2;  // flattened from (1, 2)
+  static constexpr bool BINARY_OBS = false;
+  static constexpr bool OBS_IN_REGS = false;
+  static constexpr int OBS_WORDS = 1, OBS_WORDS_PAD = 1;
+  static constexpr int DEFAULT_MAX_STEPS = 100;  // EnvParams.max_steps_in_episode: every episode lasts this long
+  static constexpr float MAPPED_REWARD = 1.1f;
+
+  PQN_HD static int reward_timestep(int context) {
+    return context == 0 ? 1 : context == 1 ? 3 : context == 2 ? 10 : context == 3 ? 30 : 100;
+  }
+
+  // words: context (-1 until the first step), mapped_action, time, max_steps_in_episode
+  struct State {
+    int context, mapped_action, time, max_steps;
+  };
+
+  template <typename W>
+  PQN_HD static void load(State& s, const W* __restrict__ st, int64_t N, int64_t i) {
+    s.context = (int)st[i]; s.mapped_action = (int)st[N + i]; s.time = (int)st[2 * N + i];
+    s.max_steps = (int)st[3 * N + i];
+  }
+  PQN_HD static void store(const State& s, uint32_t* __restrict__ st, int64_t N, int64_t i) {
+    st[i] = (uint32_t)s.context; st[N + i] = (uint32_t)s.mapped_action; st[2 * N + i] = (uint32_t)s.time;
+    st[3 * N + i] = (uint32_t)s.max_steps;
+  }
+
+  PQN_HD static void reset_env(Key key, int part, int max_steps, State& s) {
+    s.context = -1;
+    s.mapped_action = randint_scalar(key, (uint32_t)NUM_ACTIONS, part);
+    s.time = 0;
+    s.max_steps = max_steps;
+  }
+
+  PQN_HD static void step_env(Key /*key*/, int /*part*/, int max_steps, State& s, int action, float& reward,
+                              bool& done) {
+    if (s.time == 0) s.context = action;
+    s.time = s.time + 1;
+    reward = s.time == reward_timestep(s.context) ? (s.context == s.mapped_action ? MAPPED_REWARD : 1.0f) : 0.f;
+    done = s.time >= max_steps;
+  }
+
+  // fp32 IEEE division (this TU is built with -fmad=false and the division is not fast-math)
+  PQN_HD static void obs_float(const State& s, float (&o)[OBS_DIM]) {
+    o[0] = (float)s.context;
+    o[1] = (float)s.time / (float)s.max_steps;
+  }
+};
+
 }  // namespace pqn

@@ -30,6 +30,9 @@ enum EnvId : int {
   ENV_MOUNTAIN_CAR = 18,
   ENV_MEMORY_CHAIN = 32,
   ENV_CATCH = 33,
+  ENV_DEEP_SEA = 34,
+  ENV_UMBRELLA_CHAIN = 35,
+  ENV_DISCOUNTING_CHAIN = 36,
 };
 
 constexpr int LOG_WORDS = 5;

@@ -337,7 +337,7 @@ __global__ void threefry_kernel(const uint32_t* __restrict__ kp, const uint32_t*
 // host-side dispatch
 // ---------------------------------------------------------------------------
 // gymnax's unflattened observation shape of a float-observation env: a vector of OBS_DIM, or the (OBS_ROWS, OBS_COLS)
-// board of an env that defines them (Catch-bsuite)
+// board of an env that defines them (Catch-bsuite, DeepSea-bsuite)
 template <class Env, class = void>
 struct FloatObsShape {
   static constexpr int ROWS = Env::OBS_DIM, COLS = 1;
@@ -374,6 +374,9 @@ static void fill_info(pqn_env_info_t* o) {
     case ENV_MOUNTAIN_CAR: { using EnvT = MountainCarEnv; __VA_ARGS__; } break; \
     case ENV_MEMORY_CHAIN: { using EnvT = MemoryChainEnv; __VA_ARGS__; } break; \
     case ENV_CATCH: { using EnvT = CatchEnv; __VA_ARGS__; } break;              \
+    case ENV_DEEP_SEA: { using EnvT = DeepSeaEnv; __VA_ARGS__; } break;         \
+    case ENV_UMBRELLA_CHAIN: { using EnvT = UmbrellaChainEnv; __VA_ARGS__; } break; \
+    case ENV_DISCOUNTING_CHAIN: { using EnvT = DiscountingChainEnv; __VA_ARGS__; } break; \
     default: return set_error(PQN_E_UNSUPPORTED, "env id %d is not built into libpqn_b200", env_id); \
   }
 

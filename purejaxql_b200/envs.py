@@ -34,6 +34,9 @@ ENV_IDS = {
     "MountainCar-v0": 18,
     "MemoryChain-bsuite": 32,
     "Catch-bsuite": 33,
+    "DeepSea-bsuite": 34,
+    "UmbrellaChain-bsuite": 35,
+    "DiscountingChain-bsuite": 36,
 }
 # PQN_ENV_SEAQUEST (4) is reserved in include/pqn_b200.h but not built: gymnax 0.0.6 (the reference's pin) does not
 # register "Seaquest-MinAtar" in gymnax.make either (DESIGN.md section 8), so the reference cannot run it.
@@ -164,6 +167,31 @@ def state_to_fields(env_name: str, state: torch.Tensor) -> dict:
         for j, k in enumerate(("query", "total_perfect", "total_regret", "time", "memory_length"), 1):
             f[k] = st[j]                                                    # memory_length: the EnvParams word
         core = 6
+    elif env_name == "DeepSea-bsuite":
+        w = st[0]
+        f["row"] = w & 255
+        f["column"] = (w >> 8) & 255
+        f["bad_episode"] = ((w >> 16) & 1).bool()
+        f["total_bad_episodes"] = st[1]
+        f["denoised_return"] = st[2]
+        f["optimal_return"] = _u2f(st[3])
+        f["optimal_no_cost"] = _u2f(st[4])
+        n = st.shape[1]
+        p = torch.arange(64, device=st.device)
+        words = st[5:7].to(torch.int64) & 0xFFFFFFFF                       # [2, N]
+        bits = (words[p >> 5] >> (p & 31).unsqueeze(1)) & 1                # [64, N]
+        f["action_mapping"] = bits.t().reshape(n, 8, 8).to(torch.float32)
+        f["time"] = st[7]
+        core = 8
+    elif env_name == "UmbrellaChain-bsuite":
+        for j, k in enumerate(("need_umbrella", "has_umbrella", "total_regret", "time")):
+            f[k] = st[j]
+        core = 4
+    elif env_name == "DiscountingChain-bsuite":
+        # gymnax keeps the five rewards; the state keeps the index of the 1.1 among ones
+        for j, k in enumerate(("context", "mapped_action", "time", "max_steps_in_episode")):
+            f[k] = st[j]                                                    # max_steps_in_episode: the EnvParams word
+        core = 4
     else:
         raise KeyError(env_name)
     f["log_episode_returns"] = _u2f(st[core + 0])
@@ -243,6 +271,19 @@ def fields_to_state(env_name: str, f: dict) -> torch.Tensor:
         ctx = i32(f["context"])
         core = [ctx.reshape(ctx.shape[0], -1)[:, 0]] + [i32(f[k]) for k in
                                                          ("query", "total_perfect", "total_regret", "time", "memory_length")]
+    elif env_name == "DeepSea-bsuite":
+        n = i32(f["row"]).shape[0]
+        am = (torch.as_tensor(f["action_mapping"]).reshape(n, 64) != 0).to(torch.int64)
+        sh = torch.arange(32, device=am.device)
+        words = [(am[:, 32 * k:32 * k + 32] << sh).sum(1) for k in range(2)]
+        words = [torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32) for v in words]
+        core = [i32(f["row"]) | (i32(f["column"]) << 8) | (i32(f["bad_episode"]) << 16), i32(f["total_bad_episodes"]),
+                i32(f["denoised_return"]), _f2u(torch.as_tensor(f["optimal_return"])),
+                _f2u(torch.as_tensor(f["optimal_no_cost"]))] + words + [i32(f["time"])]
+    elif env_name == "UmbrellaChain-bsuite":
+        core = [i32(f[k]) for k in ("need_umbrella", "has_umbrella", "total_regret", "time")]
+    elif env_name == "DiscountingChain-bsuite":
+        core = [i32(f[k]) for k in ("context", "mapped_action", "time", "max_steps_in_episode")]
     else:
         raise KeyError(env_name)
     log = [_f2u(torch.as_tensor(f["log_episode_returns"])), i32(f["log_episode_lengths"]),
@@ -297,7 +338,7 @@ class BatchedEnv:
         self.num_actions = info.num_actions
         if self.binary_obs:
             shape = tuple(info.obs_shape)
-        else:   # a vector, or a 2-D board (Catch-bsuite's (10, 5)): gymnax's unflattened shape
+        else:   # a vector, or a 2-D board (Catch-bsuite's (10, 5), DeepSea-bsuite's (8, 8)): gymnax's unflattened shape
             shape = (info.obs_shape[0], info.obs_shape[1]) if info.obs_shape[1] > 1 else (info.obs_dim,)
         self._obs_shape = (info.obs_dim,) if flatten_obs else shape
         self.default_params = EnvParams(max_steps_in_episode=info.max_steps)
