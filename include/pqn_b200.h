@@ -49,14 +49,20 @@ extern "C" {
 #define PQN_ENV_DEEP_SEA 34       /* "DeepSea-bsuite" */
 #define PQN_ENV_UMBRELLA_CHAIN 35 /* "UmbrellaChain-bsuite" */
 #define PQN_ENV_DISCOUNTING_CHAIN 36 /* "DiscountingChain-bsuite" */
+#define PQN_ENV_SIMPLE_BANDIT 37  /* "SimpleBandit-bsuite" */
+#define PQN_ENV_BERNOULLI_BANDIT 48 /* "BernoulliBandit-misc" */
+#define PQN_ENV_FOUR_ROOMS 49     /* "FourRooms-misc" */
+#define PQN_ENV_META_MAZE 50      /* "MetaMaze-misc" */
 
 typedef struct pqn_env_info_t {
   int32_t state_words;      /* uint32 words per env in the SoA state block (incl. 5 LogWrapper words) */
   int32_t obs_dim;          /* flattened observation length (400 Breakout, 4 CartPole, 6 Acrobot, 2 MountainCar,
-                               3 MemoryChain, 50 Catch, 64 DeepSea, 3 UmbrellaChain, 2 DiscountingChain) */
-  int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control, MemoryChain, UmbrellaChain and
-                               DiscountingChain, (10, 5, 1) for Catch's board and (8, 8, 1) for DeepSea's; obs buffers
-                               hold the obs_dim floats of an env contiguously either way */
+                               3 MemoryChain, 50 Catch, 64 DeepSea, 3 UmbrellaChain, 2 DiscountingChain,
+                               1 SimpleBandit, 4 BernoulliBandit, 4 FourRooms, 15 MetaMaze) */
+  int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control, MemoryChain, UmbrellaChain,
+                               DiscountingChain and the misc envs, (10, 5, 1) for Catch's board, (8, 8, 1) for
+                               DeepSea's and (1, 1, 1) for SimpleBandit's (1, 1); obs buffers hold the obs_dim floats
+                               of an env contiguously either way */
   int32_t num_actions;      /* env.action_space(params).n  — pqn_minatar.py:151 */
   int32_t max_steps;        /* env_params.max_steps_in_episode default — pqn_minatar.py:105 */
   int32_t binary_obs;       /* 1: obs are {0,1}; the rollout buffer stores them bit-packed */

@@ -373,4 +373,83 @@ struct DiscountingChainEnv {
   }
 };
 
+// gymnax bsuite/bandit.py (SimpleBandit-bsuite) with the constructor's num_actions = 11 and the default EnvParams
+// (optimal_return = 1).  Restated from recollection of gymnax 0.0.6:
+//   reset_env:  action_mask = choice(key, arange(11), (11,), replace=False), which is permutation(key, arange(11));
+//               rewards = linspace(0, 1, 11)[action_mask], total_regret = 0.0, time = 0
+//   step_env:   reward = rewards[action]; total_regret += optimal_return - reward; time += 1;
+//               done = is_terminal = True: every step ends the episode, so every step auto-resets and redraws
+//   get_obs:    ones((1, 1))
+// permutation is jax's _shuffle: ceil(3 ln 11 / ln(2^32 - 1)) = 1 round, a stable sort of arange(11) by
+// random_bits(sub, 32, (11,)) with (key, sub) = split(key).  jnp.linspace in jax 0.4.x computes
+// start * (1 - step) + stop * step with step = iota / 10 in fp32, which at start 0 and stop 1 is the quotient k / 10.
+// The state keeps action_mask (4 bits per action), so reward = action_mask[action] / 10.  Integer work plus one fp32
+// division: bit-exact.
+struct SimpleBanditEnv {
+  static constexpr int ID = ENV_SIMPLE_BANDIT;
+  static constexpr int CORE_WORDS = 5;
+  static constexpr int STATE_WORDS = CORE_WORDS + LOG_WORDS;
+  static constexpr int NUM_ACTIONS = 11;
+  static constexpr int OBS_DIM = 1;
+  static constexpr int OBS_ROWS = 1, OBS_COLS = 1;  // gymnax's (1, 1) observation, unflattened
+  static constexpr bool BINARY_OBS = false;
+  static constexpr bool OBS_IN_REGS = false;
+  static constexpr int OBS_WORDS = 1, OBS_WORDS_PAD = 1;
+  static constexpr int DEFAULT_MAX_STEPS = 100;  // EnvParams.max_steps_in_episode; every step is terminal anyway
+  static constexpr float OPTIMAL_RETURN = 1.0f;
+
+  // words 0, 1: action_mask, entry j in bits 4 (j mod 8) of word j / 8;  2: total_regret (fp32 bits);  3: time;
+  // 4: optimal_return (fp32 bits, the EnvParams word the step reads)
+  struct State {
+    uint32_t mask_lo, mask_hi;
+    float total_regret;
+    int time;
+    float optimal_return;
+  };
+
+  template <typename W>
+  PQN_HD static void load(State& s, const W* __restrict__ st, int64_t N, int64_t i) {
+    s.mask_lo = (uint32_t)st[i]; s.mask_hi = (uint32_t)st[N + i]; s.total_regret = u2f((uint32_t)st[2 * N + i]);
+    s.time = (int)st[3 * N + i]; s.optimal_return = u2f((uint32_t)st[4 * N + i]);
+  }
+  PQN_HD static void store(const State& s, uint32_t* __restrict__ st, int64_t N, int64_t i) {
+    st[i] = s.mask_lo; st[N + i] = s.mask_hi; st[2 * N + i] = f2u(s.total_regret); st[3 * N + i] = (uint32_t)s.time;
+    st[4 * N + i] = f2u(s.optimal_return);
+  }
+
+  PQN_HD static void reset_env(Key key, int part, int /*max_steps*/, State& s) {
+    Key k_next, sub;
+    split2(key, part, k_next, sub);
+    uint32_t sk[NUM_ACTIONS];
+#pragma unroll
+    for (int j = 0; j < NUM_ACTIONS; ++j) sk[j] = bits_at(sub, (uint32_t)NUM_ACTIONS, (uint32_t)j, part);
+    // stable sort: element j lands at its rank, the number of keys below it plus the equal keys before it
+    uint32_t lo = 0u, hi = 0u;
+#pragma unroll
+    for (int j = 0; j < NUM_ACTIONS; ++j) {
+      int rank = 0;
+#pragma unroll
+      for (int i = 0; i < NUM_ACTIONS; ++i) rank += (sk[i] < sk[j] || (sk[i] == sk[j] && i < j)) ? 1 : 0;
+      if (rank < 8) lo |= (uint32_t)j << (4 * rank); else hi |= (uint32_t)j << (4 * (rank - 8));
+    }
+    s.mask_lo = lo; s.mask_hi = hi;
+    s.total_regret = 0.f; s.time = 0;
+    s.optimal_return = OPTIMAL_RETURN;
+  }
+
+  PQN_HD static int mask_at(const State& s, int j) {
+    return (int)(((j < 8 ? s.mask_lo : s.mask_hi) >> (4 * (j & 7))) & 15u);
+  }
+
+  PQN_HD static void step_env(Key /*key*/, int /*part*/, int /*max_steps*/, State& s, int action, float& reward,
+                              bool& done) {
+    reward = (float)mask_at(s, action) / 10.0f;
+    s.total_regret = s.total_regret + s.optimal_return - reward;
+    s.time = s.time + 1;
+    done = true;
+  }
+
+  PQN_HD static void obs_float(const State& /*s*/, float (&o)[OBS_DIM]) { o[0] = 1.f; }
+};
+
 }  // namespace pqn

@@ -33,6 +33,10 @@ enum EnvId : int {
   ENV_DEEP_SEA = 34,
   ENV_UMBRELLA_CHAIN = 35,
   ENV_DISCOUNTING_CHAIN = 36,
+  ENV_SIMPLE_BANDIT = 37,
+  ENV_BERNOULLI_BANDIT = 48,
+  ENV_FOUR_ROOMS = 49,
+  ENV_META_MAZE = 50,
 };
 
 constexpr int LOG_WORDS = 5;

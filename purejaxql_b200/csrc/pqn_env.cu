@@ -20,6 +20,7 @@
 #include "env_bsuite.cuh"
 #include "env_classic.cuh"
 #include "env_minatar_more.cuh"
+#include "env_misc.cuh"
 #include "rollout_logic.cuh"
 
 namespace pqn {
@@ -337,7 +338,7 @@ __global__ void threefry_kernel(const uint32_t* __restrict__ kp, const uint32_t*
 // host-side dispatch
 // ---------------------------------------------------------------------------
 // gymnax's unflattened observation shape of a float-observation env: a vector of OBS_DIM, or the (OBS_ROWS, OBS_COLS)
-// board of an env that defines them (Catch-bsuite, DeepSea-bsuite)
+// board of an env that defines them (Catch-bsuite, DeepSea-bsuite, and SimpleBandit-bsuite's (1, 1))
 template <class Env, class = void>
 struct FloatObsShape {
   static constexpr int ROWS = Env::OBS_DIM, COLS = 1;
@@ -377,6 +378,10 @@ static void fill_info(pqn_env_info_t* o) {
     case ENV_DEEP_SEA: { using EnvT = DeepSeaEnv; __VA_ARGS__; } break;         \
     case ENV_UMBRELLA_CHAIN: { using EnvT = UmbrellaChainEnv; __VA_ARGS__; } break; \
     case ENV_DISCOUNTING_CHAIN: { using EnvT = DiscountingChainEnv; __VA_ARGS__; } break; \
+    case ENV_SIMPLE_BANDIT: { using EnvT = SimpleBanditEnv; __VA_ARGS__; } break; \
+    case ENV_BERNOULLI_BANDIT: { using EnvT = BernoulliBanditEnv; __VA_ARGS__; } break; \
+    case ENV_FOUR_ROOMS: { using EnvT = FourRoomsEnv; __VA_ARGS__; } break;      \
+    case ENV_META_MAZE: { using EnvT = MetaMazeEnv; __VA_ARGS__; } break;        \
     default: return set_error(PQN_E_UNSUPPORTED, "env id %d is not built into libpqn_b200", env_id); \
   }
 

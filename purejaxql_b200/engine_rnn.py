@@ -10,8 +10,8 @@ with a static ``batch_stats`` buffer: the loss updates the running statistics in
 module owns the buffers, walks the reference's PRNG key chain — including its re-bindings of ``rng`` to the final
 carry of the rollout scans (:222-228, :531-537) — and keeps the memory of the last MEMORY_WINDOW + NUM_STEPS
 transitions.  Minibatches are whole env trajectories: ``jax.random.permutation(rng, x, axis=1)`` (:368-379).
-Any float-observation env of ``envs.ENV_IDS`` runs, at its own observation width (2 for MountainCar-v0 up to 64 for
-DeepSea-bsuite); binary-observation (MinAtar) envs are refused.
+Any float-observation env of ``envs.ENV_IDS`` runs, at its own observation width (1 for SimpleBandit-bsuite up to 64
+for DeepSea-bsuite); binary-observation (MinAtar) envs are refused.
 """
 from __future__ import annotations
 

@@ -37,7 +37,13 @@ ENV_IDS = {
     "DeepSea-bsuite": 34,
     "UmbrellaChain-bsuite": 35,
     "DiscountingChain-bsuite": 36,
+    "SimpleBandit-bsuite": 37,
+    "BernoulliBandit-misc": 48,
+    "FourRooms-misc": 49,
+    "MetaMaze-misc": 50,
 }
+# float-observation envs whose gymnax observation is 2-D although pqn_env_info's (rows, cols) = (1, 1) cannot say so
+_2D_OBS = {"SimpleBandit-bsuite"}
 # PQN_ENV_SEAQUEST (4) is reserved in include/pqn_b200.h but not built: gymnax 0.0.6 (the reference's pin) does not
 # register "Seaquest-MinAtar" in gymnax.make either (DESIGN.md section 8), so the reference cannot run it.
 MINATAR_GAMES = ("Breakout-MinAtar", "Asterix-MinAtar", "SpaceInvaders-MinAtar", "Freeway-MinAtar")
@@ -192,6 +198,38 @@ def state_to_fields(env_name: str, state: torch.Tensor) -> dict:
         for j, k in enumerate(("context", "mapped_action", "time", "max_steps_in_episode")):
             f[k] = st[j]                                                    # max_steps_in_episode: the EnvParams word
         core = 4
+    elif env_name == "SimpleBandit-bsuite":
+        # gymnax keeps the eleven rewards; the state keeps action_mask, their indices into linspace(0, 1, 11)
+        j = torch.arange(11, device=st.device)
+        words = st[0:2].to(torch.int64) & 0xFFFFFFFF                       # [2, N]
+        f["action_mask"] = ((words[j >> 3] >> (4 * (j & 7)).unsqueeze(1)) & 15).t().to(torch.int32)   # [N, 11]
+        f["total_regret"] = _u2f(st[2])
+        f["time"] = st[3]
+        f["optimal_return"] = _u2f(st[4])                                   # the EnvParams word
+        core = 5
+    elif env_name == "BernoulliBandit-misc":
+        f["last_action"] = st[0]
+        f["last_reward"] = st[1]
+        f["reward_probs"] = torch.stack([_u2f(st[2]), _u2f(st[3])], 1)     # [N, 2]
+        f["exp_reward_best"] = _u2f(st[4])
+        f["time"] = st[5]
+        core = 6
+    elif env_name == "FourRooms-misc":
+        w = st[0]
+        f["pos"] = torch.stack([w & 255, (w >> 8) & 255], 1)
+        f["goal"] = torch.stack([(w >> 16) & 255, (w >> 24) & 255], 1)
+        f["time"] = st[1]
+        f["fail_prob"] = _u2f(st[2])                                        # the EnvParams word
+        core = 3
+    elif env_name == "MetaMaze-misc":
+        f["last_action"] = st[0]
+        f["last_reward"] = _u2f(st[1])
+        w = st[2]
+        f["pos"] = torch.stack([w & 255, (w >> 8) & 255], 1)
+        f["goal"] = torch.stack([(w >> 16) & 255, (w >> 24) & 255], 1)
+        f["time"] = st[3]
+        f["reward"] = _u2f(st[4])                                           # the EnvParams word
+        core = 5
     else:
         raise KeyError(env_name)
     f["log_episode_returns"] = _u2f(st[core + 0])
@@ -284,9 +322,28 @@ def fields_to_state(env_name: str, f: dict) -> torch.Tensor:
         core = [i32(f[k]) for k in ("need_umbrella", "has_umbrella", "total_regret", "time")]
     elif env_name == "DiscountingChain-bsuite":
         core = [i32(f[k]) for k in ("context", "mapped_action", "time", "max_steps_in_episode")]
+    elif env_name == "SimpleBandit-bsuite":
+        m = torch.as_tensor(f["action_mask"]).to(torch.int64)                # [N, 11]
+        sh = 4 * torch.arange(8, device=m.device)
+        words = [(m[:, 0:8] << sh).sum(1), (m[:, 8:11] << sh[:3]).sum(1)]
+        words = [torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32) for v in words]
+        core = words + [_f2u(torch.as_tensor(f["total_regret"])), i32(f["time"]),
+                        _f2u(torch.as_tensor(f["optimal_return"]))]
+    elif env_name == "BernoulliBandit-misc":
+        p = torch.as_tensor(f["reward_probs"])
+        core = [i32(f["last_action"]), i32(f["last_reward"]), _f2u(p[:, 0]), _f2u(p[:, 1]),
+                _f2u(torch.as_tensor(f["exp_reward_best"])), i32(f["time"])]
+    elif env_name in ("FourRooms-misc", "MetaMaze-misc"):
+        pos, goal = i32(f["pos"]), i32(f["goal"])
+        w = pos[:, 0] | (pos[:, 1] << 8) | (goal[:, 0] << 16) | (goal[:, 1] << 24)
+        if env_name == "FourRooms-misc":
+            core = [w, i32(f["time"]), _f2u(torch.as_tensor(f["fail_prob"]))]
+        else:
+            core = [i32(f["last_action"]), _f2u(torch.as_tensor(f["last_reward"])), w, i32(f["time"]),
+                    _f2u(torch.as_tensor(f["reward"]))]
     else:
         raise KeyError(env_name)
-    log = [_f2u(torch.as_tensor(f["log_episode_returns"])), i32(f["log_episode_lengths"]),
+    log =[_f2u(torch.as_tensor(f["log_episode_returns"])), i32(f["log_episode_lengths"]),
            _f2u(torch.as_tensor(f["log_returned_episode_returns"])), i32(f["log_returned_episode_lengths"]),
            i32(f["log_timestep"])]
     return torch.stack(core + log).contiguous()
@@ -338,8 +395,10 @@ class BatchedEnv:
         self.num_actions = info.num_actions
         if self.binary_obs:
             shape = tuple(info.obs_shape)
-        else:   # a vector, or a 2-D board (Catch-bsuite's (10, 5), DeepSea-bsuite's (8, 8)): gymnax's unflattened shape
-            shape = (info.obs_shape[0], info.obs_shape[1]) if info.obs_shape[1] > 1 else (info.obs_dim,)
+        else:   # a vector, or a 2-D board (Catch-bsuite's (10, 5), DeepSea-bsuite's (8, 8), SimpleBandit-bsuite's
+            # (1, 1)): gymnax's unflattened shape
+            board = info.obs_shape[1] > 1 or name in _2D_OBS
+            shape = (info.obs_shape[0], info.obs_shape[1]) if board else (info.obs_dim,)
         self._obs_shape = (info.obs_dim,) if flatten_obs else shape
         self.default_params = EnvParams(max_steps_in_episode=info.max_steps)
         self.rng_mode = rng_mode
