@@ -53,12 +53,13 @@ extern "C" {
 #define PQN_ENV_BERNOULLI_BANDIT 48 /* "BernoulliBandit-misc" */
 #define PQN_ENV_FOUR_ROOMS 49     /* "FourRooms-misc" */
 #define PQN_ENV_META_MAZE 50      /* "MetaMaze-misc" */
+#define PQN_ENV_GAUSSIAN_BANDIT 51 /* "GaussianBandit-misc" */
 
 typedef struct pqn_env_info_t {
   int32_t state_words;      /* uint32 words per env in the SoA state block (incl. 5 LogWrapper words) */
   int32_t obs_dim;          /* flattened observation length (400 Breakout, 4 CartPole, 6 Acrobot, 2 MountainCar,
                                3 MemoryChain, 50 Catch, 64 DeepSea, 3 UmbrellaChain, 2 DiscountingChain,
-                               1 SimpleBandit, 4 BernoulliBandit, 4 FourRooms, 15 MetaMaze) */
+                               1 SimpleBandit, 4 BernoulliBandit, 4 FourRooms, 15 MetaMaze, 4 GaussianBandit) */
   int32_t obs_shape[3];     /* (H, W, C) for MinAtar, (D, 1, 1) for classic control, MemoryChain, UmbrellaChain,
                                DiscountingChain and the misc envs, (10, 5, 1) for Catch's board, (8, 8, 1) for
                                DeepSea's and (1, 1, 1) for SimpleBandit's (1, 1); obs buffers hold the obs_dim floats
@@ -94,6 +95,13 @@ int pqn_threefry2x32(const uint32_t* key_pairs, const uint32_t* ctr_pairs, uint3
                      void* stream);
 /* out[n][len] = jax.random.random_bits(keys[n], 32, (len,)) — sort keys of jax.random.permutation (:303) */
 int pqn_rng_bits(const uint32_t* keys, int64_t n, int64_t len, uint32_t* out, int rng_mode, void* stream);
+/* out[n] (float32) = jax.random.normal(key, (n,)) for the one key keys[2], 0 < n < 2^31: sqrt(2) * erf_inv of a
+ * uniform in (-1, 1), with XLA's fp32 erf_inv (csrc/threefry.cuh).  No reference call site of its own: gymnax's
+ * GaussianBandit-misc draws it inside Environment.step. */
+int pqn_random_normal(const uint32_t* keys, float* out, int64_t n, int rng_mode, void* stream);
+/* out[n] = the normal jax.random.normal makes of the 32 random bits bits[n] (only bits >> 9 matter): hook for tests,
+ * which cover all 2^23 distinct values. */
+int pqn_normal_from_bits(const uint32_t* bits, float* out, int64_t n, void* stream);
 /* out[S][n] (int32) = jax.random.permutation(keys[s], n) as an index permutation, i.e. the shuffle that
  * `jax.random.permutation(rng, x)` applies to every leaf of the flattened rollout (pqn_minatar.py:299-315): jax's
  * rounds of a stable sort by fresh 32-bit keys, done as an exact bucket + rank sort (csrc/pqn_perm.cu).

@@ -56,6 +56,8 @@ _SIGS = {
     "pqn_rng_split": (c_int, [c_void_p, c_int64, c_int32, c_void_p, c_int, c_void_p]),
     "pqn_threefry2x32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pqn_rng_bits": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int, c_void_p]),
+    "pqn_random_normal": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "pqn_normal_from_bits": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "pqn_set_permutation_bucket_log2": (c_int, [c_int]),
     "pqn_permutation_workspace_bytes": (c_int64, [c_int64, c_int]),
     "pqn_permutation": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),

@@ -37,6 +37,7 @@ enum EnvId : int {
   ENV_BERNOULLI_BANDIT = 48,
   ENV_FOUR_ROOMS = 49,
   ENV_META_MAZE = 50,
+  ENV_GAUSSIAN_BANDIT = 51,
 };
 
 constexpr int LOG_WORDS = 5;

@@ -1,10 +1,11 @@
-// gymnax's discrete-action misc environments that need nothing external (BernoulliBandit-misc, FourRooms-misc,
-// MetaMaze-misc), one env per thread, with gymnax's default constructor arguments and EnvParams.
+// gymnax's discrete-action misc environments that need nothing external (BernoulliBandit-misc, GaussianBandit-misc,
+// FourRooms-misc, MetaMaze-misc), one env per thread, with gymnax's default constructor arguments and EnvParams.
 //
 // Restated from recollection of gymnax==0.0.6 gymnax/environments/misc/ (third party; call sites
 // purejaxql/pqn_gymnax.py:92 and purejaxql/pqn_rnn_gymnax.py:133-139, `gymnax.make(config["ENV_NAME"])`).
-// tests/misc_envs_oracle.py lists every recollected point; tests/golden/make_misc_golden_from_ref.py records gymnax
-// trajectories that check them.
+// tests/misc_envs_oracle.py and tests/gaussian_bandit_oracle.py list every recollected point;
+// tests/golden/make_misc_golden_from_ref.py and make_gaussian_bandit_golden_from_ref.py record gymnax trajectories
+// that check them.
 #pragma once
 #include "env_common.cuh"
 
@@ -74,6 +75,75 @@ struct BernoulliBanditEnv {
     o[0] = s.last_action == 0 ? 1.f : 0.f;
     o[1] = s.last_action == 1 ? 1.f : 0.f;
     o[2] = (float)s.last_reward;
+    o[3] = misc_time_normalization(s.time);
+  }
+};
+
+// misc/gaussian_bandit.py (GaussianBandit-misc), two arms, with the default EnvParams (mu1 = 0.0, sigma_p = 1.0,
+// sigma_l = 1.0, normalize_time = True):
+//   reset_env:  mu2 = sigma_p * normal(key, ()), drawn from the reset key itself; exp_reward_best = max(mu1, mu2),
+//               last_action = 0, last_reward = 0.0, time = 0
+//   step_env:   reward = mu1 if action == 0 else mu2 + sigma_l * normal(key, ()), drawn from the step key itself;
+//               last_action = action, last_reward = reward, time += 1; done = time >= max_steps_in_episode (100)
+//   get_obs:    [one_hot(last_action, 2), last_reward, time_normalization(time)]
+// Arm 0 pays mu1 and arm 1 a normal around its mean mu2.  gymnax draws the step's normal for both arms and selects it
+// away for arm 0, so this env draws it only for arm 1.  mu1 and sigma_l are kept in state words (the step reads them
+// from EnvParams).  The step's mu2 + sigma_l * n is one fma, as the Horner steps of erf_inv (threefry.cuh); at
+// sigma_l = 1 the product is exact and the fma and the rounded add agree.  The normal's log1pf makes the rewards and
+// mu2 depend on the math library: libdevice's on the device, as XLA:GPU's jax.random.normal.
+struct GaussianBanditEnv {
+  static constexpr int ID = ENV_GAUSSIAN_BANDIT;
+  static constexpr int CORE_WORDS = 7;
+  static constexpr int STATE_WORDS = CORE_WORDS + LOG_WORDS;
+  static constexpr int NUM_ACTIONS = 2;
+  static constexpr int OBS_DIM = 4;
+  static constexpr bool BINARY_OBS = false;
+  static constexpr bool OBS_IN_REGS = false;
+  static constexpr int OBS_WORDS = 1, OBS_WORDS_PAD = 1;
+  static constexpr int DEFAULT_MAX_STEPS = 100;  // EnvParams.max_steps_in_episode: every episode lasts this long
+  static constexpr float MU1 = 0.0f, SIGMA_P = 1.0f, SIGMA_L = 1.0f;
+
+  // words: last_action, last_reward, mu2, exp_reward_best (fp32 bits), time, then the EnvParams words mu1 and
+  // sigma_l (fp32 bits)
+  struct State {
+    int last_action;
+    float last_reward, mu2, exp_reward_best;
+    int time;
+    float mu1, sigma_l;
+  };
+
+  template <typename W>
+  PQN_HD static void load(State& s, const W* __restrict__ st, int64_t N, int64_t i) {
+    s.last_action = (int)st[i]; s.last_reward = u2f((uint32_t)st[N + i]);
+    s.mu2 = u2f((uint32_t)st[2 * N + i]); s.exp_reward_best = u2f((uint32_t)st[3 * N + i]);
+    s.time = (int)st[4 * N + i];
+    s.mu1 = u2f((uint32_t)st[5 * N + i]); s.sigma_l = u2f((uint32_t)st[6 * N + i]);
+  }
+  PQN_HD static void store(const State& s, uint32_t* __restrict__ st, int64_t N, int64_t i) {
+    st[i] = (uint32_t)s.last_action; st[N + i] = f2u(s.last_reward);
+    st[2 * N + i] = f2u(s.mu2); st[3 * N + i] = f2u(s.exp_reward_best);
+    st[4 * N + i] = (uint32_t)s.time;
+    st[5 * N + i] = f2u(s.mu1); st[6 * N + i] = f2u(s.sigma_l);
+  }
+
+  PQN_HD static void reset_env(Key key, int part, int /*max_steps*/, State& s) {
+    s.mu1 = MU1; s.sigma_l = SIGMA_L;
+    s.mu2 = mul_rn(SIGMA_P, normal_scalar(key, part));
+    s.exp_reward_best = s.mu2 > s.mu1 ? s.mu2 : s.mu1;
+    s.last_action = 0; s.last_reward = 0.f; s.time = 0;
+  }
+
+  PQN_HD static void step_env(Key key, int part, int max_steps, State& s, int action, float& reward, bool& done) {
+    reward = action == 0 ? s.mu1 : fmaf(s.sigma_l, normal_scalar(key, part), s.mu2);
+    s.last_action = action; s.last_reward = reward;
+    s.time = s.time + 1;
+    done = s.time >= max_steps;
+  }
+
+  PQN_HD static void obs_float(const State& s, float (&o)[OBS_DIM]) {
+    o[0] = s.last_action == 0 ? 1.f : 0.f;
+    o[1] = s.last_action == 1 ? 1.f : 0.f;
+    o[2] = s.last_reward;
     o[3] = misc_time_normalization(s.time);
   }
 };

@@ -324,6 +324,19 @@ __global__ void rng_bits_kernel(const uint32_t* __restrict__ keys, int64_t n, in
   out[g] = bits_at(Key{keys[2 * k], keys[2 * k + 1]}, (uint32_t)len, (uint32_t)j, part);
 }
 
+// jax.random.normal(key, (n,)): element j is the normal of random_bits(key, 32, (n,))[j]
+__global__ void random_normal_kernel(const uint32_t* __restrict__ key, int64_t n, float* __restrict__ out, int part) {
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n) return;
+  out[g] = normal_from_bits(bits_at(Key{key[0], key[1]}, (uint32_t)n, (uint32_t)g, part));
+}
+
+__global__ void normal_from_bits_kernel(const uint32_t* __restrict__ bits, float* __restrict__ out, int64_t n) {
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n) return;
+  out[g] = normal_from_bits(bits[g]);
+}
+
 __global__ void threefry_kernel(const uint32_t* __restrict__ kp, const uint32_t* __restrict__ cp,
                                 uint32_t* __restrict__ out, int64_t n) {
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -382,6 +395,7 @@ static void fill_info(pqn_env_info_t* o) {
     case ENV_BERNOULLI_BANDIT: { using EnvT = BernoulliBanditEnv; __VA_ARGS__; } break; \
     case ENV_FOUR_ROOMS: { using EnvT = FourRoomsEnv; __VA_ARGS__; } break;      \
     case ENV_META_MAZE: { using EnvT = MetaMazeEnv; __VA_ARGS__; } break;        \
+    case ENV_GAUSSIAN_BANDIT: { using EnvT = GaussianBanditEnv; __VA_ARGS__; } break; \
     default: return set_error(PQN_E_UNSUPPORTED, "env id %d is not built into libpqn_b200", env_id); \
   }
 
@@ -411,6 +425,21 @@ int pqn_rng_bits(const uint32_t* keys, int64_t n, int64_t len, uint32_t* out, in
   if (n == 0) return PQN_OK;
   { LaunchScope _ls(K_RNG, (cudaStream_t)stream); rng_bits_kernel<<<blocks_for(n * len, 256), 256, 0, (cudaStream_t)stream>>>(keys, n, len, out, rng_mode); }
   return check_launch("pqn_rng_bits");
+}
+
+int pqn_random_normal(const uint32_t* keys, float* out, int64_t n, int rng_mode, void* stream) {
+  if (!keys || !out || n < 0 || n >= ((int64_t)1 << 31))
+    return set_error(PQN_E_INVALID, "pqn_random_normal: bad argument (n=%lld, 0 <= n < 2^31)", (long long)n);
+  if (n == 0) return PQN_OK;
+  { LaunchScope _ls(K_RNG, (cudaStream_t)stream); random_normal_kernel<<<blocks_for(n, 256), 256, 0, (cudaStream_t)stream>>>(keys, n, out, rng_mode); }
+  return check_launch("pqn_random_normal");
+}
+
+int pqn_normal_from_bits(const uint32_t* bits, float* out, int64_t n, void* stream) {
+  if (!bits || !out || n < 0) return set_error(PQN_E_INVALID, "pqn_normal_from_bits: bad argument");
+  if (n == 0) return PQN_OK;
+  { LaunchScope _ls(K_RNG, (cudaStream_t)stream); normal_from_bits_kernel<<<blocks_for(n, 256), 256, 0, (cudaStream_t)stream>>>(bits, out, n); }
+  return check_launch("pqn_normal_from_bits");
 }
 
 int pqn_threefry2x32(const uint32_t* key_pairs, const uint32_t* ctr_pairs, uint32_t* out_pairs, int64_t n,

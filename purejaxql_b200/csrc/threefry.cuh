@@ -1,13 +1,14 @@
 // jax.random (threefry2x32) semantics, as consumed by the PQN hot path.
 //
 // Replaces, on device, the PRNG arithmetic the reference reaches through
-// jax.random.split / uniform / randint / choice at
+// jax.random.split / uniform / randint / choice / normal at
 //   purejaxql/pqn_minatar.py:107-112 (per-env key split), :116-125 (eps-greedy),
 //   :183 (3-way split of the scan carry), and inside gymnax Environment.step.
 // Both counter layouts are supported (`part` = jax_threefry_partitionable):
 //   part=0  "original" layout, default for the reference's pinned jax<=0.4.38
 //   part=1  "partitionable" layout, default from jax 0.5
 #pragma once
+#include <math.h>
 #include <stdint.h>
 
 #if defined(__CUDACC__)
@@ -138,6 +139,83 @@ PQN_HD float uniform_from_bits(uint32_t bits, float minval, float maxval) {
   return f < minval ? minval : f;
 }
 PQN_HD float uniform_scalar(Key k, int part) { return uniform_from_bits(bits_scalar(k, part), 0.0f, 1.0f); }
+
+// ---------------------------------------------------------------------------
+// jax.random.normal(key, shape, f32): jax 0.4.x `_normal_real`,
+//   u = uniform(key, shape, lo = nextafter(-1, 0), hi = 1);  sqrt(2) * lax.erf_inv(u)
+// with lax.erf_inv lowered (chlo.erf_inv) to XLA's fp32 form of M. Giles' approximation ("Approximating the erfinv
+// function", GPU Computing Gems Jade Edition, 2011):
+//   w = -log1p(-x * x)
+//   w < 5:  t = w - 2.5,      p = Horner over the 9 "central" coefficients in t
+//   else:   t = sqrt(w) - 3,  p = Horner over the 9 "tail" coefficients in t
+//   erf_inv(x) = x * inf where |x| == 1, else p * x
+// The uniform here is 2 f - (1 - 2^-24) for f = (bits >> 9) * 2^-23: exact in fp32, never 0 and never +-1, so the
+// normal takes exactly 2^23 values, one per value of bits >> 9, and the |x| == 1 case cannot occur.  Both branches
+// occur (w >= 5 for |u| > 0.9966).
+//
+// Two points of XLA:GPU's code generation are recollection, not checked against a live jax, and fix the bits:
+//  (1) log1p is libdevice's log1pf, applied to the rounded product x * x.  This code calls log1pf (libdevice's on the
+//      device, the C library's on the host) on __fmul_rn(x, x), which no -fmad setting fuses into log1pf's first add.
+//  (2) LLVM's NVPTX backend contracts each Horner step p * t + c into one fma (its default fma level fuses an fmul
+//      feeding an fadd).  The steps are written as fmaf, so the bits do not depend on the -fmad of the unit that
+//      includes this header.  jax on the CPU does not contract and gives a different last bit in some values.
+// tests/golden/make_gaussian_bandit_golden_from_ref.py records jax's values on the CPU and on a CUDA device.
+PQN_HD float mul_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+PQN_HD float sqrt_rn(float a) {
+#if defined(__CUDA_ARCH__)
+  return __fsqrt_rn(a);
+#else
+  return sqrtf(a);
+#endif
+}
+
+// w = -log1p(-x * x), the argument of erf_inv's polynomial
+PQN_HD float erf_inv_w(float x) { return -log1pf(-mul_rn(x, x)); }
+
+// erf_inv(x) given w = erf_inv_w(x): the polynomial part, which is exact fp32 arithmetic with no library call
+PQN_HD float erf_inv_from_w(float x, float w) {
+  float p;
+  if (w < 5.0f) {
+    const float t = w - 2.5f;
+    p = 2.81022636e-08f;
+    p = fmaf(p, t, 3.43273939e-07f);
+    p = fmaf(p, t, -3.5233877e-06f);
+    p = fmaf(p, t, -4.39150654e-06f);
+    p = fmaf(p, t, 0.00021858087f);
+    p = fmaf(p, t, -0.00125372503f);
+    p = fmaf(p, t, -0.00417768164f);
+    p = fmaf(p, t, 0.246640727f);
+    p = fmaf(p, t, 1.50140941f);
+  } else {
+    const float t = sqrt_rn(w) - 3.0f;
+    p = -0.000200214257f;
+    p = fmaf(p, t, 0.000100950558f);
+    p = fmaf(p, t, 0.00134934322f);
+    p = fmaf(p, t, -0.00367342844f);
+    p = fmaf(p, t, 0.00573950773f);
+    p = fmaf(p, t, -0.0076224613f);
+    p = fmaf(p, t, 0.00943887047f);
+    p = fmaf(p, t, 1.00167406f);
+    p = fmaf(p, t, 2.83297682f);
+  }
+  return (x == 1.0f || x == -1.0f) ? x * INFINITY : p * x;
+}
+
+PQN_HD float erf_inv(float x) { return erf_inv_from_w(x, erf_inv_w(x)); }
+
+// jax.random.normal's value for the 32 random bits of one element
+PQN_HD float normal_from_bits(uint32_t bits) {
+  const float u = uniform_from_bits(bits, -0.99999994f /* nextafter(-1, 0) = -(1 - 2^-24) */, 1.0f);
+  return mul_rn(1.41421356237309504880f /* sqrt(2), rounded to fp32 */, erf_inv(u));
+}
+// jax.random.normal(key, ())
+PQN_HD float normal_scalar(Key k, int part) { return normal_from_bits(bits_scalar(k, part)); }
 
 // jax.random.randint(key, (), 0, span) with 1 <= span < 2^16 (small action sets):
 //   k1,k2 = split(key); off = ((hi % span) * mult + lo % span) % span,

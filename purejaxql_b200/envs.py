@@ -41,6 +41,7 @@ ENV_IDS = {
     "BernoulliBandit-misc": 48,
     "FourRooms-misc": 49,
     "MetaMaze-misc": 50,
+    "GaussianBandit-misc": 51,
 }
 # float-observation envs whose gymnax observation is 2-D although pqn_env_info's (rows, cols) = (1, 1) cannot say so
 _2D_OBS = {"SimpleBandit-bsuite"}
@@ -230,6 +231,15 @@ def state_to_fields(env_name: str, state: torch.Tensor) -> dict:
         f["time"] = st[3]
         f["reward"] = _u2f(st[4])                                           # the EnvParams word
         core = 5
+    elif env_name == "GaussianBandit-misc":
+        f["last_action"] = st[0]
+        f["last_reward"] = _u2f(st[1])
+        f["mu2"] = _u2f(st[2])
+        f["exp_reward_best"] = _u2f(st[3])
+        f["time"] = st[4]
+        f["mu1"] = _u2f(st[5])                                              # the EnvParams words
+        f["sigma_l"] = _u2f(st[6])
+        core = 7
     else:
         raise KeyError(env_name)
     f["log_episode_returns"] = _u2f(st[core + 0])
@@ -341,6 +351,10 @@ def fields_to_state(env_name: str, f: dict) -> torch.Tensor:
         else:
             core = [i32(f["last_action"]), _f2u(torch.as_tensor(f["last_reward"])), w, i32(f["time"]),
                     _f2u(torch.as_tensor(f["reward"]))]
+    elif env_name == "GaussianBandit-misc":
+        core = [i32(f["last_action"]), _f2u(torch.as_tensor(f["last_reward"])), _f2u(torch.as_tensor(f["mu2"])),
+                _f2u(torch.as_tensor(f["exp_reward_best"])), i32(f["time"]), _f2u(torch.as_tensor(f["mu1"])),
+                _f2u(torch.as_tensor(f["sigma_l"]))]
     else:
         raise KeyError(env_name)
     log =[_f2u(torch.as_tensor(f["log_episode_returns"])), i32(f["log_episode_lengths"]),

@@ -1,9 +1,11 @@
 """Device-side ``jax.random`` plumbing the training program needs on the host
 side of the boundary: keys are int32/uint32 bit patterns in CUDA tensors and all
-arithmetic runs in libpqn_b200 kernels (``pqn_rng_split`` / ``pqn_rng_bits``).
+arithmetic runs in libpqn_b200 kernels (``pqn_rng_split`` / ``pqn_rng_bits`` /
+``pqn_random_normal``).
 
 Mirrors the calls in purejaxql/pqn_minatar.py: ``PRNGKey`` (:456), ``split``
-(:108,112,172,183,213,309,...), ``permutation`` (:303).
+(:108,112,172,183,213,309,...), ``permutation`` (:303); and ``normal``, which
+gymnax's GaussianBandit-misc draws.
 """
 from __future__ import annotations
 
@@ -56,6 +58,17 @@ def random_bits(keys: torch.Tensor, length: int, rng_mode: int = 0) -> torch.Ten
     out = torch.empty((n, length), dtype=torch.int32, device=keys.device)
     _lib.check(_lib.lib().pqn_rng_bits(_lib.p(keys), n, length, _lib.p(out), rng_mode, _lib.stream_ptr()),
                "pqn_rng_bits")
+    return out
+
+
+def normal(key: torch.Tensor, n: int, rng_mode: int = 0) -> torch.Tensor:
+    """``jax.random.normal(key, (n,))`` (float32) for one key [2] -> float32[n], in ``pqn_random_normal``."""
+    key = key.contiguous()
+    if key.shape != (2,):
+        raise ValueError(f"normal takes one key of shape (2,), got {tuple(key.shape)}")
+    out = torch.empty(int(n), dtype=torch.float32, device=key.device)
+    _lib.check(_lib.lib().pqn_random_normal(_lib.p(key), _lib.p(out), int(n), rng_mode, _lib.stream_ptr()),
+               "pqn_random_normal")
     return out
 
 

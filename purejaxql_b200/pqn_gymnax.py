@@ -7,12 +7,13 @@ purejaxql/pqn_gymnax.py.
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=Catch-bsuite
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=DeepSea-bsuite
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=FourRooms-misc
+    python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=GaussianBandit-misc
 
 Every env of ``envs.ENV_IDS`` runs with its gymnax default ``EnvParams``: CartPole-v1, Acrobot-v1, MountainCar-v0
 (200 steps), MemoryChain-bsuite, Catch-bsuite (its 10 x 5 board flattened to 50 inputs), DeepSea-bsuite (its 8 x 8
 board flattened to 64 inputs), UmbrellaChain-bsuite, DiscountingChain-bsuite (5 actions), SimpleBandit-bsuite (one
-constant input, 11 actions: HIDDEN_SIZE 512 is refused), BernoulliBandit-misc, FourRooms-misc, MetaMaze-misc and the
-MinAtar games.
+constant input, 11 actions: HIDDEN_SIZE 512 is refused), BernoulliBandit-misc, GaussianBandit-misc, FourRooms-misc,
+MetaMaze-misc and the MinAtar games.
 
 On a MinAtar game the flattened (10,10,C) observation feeds the MLP as in the reference; the rollout keeps it as
 packed bits and Dense_0 reads those directly (PQN_NET_MLP_BITS).

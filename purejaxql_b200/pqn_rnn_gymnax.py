@@ -6,12 +6,13 @@
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=Catch-bsuite
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=UmbrellaChain-bsuite
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=MetaMaze-misc
+    python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=GaussianBandit-misc
 
 The envs are CartPole-v1, Acrobot-v1, MountainCar-v0, MemoryChain-bsuite, Catch-bsuite (50 inputs: every
 NORM_TYPE / NORM_INPUT runs on it), DeepSea-bsuite (64 inputs), UmbrellaChain-bsuite, DiscountingChain-bsuite,
-SimpleBandit-bsuite (11 actions: HIDDEN_SIZE 512 is refused), the meta-RL tasks BernoulliBandit-misc and
-MetaMaze-misc, and FourRooms-misc, each with gymnax's default ``EnvParams``.  The MinAtar games are refused: the memory
-stores float observation rows.
+SimpleBandit-bsuite (11 actions: HIDDEN_SIZE 512 is refused), the meta-RL tasks BernoulliBandit-misc,
+GaussianBandit-misc and MetaMaze-misc, and FourRooms-misc, each with gymnax's default ``EnvParams``.  The MinAtar games
+are refused: the memory stores float observation rows.
 
 ``make_train(config)`` keeps the reference's contract (pqn_rnn_gymnax.py:117-560): config mutation (NUM_UPDATES,
 NUM_UPDATES_DECAY, TEST_NUM_STEPS), ``RNNQNetwork`` (MLP trunk -> one-hot last action -> scanned GRU with done-resets ->
