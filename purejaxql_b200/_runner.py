@@ -39,16 +39,22 @@ def seed_slice(num_seeds, rank, world):
     return lo, min(num_seeds, lo + per)
 
 
-def pick_data_parallel(config, world):
+def pick_data_parallel(config, world, env_sharding=True):
     """"seeds" | "envs" for this run: DATA_PARALLEL (this repo's key, not in the reference) = "seeds" shards the
     independent seeds over the ranks (no collective); "envs" shards NUM_ENVS of every seed and all-reduces the
     gradient once per minibatch step; "auto" (default) picks "envs" when there are fewer seeds than GPUs (the
-    shipped default is NUM_SEEDS=1, config/config.yaml:2)."""
+    shipped default is NUM_SEEDS=1, config/config.yaml:2).  A script whose engine has no env-sharded mode
+    (``env_sharding=False``: the recurrent one) always shards seeds, and refuses an explicit "envs"."""
     if world <= 1:
         return "seeds"
     dp = config.get("DATA_PARALLEL", "auto")
     if dp not in ("auto", "seeds", "envs"):
         raise ValueError(f"DATA_PARALLEL={dp!r}: expected auto, seeds or envs")
+    if not env_sharding:
+        if dp == "envs":
+            raise ValueError("DATA_PARALLEL=envs: this script's engine has no env-sharded mode; use "
+                             "DATA_PARALLEL=seeds (one seed per GPU)")
+        return "seeds"
     if dp == "auto":
         dp = "envs" if int(config["NUM_SEEDS"]) < world else "seeds"
     if dp == "envs":
@@ -70,7 +76,7 @@ def _shard_seeds(rngs):
     return rngs[lo:hi], r, w
 
 
-def single_run(config, make_train, alg_file_name="pqn"):
+def single_run(config, make_train, alg_file_name="pqn", env_sharding=True):
     config = {**config, **config["alg"]}                              # :437
     print(config)
     alg_name = config.get("ALG_NAME", "pqn")
@@ -82,7 +88,7 @@ def single_run(config, make_train, alg_file_name="pqn"):
                    tags=[alg_name.upper(), env_name.upper(), "b200_native"],
                    name=f'{config["ALG_NAME"]}_{config["ENV_NAME"]}', config=config, mode=config["WANDB_MODE"])
     d_rank, d_world = init_distributed()
-    env_sharded = pick_data_parallel(config, d_world) == "envs"
+    env_sharded = pick_data_parallel(config, d_world, env_sharding) == "envs"
     rng = jr.PRNGKey(config["SEED"])                                  # :456
     t0 = time.time()
     rngs = jr.split(rng, config["NUM_SEEDS"], int(config.get("JAX_THREEFRY_PARTITIONABLE", 0)))   # :459
@@ -150,7 +156,7 @@ def tune(default_config, make_train):
     wandb.agent(sweep_id, wrapped_make_train, count=1000)
 
 
-def main(make_train, argv=None):
+def main(make_train, argv=None, env_sharding=True):
     """`python -m purejaxql_b200.pqn_minatar +alg=pqn_minatar alg.NUM_ENVS=4096 NUM_SEEDS=8`"""
     argv = sys.argv[1:] if argv is None else argv
     config = config_loader.compose(argv)
@@ -159,4 +165,4 @@ def main(make_train, argv=None):
     if config.get("HYP_TUNE", False):
         tune(config, make_train)
     else:
-        return single_run(config, make_train)
+        return single_run(config, make_train, env_sharding=env_sharding)

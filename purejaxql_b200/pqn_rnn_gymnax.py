@@ -57,11 +57,12 @@ def make_train(config):
 
 
 def single_run(config):
-    return _runner.single_run(config, make_train, alg_file_name="pqn_rnn")
+    # PQNRnnEngine has no env-sharded mode: under torchrun the ranks take seeds
+    return _runner.single_run(config, make_train, alg_file_name="pqn_rnn", env_sharding=False)
 
 
 def main(argv=None):
-    return _runner.main(make_train, argv)
+    return _runner.main(make_train, argv, env_sharding=False)
 
 
 if __name__ == "__main__":
