@@ -239,7 +239,19 @@ def test_config3_geometry_one_update_matches_oracle(env_name):
 def test_config4_acrobot_65536_env_step_and_train():
     """BASELINE configs[3]: Acrobot-v1 with NUM_ENVS=65536.  (i) the env operator at N=65536, teacher-forced against
     the oracle for 24 steps with a 20-step time limit (resets + truncation exercised), 2e-5 per step; (ii) two
-    updates through pqn_gymnax.make_train/train at that geometry: finite loss, exact step bookkeeping."""
+    updates through pqn_gymnax.make_train/train at that geometry: finite loss, exact step bookkeeping, and update 1
+    teacher-forced on its own buffers:
+      - rollout Q-values: maxq[t, e] is max_a of the fp64 MLP on obs[t, e] under the parameters update 0 ended with,
+        within 1e-5, on every 16th env (a different residue at each t) at all 64 steps;
+      - Q(lambda) targets of all 65,536 envs against the fp64 recurrence on the engine's reward / done / maxq,
+        bootstrapped by the fp64 MLP on obs[T]: within 4x the distance of the same computation in fp32 NumPy (fp32
+        bootstrap forward + fp32 recurrence) from fp64, or 4 fp32 ulps of max |target| if that is larger;
+      - transition rows: actions in [0, 3), done in {0, 1}, reward fp32 -0.1 (REW_SCALE x -1) where done is 0 and
+        -0.0 at a terminal.  No episode reaches the 500-step limit in 128 steps, so every done is a terminal.
+    Measured on one NVIDIA H100 80GB HBM3 (700 W power limit): worst |maxq - fp64| 6.6e-7; targets worst error
+    1.84e-6 = 1.00x the fp32 spread.  The kernel's recurrence does the fp32 NumPy recurrence's operations in the same
+    order without FMA contraction (pqn_env.cu), so the two agree away from the bootstrap and share their worst element.
+    Replacing gamma * lambda * delta by gamma * delta in the kernel misses by 1.9e6x the spread."""
     from purejaxql_b200 import config_loader, envs, pqn_gymnax
     name, n, atol = "Acrobot-v1", 65536, 2e-5
     oenv = G.make(name)
@@ -273,7 +285,17 @@ def test_config4_acrobot_65536_env_step_and_train():
     cfg = {**c, **c["alg"]}
     T = cfg["NUM_STEPS"]
     cfg["TOTAL_TIMESTEPS"] = cfg["TOTAL_TIMESTEPS_DECAY"] = float(2 * T * 65536)   # SURVEY 8: must override (0 updates)
-    out = pqn_gymnax.make_train(cfg)(jr.split(jr.PRNGKey(0), 1))
+    train = pqn_gymnax.make_train(cfg)
+    eng = train.engine
+    snap = {}
+
+    def grab(n_upd, b):                              # static buffers: copy them before the next update rewrites them
+        if n_upd == 0:
+            snap["params"] = b["params"].clone()     # update 1 rolls out and bootstraps with these
+        else:
+            snap.update({k: b[k][0].cpu().numpy() for k in ("obs", "reward", "done", "maxq", "targets", "action")})
+    eng.on_update_end = grab
+    out = train(jr.split(jr.PRNGKey(0), 1))
     m = out["metrics"]
     assert m["td_loss"].shape == (1, 2) and torch.isfinite(m["td_loss"]).all()
     assert m["env_step"][0].tolist() == [T * 65536, 2 * T * 65536]
@@ -282,3 +304,32 @@ def test_config4_acrobot_65536_env_step_and_train():
     assert "env_frame" not in m                                           # pqn_gymnax.py:324-331 has no env_frame
     # Acrobot: reward -1 per step, timestep of the LogWrapper advances by one per env per step
     assert float(m["timestep"][0, 0]) > 0 and float(m["returned_episode_returns"][0, -1]) <= 0.0
+
+    # ---- update 1, teacher-forced on its own buffers
+    E = 65536
+    obs, reward, done, maxq, targets, action = (snap[k] for k in ("obs", "reward", "done", "maxq", "targets", "action"))
+    assert obs.shape[:2] == (T + 1, E) and reward.shape == done.shape == maxq.shape == targets.shape == (T, E)
+    p32 = _seed_params(eng, eng.spec.unflatten(snap["params"]), 0)
+    p64 = {k: v.astype(np.float64) for k, v in p32.items()}
+    assert eng.A == 3
+    assert ((action >= 0) & (action < 3)).all()
+    assert np.isin(done, (0, 1)).all()
+    want_bits = np.where(done == 1, np.float32(-0.0).view(np.uint32), np.float32(-0.1).view(np.uint32))
+    assert np.array_equal(reward.view(np.uint32), want_bits)
+    worst_q = 0.0
+    for t in range(T):
+        e = np.arange(t % 16, E, 16)
+        q64 = R.mlp_forward(p64, obs[t, e].astype(np.float64)).max(-1)
+        worst_q = max(worst_q, float(np.abs(maxq[t, e] - q64).max()))
+    assert worst_q < 1e-5, worst_q
+    gamma, lam = cfg["GAMMA"], cfg["LAMBDA"]
+    assert (gamma, lam) == (0.99, 0.95)
+    last64 = R.mlp_forward(p64, obs[T].astype(np.float64)).max(-1)
+    want = R.q_lambda_targets(reward.astype(np.float64), done, maxq.astype(np.float64)[..., None], last64, gamma, lam)
+    want32 = R.q_lambda_targets(reward, done, maxq[..., None], R.mlp_forward(p32, obs[T]).max(-1), gamma, lam)
+    err = float(np.abs(targets - want).max())
+    spread = float(np.abs(want32 - want).max())
+    bound = max(4 * spread, 4 * 2.0 ** -23 * float(np.abs(want).max()))
+    print(f"\n[config4 update 1] {int(done.sum())} terminals; worst |maxq - fp64| {worst_q:.2e}; targets: worst err "
+          f"{err:.2e}, fp32 spread {spread:.2e}, err / spread {err / max(spread, 1e-30):.2f}, bound {bound:.2e}")
+    assert err <= bound, (err, spread, bound)
