@@ -1215,22 +1215,24 @@ __device__ __forceinline__ void conv_mma_block2_exp(const uint32_t* __restrict__
   }
 }
 
-// LayerNorm statistics over the 16 channels of pixel rows g (z[.][0..1]) and g+8 (z[.][2..3]); quad reduction
+// LayerNorm statistics over the 16 channels of pixel rows g (z[.][0..1]) and g+8 (z[.][2..3]); quad reduction.
+// Every rounding is spelled out (no FMA contraction left to the compiler): the fp16 conv backward rebuilds rstd and
+// xhat with this function and must land on the training forward's bits.
 __device__ __forceinline__ void ln16_quad(const float (&z)[2][4], float& mean0, float& rstd0, float& mean1,
                                           float& rstd1) {
   float s0 = z[0][0] + z[0][1] + z[1][0] + z[1][1];
-  float q0 = z[0][0] * z[0][0] + z[0][1] * z[0][1] + z[1][0] * z[1][0] + z[1][1] * z[1][1];
+  float q0 = fmaf(z[1][1], z[1][1], fmaf(z[1][0], z[1][0], fmaf(z[0][0], z[0][0], __fmul_rn(z[0][1], z[0][1]))));
   float s1 = z[0][2] + z[0][3] + z[1][2] + z[1][3];
-  float q1 = z[0][2] * z[0][2] + z[0][3] * z[0][3] + z[1][2] * z[1][2] + z[1][3] * z[1][3];
+  float q1 = fmaf(z[1][3], z[1][3], fmaf(z[1][2], z[1][2], fmaf(z[0][2], z[0][2], __fmul_rn(z[0][3], z[0][3]))));
 #pragma unroll
   for (int o = 1; o <= 2; o <<= 1) {
     s0 += __shfl_xor_sync(0xffffffffu, s0, o); q0 += __shfl_xor_sync(0xffffffffu, q0, o);
     s1 += __shfl_xor_sync(0xffffffffu, s1, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
   }
-  mean0 = s0 * (1.0f / CONV_O); mean1 = s1 * (1.0f / CONV_O);
+  mean0 = __fmul_rn(s0, 1.0f / CONV_O); mean1 = __fmul_rn(s1, 1.0f / CONV_O);
   // MUFU.RSQ (2 ulp) instead of the IEEE 1/sqrt sequence, whose slow-path branches cost more than the conv MMAs
-  rstd0 = rsqrtf(fmaxf(q0 * (1.0f / CONV_O) - mean0 * mean0, 0.f) + LN_EPS);
-  rstd1 = rsqrtf(fmaxf(q1 * (1.0f / CONV_O) - mean1 * mean1, 0.f) + LN_EPS);
+  rstd0 = rsqrtf(fmaxf(fmaf(q0, 1.0f / CONV_O, -__fmul_rn(mean0, mean0)), 0.f) + LN_EPS);
+  rstd1 = rsqrtf(fmaxf(fmaf(q1, 1.0f / CONV_O, -__fmul_rn(mean1, mean1)), 0.f) + LN_EPS);
 }
 
 constexpr int CONV_MMA_WARPS = 8;
@@ -1406,7 +1408,7 @@ struct Conv16 {
 
 // Output channel of column n (0..7) of n-tile h.  NOT the natural 8h + n: with 4 (n / 2) + 2h + (n % 2) the accumulator
 // columns (2t, 2t+1) of the two n-tiles are the four CONSECUTIVE channels 4t .. 4t+3 of a pixel, so a thread stores 16
-// bytes of xhat / 8 bytes of each fp16 plane per pixel with one instruction and no lane exchange (the kernel's time
+// bytes of fp32 h1 / 8 bytes of each fp16 plane per pixel with one instruction and no lane exchange (the kernel's time
 // follows its store instructions).
 __host__ __device__ constexpr int conv16_channel(int h, int n) { return 4 * (n >> 1) + 2 * h + (n & 1); }
 
@@ -1479,25 +1481,28 @@ __device__ __forceinline__ void store_patch16(const uint32_t* __restrict__ so, i
     *reinterpret_cast<uint4*>(row + 4 * q) = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
 }
 
-template <int C>
-__device__ __forceinline__ void conv16_block2(const uint32_t* __restrict__ xp, const uint4* __restrict__ wb,
-                                              const float* __restrict__ cb, int mbp, int lane, float (&z)[2][2][4]) {
+// conv output z of the NB m-blocks mb0 .. mb0 + NB - 1 (m-block mb = pixels 16 mb .. 16 mb + 15): z[i] holds pixel
+// rows 16 (mb0 + i) + g and + 8.  The training forward runs two m-blocks at a time, the backward one; every
+// accumulator sees the same MMA sequence either way, so both get the same bits.
+template <int C, int NB>
+__device__ __forceinline__ void conv16_blocks(const uint32_t* __restrict__ xp, const uint4* __restrict__ wb,
+                                              const float* __restrict__ cb, int mb0, int lane, float (&z)[NB][2][4]) {
   using M = Conv16<C>;
   const int g = lane >> 2, t = lane & 3;
   const uint32_t mask = (1u << (10 + t)) | (1u << (26 + t));
 #pragma unroll
-  for (int i = 0; i < 2; ++i)
+  for (int i = 0; i < NB; ++i)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       z[i][h][0] = z[i][h][2] = cb[4 * t + 2 * h];       // conv16_channel(h, 2t), (h, 2t + 1)
       z[i][h][1] = z[i][h][3] = cb[4 * t + 2 * h + 1];
     }
-  const uint32_t* r00 = xp + (32 * mbp + g) * M::ROW;
+  const uint32_t* r00 = xp + (16 * mb0 + g) * M::ROW;
 #pragma unroll
   for (int s = 0; s < M::KS; ++s) {
-    uint32_t a[2][4];
+    uint32_t a[NB][4];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < NB; ++i) {
       const uint2 w0 = *reinterpret_cast<const uint2*>(r00 + (16 * i) * M::ROW + 2 * s);       // pixel row g
       const uint2 w1 = *reinterpret_cast<const uint2*>(r00 + (16 * i + 8) * M::ROW + 2 * s);   // pixel row g + 8
       a[i][0] = w0.x & mask; a[i][1] = w1.x & mask; a[i][2] = w0.y & mask; a[i][3] = w1.y & mask;
@@ -1505,16 +1510,32 @@ __device__ __forceinline__ void conv16_block2(const uint32_t* __restrict__ xp, c
     uint4 b[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) b[h] = wb[(s * 2 + h) * 32 + lane];
-    // lo pass of all four accumulators, then the hi pass: no back-to-back dependent MMAs
+    // lo pass of all accumulators, then the hi pass: no back-to-back dependent MMAs
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int i = 0; i < 2; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].z, b[h].w);
+      for (int i = 0; i < NB; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].z, b[h].w);
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int i = 0; i < 2; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].x, b[h].y);
+      for (int i = 0; i < NB; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].x, b[h].y);
   }
+}
+
+// LayerNorm of one m-block of conv16_blocks: xhat of pixel rows 16 mb + g (x0) and + 8 (x1) in the thread's channels
+// 4t .. 4t+3, and the rows' rstd.  xhat = z * rstd - mean * rstd: one FFMA per element.
+__device__ __forceinline__ void conv16_xhat(const float (&z)[2][4], float (&x0)[4], float (&x1)[4], float& rstd0,
+                                            float& rstd1) {
+  float mean0, mean1;
+  ln16_quad(z, mean0, rstd0, mean1, rstd1);
+  const float nm0 = -__fmul_rn(mean0, rstd0), nm1 = -__fmul_rn(mean1, rstd1);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      x0[2 * h + c] = fmaf(z[h][c], rstd0, nm0);
+      x1[2 * h + c] = fmaf(z[h][2 + c], rstd1, nm1);
+    }
 }
 
 __device__ __forceinline__ uint32_t cvt_f16x2_satfinite(float lo, float hi) {
@@ -1533,8 +1554,7 @@ template <int C, bool TRAIN, bool H16>
 __global__ void __launch_bounds__(CONV16_WARPS * 32, CONV16_CTAS_PER_SM)
     conv_fwd_mma16_kernel(const uint32_t* __restrict__ obs, int64_t obs_rows_per_seed, const int32_t* __restrict__ gather,
                           const float* __restrict__ params, int64_t P, pqn_net_layout_t L, float* __restrict__ H1,
-                          float* __restrict__ H1LO, float* __restrict__ XH1, float* __restrict__ RS1,
-                          uint32_t* __restrict__ RB, float* __restrict__ bn_sums, int rows) {
+                          float* __restrict__ H1LO, uint32_t* __restrict__ RB, float* __restrict__ bn_sums, int rows) {
   using Cfg = ConvCfg<C>;
   using M = Conv16<C>;
   __shared__ __align__(16) uint4 wb[M::KS * 2 * 32];
@@ -1598,38 +1618,27 @@ __global__ void __launch_bounds__(CONV16_WARPS * 32, CONV16_CTAS_PER_SM)
     float* __restrict__ hrow = H16 ? nullptr : H1 + grow * FLAT_CNN;
     __half* __restrict__ hrow16 = H16 ? reinterpret_cast<__half*>(H1) + grow * FLAT_CNN : nullptr;
     __half* __restrict__ lrow16 = H16 ? reinterpret_cast<__half*>(H1LO) + grow * FLAT_CNN : nullptr;
-    float* __restrict__ xrow = (TRAIN && XH1) ? XH1 + grow * FLAT_CNN : nullptr;
-    float* __restrict__ rrow = (TRAIN && RS1) ? RS1 + grow * CONV_PIX : nullptr;
     uint16_t* __restrict__ brow = (TRAIN && RB) ? reinterpret_cast<uint16_t*>(RB + grow * (FLAT_CNN / 32)) : nullptr;
-    // rstd and the ReLU masks of m-block t are kept by lane t of every quad and stored once per sample (2 + 2 store
-    // instructions instead of 8 + 8 predicated ones)
-    float keep_rs0 = 0.f, keep_rs1 = 0.f;
+    // the ReLU masks of m-block t are kept by lane t of every quad and stored once per sample (2 store instructions
+    // instead of 8 predicated ones)
     uint32_t keep_rb = 0u;
 #pragma unroll 1
     for (int mbp = 0; mbp < 2; ++mbp) {
       float z2[2][2][4];
-      conv16_block2<C>(sxp[warp], wb, cb, mbp, lane, z2);
+      conv16_blocks<C, 2>(sxp[warp], wb, cb, 2 * mbp, lane, z2);
 #pragma unroll
       for (int mi = 0; mi < 2; ++mi) {
         const int mb = 2 * mbp + mi;
-        float (&z)[2][4] = z2[mi];
-        float mean0, rstd0, mean1, rstd1;
-        ln16_quad(z, mean0, rstd0, mean1, rstd1);
-        const float nm0 = -mean0 * rstd0, nm1 = -mean1 * rstd1;   // xhat = z * rstd - mean * rstd: one FFMA
+        float x0[4], x1[4], rstd0, rstd1;
+        conv16_xhat(z2[mi], x0, x1, rstd0, rstd1);
         uint32_t rb0 = 0u, rb1 = 0u;
         // the thread's channels of pixel rows p0 = 16 mb + g and p1 = p0 + 8: 4t .. 4t+3 (n-tile h -> 4t + 2h, + 1)
         const int p0 = 16 * mb + g, p1 = p0 + 8, o4 = 4 * t;
-        float x0[4], x1[4], v0[4], v1[4];
+        float v0[4], v1[4];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int o = o4 + 2 * h + c;
-            x0[2 * h + c] = fmaf(z[h][c], rstd0, nm0);
-            x1[2 * h + c] = fmaf(z[h][2 + c], rstd1, nm1);
-            v0[2 * h + c] = fmaxf(fmaf(x0[2 * h + c], sc[o], bi[o]), 0.f);
-            v1[2 * h + c] = fmaxf(fmaf(x1[2 * h + c], sc[o], bi[o]), 0.f);
-          }
+        for (int c = 0; c < 4; ++c) {
+          v0[c] = fmaxf(fmaf(x0[c], sc[o4 + c], bi[o4 + c]), 0.f);
+          v1[c] = fmaxf(fmaf(x1[c], sc[o4 + c], bi[o4 + c]), 0.f);
         }
         if (H16) {
           // hi = fp16(h) (saturating: no inf), lo = fp16((h - hi) * 2^11); 8-byte stores
@@ -1659,11 +1668,6 @@ __global__ void __launch_bounds__(CONV16_WARPS * 32, CONV16_CTAS_PER_SM)
             rb1 |= (v1[c] > 0.f ? 1u : 0u) << (o4 + c);
           }
         }
-        if (xrow) {
-          *reinterpret_cast<float4*>(xrow + p0 * CONV_O + o4) = make_float4(x0[0], x0[1], x0[2], x0[3]);
-          *reinterpret_cast<float4*>(xrow + p1 * CONV_O + o4) = make_float4(x1[0], x1[1], x1[2], x1[3]);
-          if (t == mb) { keep_rs0 = rstd0; keep_rs1 = rstd1; }
-        }
         if (TRAIN && brow) {
           uint32_t rb = rb0 | (rb1 << 16);      // both pixel rows in one register: two shuffles instead of four
           rb |= __shfl_xor_sync(0xffffffffu, rb, 1);
@@ -1672,10 +1676,7 @@ __global__ void __launch_bounds__(CONV16_WARPS * 32, CONV16_CTAS_PER_SM)
         }
       }
     }
-    if (TRAIN) {
-      if (rrow) { rrow[16 * t + g] = keep_rs0; rrow[16 * t + g + 8] = keep_rs1; }
-      if (brow) { brow[16 * t + g] = (uint16_t)keep_rb; brow[16 * t + g + 8] = (uint16_t)(keep_rb >> 16); }
-    }
+    if (TRAIN && brow) { brow[16 * t + g] = (uint16_t)keep_rb; brow[16 * t + g + 8] = (uint16_t)(keep_rb >> 16); }
   }
   if (TRAIN && bn_sums != nullptr) {
 #pragma unroll
@@ -1966,6 +1967,11 @@ __global__ void __launch_bounds__(ConvBwdSmem<C>::WARPS * 32, 2)
 //   * 48 MMAs per sample (3 m-tiles x 2 n-tiles x 4 k-steps x {hi, lo}) instead of 96 tf32 ones.
 // Phase A works on the pixel pair (16 mb + 2g, + 1) per thread (it was (g, g + 8)): a thread's two dz values of one
 // channel are exactly one B word.  The DY / xhat stage has a row + column swizzle for that access pattern.
+// xhat and rstd are not read from memory: just before phase A handles m-block mb, the warp rebuilds that m-block's
+// conv output from the sample's packed observation with the training forward's own code (conv16_blocks,
+// conv16_xhat) and the same parameters, so they are bit for bit what the forward computed.  The rebuild costs the
+// forward's MMAs again (48 at C = 4, 96 at C = 10); it saves 4,352 bytes per sample of HBM writes in the forward and as
+// many reads here.
 // ---------------------------------------------------------------------------------------------------------------
 template <int C>
 struct ConvBwd16 {
@@ -1973,18 +1979,20 @@ struct ConvBwd16 {
   static constexpr int NG = 4 * MT;                             // tap groups of 4 per pixel pair
   static constexpr int NGP = (NG % 8 == 4) ? NG : NG + 4;       // pair stride in words: the 4 t-lanes hit distinct banks
   static constexpr int DY = 0;                                  // [64][16] upstream gradient (swizzled)
-  static constexpr int XH = DY + FLAT_CNN;                      // [64][16] saved xhat (swizzled)
-  static constexpr int RS = XH + FLAT_CNN;                      // [64] saved rstd
-  static constexpr int DZT = RS + CONV_PIX;                     // 2 planes x [16 ch][32 pair words]; aliases the obs row
+  static constexpr int XH = DY + FLAT_CNN;                      // [16][16] xhat of the m-block phase A is on (swizzled)
+  static constexpr int RS = XH + 16 * CONV_O;                   // [16] its rstd
+  static constexpr int DZT = RS + 16;                           // 2 planes x [16 ch][32 pair words]; aliases the obs row
   static constexpr int PW = DZT + 2 * CONV_O * 32;              // [32 pairs][NGP] exponent-coded pair words
-  static constexpr int WARP_FLOATS = (PW + 32 * NGP + 3) / 4 * 4;
+  static constexpr int XP = PW + 32 * NGP;                      // [64 pixels][Conv16::ROW] the forward's patch words
+  static constexpr int WARP_FLOATS = (XP + CONV_PIX * Conv16<C>::ROW + 3) / 4 * 4;
   static constexpr int WARPS = (C == 4) ? 8 : 6;                // keeps two CTAs per SM for the wider observations
-  static constexpr int BYTES = (WARPS * WARP_FLOATS + 4 * CONV_O) * 4;  // + sc[16] + s_red[48]
+  static constexpr int WB = WARPS * WARP_FLOATS;                // the forward's weight fragments, Conv16::KS x 2 x 32 uint4
+  static constexpr int BYTES = (WB + Conv16<C>::KS * 2 * 32 * 4 + 6 * CONV_O) * 4;  // + cb, sc, bi[16] + s_red[48]
 };
 
-// float offset of (pixel row p, channel column col) in the swizzled [64][16] DY / xhat stage: the rows 2g of one
-// fragment group would all start on bank 0, so odd (p / 4) swaps the two rows of a pair and odd (p / 2) swaps the
-// column halves -- the four g of a half-warp then cover the 32 banks once
+// float offset of (pixel row p, channel column col) in the swizzled [64][16] DY stage (and, with p < 16, the [16][16]
+// xhat stage): the rows 2g of one fragment group would all start on bank 0, so odd (p / 4) swaps the two rows of a pair
+// and odd (p / 2) swaps the column halves -- the four g of a half-warp then cover the 32 banks once
 __device__ __forceinline__ int cswz16(int p, int col) {
   return ((p ^ ((p >> 2) & 1)) << 4) + (col ^ (((p >> 1) & 1) << 3));
 }
@@ -1998,8 +2006,7 @@ template <int C>
 __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
     conv_bwd_mma16_kernel(const uint32_t* __restrict__ obs, int64_t obs_rows_per_seed, const int32_t* __restrict__ gather,
                           const float* __restrict__ params, int64_t P, pqn_net_layout_t L, const float* __restrict__ DY1,
-                          const float* __restrict__ XH1, const float* __restrict__ RS1, float* __restrict__ part,
-                          int rows, float gs) {
+                          float* __restrict__ part, int rows, float gs) {
   using Cfg = ConvCfg<C>;
   using M = ConvMma<C>;
   using SM = ConvBwd16<C>;
@@ -2013,15 +2020,20 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
   float* my_xh = my + SM::XH;
   float* my_rs = my + SM::RS;
   uint32_t* my_dzt = reinterpret_cast<uint32_t*>(my + SM::DZT);   // plane 0 = hi, plane 1 = lo: 512 words each
-  uint32_t* my_so = reinterpret_cast<uint32_t*>(my + SM::DZT);    // packed obs row: only needed until the pair words exist
+  uint32_t* my_so = reinterpret_cast<uint32_t*>(my + SM::DZT);    // packed obs row: only needed until the patch words exist
   uint32_t* my_pw = reinterpret_cast<uint32_t*>(my + SM::PW);
-  float* sc = smem_bwd + SM::WARPS * SM::WARP_FLOATS;
-  float* s_red = sc + CONV_O;
+  uint32_t* my_xp = reinterpret_cast<uint32_t*>(my + SM::XP);
+  uint4* wb = reinterpret_cast<uint4*>(smem_bwd + SM::WB);
+  float* cb = smem_bwd + SM::WB + Conv16<C>::KS * 2 * 32 * 4;
+  float* sc = cb + CONV_O;
+  float* bi = sc + CONV_O;   // loaded with the forward's weights, not used here
+  float* s_red = bi + CONV_O;
   float* s_w = smem_bwd;  // block-level dW reduction buffer, aliases warp 0's slice; only used after the row loop
   static_assert(Cfg::SW <= 2 * CONV_O * 32, "obs staging aliases the dz planes");
   static_assert(M::MT * 16 * CONV_O <= SM::WARP_FLOATS * SM::WARPS, "dW reduction buffer aliases the warp slices");
   static_assert(Cfg::PW <= 32, "one packed observation word per lane");
-  if (tid < CONV_O) sc[tid] = __ldg(params + (int64_t)seed * P + L.ln0_scale + tid);
+  static_assert(SM::XP % 4 == 0 && SM::WB % 4 == 0, "16-byte aligned patch rows and weight fragments");
+  conv16_load_weights<C>(params + (int64_t)seed * P, L, wb, cb, sc, bi);
   if (tid < 3 * CONV_O) s_red[tid] = 0.f;
   __syncthreads();
   float a_dsc[4] = {0.f, 0.f, 0.f, 0.f}, a_dbi[4] = {0.f, 0.f, 0.f, 0.f}, a_dcb[4] = {0.f, 0.f, 0.f, 0.f};
@@ -2047,26 +2059,21 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
   auto fetch_obs = [&](int src) -> uint32_t {
     return __ldg(obs + ((int64_t)seed * obs_rows_per_seed + src) * Cfg::PW + (lane < Cfg::PW ? lane : 0));
   };
-  auto fetch_rows = [&](int r) {  // async copy of the sample's dy / xhat / rstd rows into this warp's slice
+  auto fetch_dy = [&](int r) {  // async copy of the sample's dy row into this warp's slice
     if (r < rows) {
-      const int64_t gr = (int64_t)seed * rows + r;
-      const float* dsrc = DY1 + gr * FLAT_CNN;
-      const float* xsrc = XH1 + gr * FLAT_CNN;
+      const float* dsrc = DY1 + ((int64_t)seed * rows + r) * FLAT_CNN;
 #pragma unroll
       for (int i = 0; i < FLAT_CNN / 4 / 32; ++i) {
         const int q = i * 32 + lane, prow = q >> 2;              // 16-byte chunk q = (pixel row, column quad)
-        const int dst = cswz16(prow, (q & 3) * 4);               // the swizzles move whole chunks
-        cp_async16(my_dy + dst, dsrc + q * 4);
-        cp_async16(my_xh + dst, xsrc + q * 4);
+        cp_async16(my_dy + cswz16(prow, (q & 3) * 4), dsrc + q * 4);   // the swizzles move whole chunks
       }
-      if (lane < CONV_PIX / 4) cp_async16(my_rs + lane * 4, RS1 + gr * CONV_PIX + lane * 4);
     }
     cp_async_commit();
   };
   int row = blockIdx.x * SM::WARPS + warp;
   uint32_t pre = fetch_obs(fetch_index(row));
   int src_next = fetch_index(row + row_stride);
-  fetch_rows(row);
+  fetch_dy(row);
   for (; row < rows; row += row_stride) {
     __syncwarp();
     if (lane < Cfg::PW) my_so[lane] = pre;
@@ -2074,6 +2081,8 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
     __syncwarp();
     pre = fetch_obs(src_next);
     src_next = fetch_index(row + 2 * row_stride);
+    store_patch16<C>(my_so, lane, my_xp + lane * Conv16<C>::ROW);   // the forward's patch words, for the xhat rebuild
+    store_patch16<C>(my_so, lane + 32, my_xp + (lane + 32) * Conv16<C>::ROW);
     {  // exponent-coded pair words of pixel pair `lane`
       uint32_t w0[PWD], w1[PWD];
       patch_bits<C>(my_so, 2 * lane, w0);
@@ -2103,6 +2112,16 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
     // ---- phase A: LayerNorm backward of the pixel pair (16 mb + 2g, + 1); dz * gs -> fp16 (hi, lo) planes
 #pragma unroll 1
     for (int mb = 0; mb < 4; ++mb) {
+      {  // xhat / rstd of m-block mb, rebuilt as the forward computed them, into the [16][16] stage
+        float zc[1][2][4], x0[4], x1[4], rs0, rs1;
+        conv16_blocks<C, 1>(my_xp, wb, cb, mb, lane, zc);
+        conv16_xhat(zc[0], x0, x1, rs0, rs1);
+        __syncwarp();   // phase A of the previous m-block is done with the stage
+        *reinterpret_cast<float4*>(my_xh + cswz16(g, 4 * t)) = make_float4(x0[0], x0[1], x0[2], x0[3]);
+        *reinterpret_cast<float4*>(my_xh + cswz16(g + 8, 4 * t)) = make_float4(x1[0], x1[1], x1[2], x1[3]);
+        if (t == 0) { my_rs[g] = rs0; my_rs[g + 8] = rs1; }
+        __syncwarp();
+      }
       const int p0 = 16 * mb + 2 * g, p1 = p0 + 1;
       float z[2][4];
       float2 dyv[2][2];
@@ -2110,13 +2129,13 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
       for (int h = 0; h < 2; ++h) {
         dyv[h][0] = *reinterpret_cast<const float2*>(my_dy + cswz16(p0, 8 * h + 2 * t));
         dyv[h][1] = *reinterpret_cast<const float2*>(my_dy + cswz16(p1, 8 * h + 2 * t));
-        const float2 a0 = *reinterpret_cast<const float2*>(my_xh + cswz16(p0, 8 * h + 2 * t));
-        const float2 a1 = *reinterpret_cast<const float2*>(my_xh + cswz16(p1, 8 * h + 2 * t));
+        const float2 a0 = *reinterpret_cast<const float2*>(my_xh + cswz16(2 * g, 8 * h + 2 * t));
+        const float2 a1 = *reinterpret_cast<const float2*>(my_xh + cswz16(2 * g + 1, 8 * h + 2 * t));
         z[h][0] = a0.x; z[h][1] = a0.y; z[h][2] = a1.x; z[h][3] = a1.y;
       }
       // rstd * gs: dz comes out pre-scaled for the fp16 planes (gs is a power of two; the conv-bias sum is unscaled at
       // the end), which saves a multiplication per element
-      const float rstd0 = my_rs[p0] * gs, rstd1 = my_rs[p1] * gs;
+      const float rstd0 = my_rs[2 * g] * gs, rstd1 = my_rs[2 * g + 1] * gs;
       float dxh[2][4];
       float m1a = 0.f, m2a = 0.f, m1b = 0.f, m2b = 0.f;
 #pragma unroll
@@ -2162,7 +2181,7 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
       }
     }
     __syncwarp();
-    fetch_rows(row + row_stride);  // overlaps phase B
+    fetch_dy(row + row_stride);    // overlaps phase B
     // ---- phase B: dW[tap][o] += sum_pixels x[pixel, tap] * dz[pixel][o]   (fresh accumulators per sample)
     float wacc[M::MT][2][4];
 #pragma unroll
@@ -2287,7 +2306,7 @@ struct Workspace {
   // CNN
   float *h1, *h2, *xhat2, *rstd2, *dz2;
   float *h1_lo, *dz2_lo, *w1_lo;  // 3xTF32 "lo" operands of the TF32 path; regions of the fp16-split planes (Planes16)
-  float *cxhat, *crstd;           // conv LayerNorm xhat / rstd saved by the training forward (MMA conv path)
+  float *cxhat, *crstd;           // conv LayerNorm xhat / rstd saved by the training forward (tf32 conv path 3 only)
   uint32_t* relu_bits;            // packed (h1 > 0) mask, 1024 bits per row (MMA conv path -> tensor-core dgrad epilogue)
   float *rb_part, *cb_part;       // per-CTA partial vectors of the deterministic row_bwd / conv_bwd reductions
   float* wg_part;                 // split-K partial outputs of the tensor-core weight gradient (small S: few output tiles)
@@ -2536,12 +2555,11 @@ static int launch_conv_bwd_mma(dim3 grid, cudaStream_t st, const uint32_t* obs, 
 template <int C>
 static int launch_conv_bwd_mma16(dim3 grid, cudaStream_t st, const uint32_t* obs, int64_t orps, const int32_t* gather,
                                  const float* params, int64_t P, const pqn_net_layout_t& L, const float* dy1,
-                                 const float* xh1, const float* rs1, float* grads, float* part, int rows, float gs) {
+                                 float* grads, float* part, int rows, float gs) {
   auto kfn = conv_bwd_mma16_kernel<C>;
   if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, ConvBwd16<C>::BYTES) != cudaSuccess)
     return check_launch("conv_bwd_mma16(cudaFuncSetAttribute)");
-  kfn<<<grid, ConvBwd16<C>::WARPS * 32, ConvBwd16<C>::BYTES, st>>>(obs, orps, gather, params, P, L, dy1, xh1, rs1, part,
-                                                                   rows, gs);
+  kfn<<<grid, ConvBwd16<C>::WARPS * 32, ConvBwd16<C>::BYTES, st>>>(obs, orps, gather, params, P, L, dy1, part, rows, gs);
   const int n = 9 * C * CONV_O + 3 * CONV_O;
   if (final_slices((int)grid.x) == 32)
     conv_bwd_final_kernel<32><<<dim3(cdiv(n, 8), grid.y), 256, 0, st>>>(part, (int)grid.x, 9 * C * CONV_O, grads, P, L);
@@ -2636,8 +2654,8 @@ static int launch_conv_fwd(int C, dim3 grid, cudaStream_t st, const uint32_t* ob
     const dim3 mg(conv_mma_ctas((int)grid.y, rows, CONV16_CTAS_PER_SM), grid.y);
     LaunchScope _ls(TRAIN ? K_CONV_FWD : K_CONV_FWD_INFER, st);
 #define PQN_CONV16(CC)                                                                                              \
-  if (h16) conv_fwd_mma16_kernel<CC, TRAIN, true><<<mg, CONV16_WARPS * 32, 0, st>>>(obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, rb, bn, rows); \
-  else conv_fwd_mma16_kernel<CC, TRAIN, false><<<mg, CONV16_WARPS * 32, 0, st>>>(obs, orps, gather, params, P, L, h1, h1lo, xh1, rs1, rb, bn, rows)
+  if (h16) conv_fwd_mma16_kernel<CC, TRAIN, true><<<mg, CONV16_WARPS * 32, 0, st>>>(obs, orps, gather, params, P, L, h1, h1lo, rb, bn, rows); \
+  else conv_fwd_mma16_kernel<CC, TRAIN, false><<<mg, CONV16_WARPS * 32, 0, st>>>(obs, orps, gather, params, P, L, h1, h1lo, rb, bn, rows)
     switch (C) {
       case 4: PQN_CONV16(4); break;
       case 6: PQN_CONV16(6); break;
@@ -3356,7 +3374,7 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
     const float gscale = f16 ? grad_scale(rows) : 1.0f;
     launch_conv_fwd<true>(d->in_c, dim3(cdiv(rows, 4), S), st, ob, obs_rows_per_seed, gather, params, P, L,
                           conv16 ? (float*)pl.h1_hi : w.h1, conv16 ? (float*)pl.h1_lo : nullptr, bn_sums, R,
-                          g_conv_mma ? w.cxhat : nullptr, g_conv_mma ? w.crstd : nullptr,
+                          g_conv_mma == 3 ? w.cxhat : nullptr, g_conv_mma == 3 ? w.crstd : nullptr,
                           (g_conv_mma == 1 || g_conv_mma == 3) ? w.relu_bits : nullptr, conv16);
     if (f16) {
       if (!conv16) launch_split16_h1(w.h1, pl, (int64_t)S * rows * FLAT_CNN, st);
@@ -3396,10 +3414,10 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
       const float gs16 = grad_scale((int)rows) * (1.0f / 16.0f);
       if (g_conv_mma == 1) {
         switch (d->in_c) {
-          case 4: rc = launch_conv_bwd_mma16<4>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, w.cxhat, w.crstd, grads, w.cb_part, R, gs16); break;
-          case 6: rc = launch_conv_bwd_mma16<6>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, w.cxhat, w.crstd, grads, w.cb_part, R, gs16); break;
-          case 7: rc = launch_conv_bwd_mma16<7>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, w.cxhat, w.crstd, grads, w.cb_part, R, gs16); break;
-          case 10: rc = launch_conv_bwd_mma16<10>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, w.cxhat, w.crstd, grads, w.cb_part, R, gs16); break;
+          case 4: rc = launch_conv_bwd_mma16<4>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, grads, w.cb_part, R, gs16); break;
+          case 6: rc = launch_conv_bwd_mma16<6>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, grads, w.cb_part, R, gs16); break;
+          case 7: rc = launch_conv_bwd_mma16<7>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, grads, w.cb_part, R, gs16); break;
+          case 10: rc = launch_conv_bwd_mma16<10>(mg, st, ob, obs_rows_per_seed, gather, params, P, L, w.h1, grads, w.cb_part, R, gs16); break;
         }
       } else
       switch (d->in_c) {
