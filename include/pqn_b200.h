@@ -332,6 +332,11 @@ int pqn_set_tensor_core_path(int on);
  *  mma.sync kernel; 0 = fp32 CUDA cores; any other value is rejected (PQN_E_UNSUPPORTED).  The conv weight gradient
  *  runs on mma.sync for 1 and 3. */
 int pqn_set_conv_mma_path(int on);
+/*  conv fused into the dense forward GEMM of pqn_qnet_forward (tensor-core path 2 with conv path 1): 1 (default) = the
+ *  GEMM computes h1 from the packed observations, so the h1 planes are neither written nor read; 0 = the conv kernel
+ *  and the GEMM as two launches.  The Q values are bit-identical either way; pqn_qnet_loss_grad is not affected.  Any
+ *  other value is rejected (PQN_E_UNSUPPORTED). */
+int pqn_set_conv_fusion(int on);
 
 /* ---- tensor-core (sm_90a) paths of the dense contractions ----------
  * lo[i] = x[i] - trunc_tf32(x[i]): the error-compensation operand of 3xTF32. */

@@ -99,6 +99,7 @@ _SIGS = {
     "pqn_bn_stats_update": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int64, c_float, c_float, c_void_p]),
     "pqn_set_tensor_core_path": (c_int, [c_int]),
     "pqn_set_conv_mma_path": (c_int, [c_int]),
+    "pqn_set_conv_fusion": (c_int, [c_int]),
     "pqn_tc_split_lo": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "pqn_tc_split16": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_float, c_void_p]),
     "pqn_tc_gemm_test": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,

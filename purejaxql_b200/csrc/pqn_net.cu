@@ -17,22 +17,21 @@
 #include "../../include/pqn_b200.h"
 #include "api_common.h"
 #include "tc_common.cuh"
+#include "conv16.cuh"
 
 namespace pqn {
 
 constexpr int GT = 256;   // threads per GEMM CTA (16 x 16)
 constexpr int BK = 16;    // reduce-dim tile
-constexpr float LN_EPS = 1e-6f;
-constexpr int CONV_O = 16;   // conv output channels
-constexpr int CONV_PIX = 64; // 8x8 output pixels
-constexpr int HID_CNN = 128;
-constexpr int FLAT_CNN = CONV_PIX * CONV_O;  // 1024
 
 // wgmma path for the CNN dense layer (pqn_set_tensor_core_path); default on
 static int g_use_tc = 2;  // 0 FFMA, 1 3xTF32 on mma.sync (A_lo derived in the kernel), 2 wgmma on fp16-split planes (default)
 // warp-level tensor-core (mma.sync tf32) conv kernels (pqn_set_conv_mma_path); default on
 static int g_conv_mma = 1;   // 0: fp32 CUDA cores, 1: fp16 mma.sync forward (default), 3: tf32 mma.sync forward
                              // (1, 3: mma.sync backward)
+// the Q-value forward (rollout, bootstrap, evaluation) computes the conv inside the dense forward GEMM
+// (pqn_set_conv_fusion), with tensor-core path 2 and conv path 1; default on
+static int g_conv_fuse = 1;
 
 __host__ __device__ static inline int64_t align4(int64_t x) { return (x + 3) & ~(int64_t)3; }
 
@@ -750,14 +749,6 @@ __global__ void row_bwd_final_kernel(const float* __restrict__ part, int nctas, 
 // MinAtar conv 3x3 (C -> 16, VALID) + LayerNorm(16) + ReLU from bit-packed obs.
 // thread = (sample, output pixel); block = 4 samples; grid = (ceil(rows/4), S)
 // ---------------------------------------------------------------------------
-template <int C>
-struct ConvCfg {
-  static constexpr int TAPS = 9 * C;
-  static constexpr int OBS_BITS = 100 * C;
-  static constexpr int OBS_WORDS = (OBS_BITS + 31) / 32;
-  static constexpr int PW = (OBS_WORDS + 3) / 4 * 4;       // packed row words (matches env OBS_WORDS_PAD)
-  static constexpr int SW = PW + 1;                        // smem row (+1 so the funnel shift may read past the end)
-};
 
 // the C channel bits of input pixel p of a packed row held in shared memory
 template <int C>
@@ -1071,33 +1062,6 @@ struct ConvMma {
   static constexpr int MT = (TAPS + 15) / 16;  // m-blocks of the weight-gradient GEMM (taps)
 };
 
-// im2col "patch" of one output pixel as bits: bit k = tap k = (di*3+dj)*C + c, i.e. obs bit
-// ((y+di)*10 + x+dj)*C + c.  9C <= 90 bits -> PatchCfg::WORDS words; bits beyond 9C are zero.  Built once per
-// sample into shared memory (patch[pixel][word]); the MMA fragment builders then test bits with a shift instead of
-// re-deriving the observation bit address for every (pixel, tap) pair.
-template <int C>
-struct PatchCfg {
-  static constexpr int WORDS = (9 * C + 31) / 32;
-};
-
-// The 9C patch bits of output pixel `pix` as PatchCfg::WORDS words.  The packed observation is pixel-major /
-// channel-minor, so the three taps (dj = 0..2) x C channels of one patch row are 3C CONSECUTIVE bits of the input row:
-// three funnel-shift extracts instead of nine per-pixel ones.
-template <int C>
-__device__ __forceinline__ void patch_bits(const uint32_t* __restrict__ so, int pix, uint32_t (&w)[PatchCfg<C>::WORDS]) {
-  constexpr int W = PatchCfg<C>::WORDS;
-#pragma unroll
-  for (int k = 0; k < W; ++k) w[k] = 0u;
-  const int y = pix >> 3, x = pix & 7;
-#pragma unroll
-  for (int di = 0; di < 3; ++di) {
-    const int f0 = ((y + di) * 10 + x) * C;
-    const uint32_t r = __funnelshift_r(so[f0 >> 5], so[(f0 >> 5) + 1], f0 & 31) & ((1u << (3 * C)) - 1u);
-    const int o = 3 * C * di;  // compile-time after unrolling
-    w[o >> 5] |= r << (o & 31);
-    if ((o & 31) + 3 * C > 32) w[min((o >> 5) + 1, W - 1)] |= r >> (32 - (o & 31));
-  }
-}
 
 template <int C>
 __device__ __forceinline__ void build_patch(const uint32_t* __restrict__ so, int pix, uint32_t* __restrict__ out) {
@@ -1215,25 +1179,6 @@ __device__ __forceinline__ void conv_mma_block2_exp(const uint32_t* __restrict__
   }
 }
 
-// LayerNorm statistics over the 16 channels of pixel rows g (z[.][0..1]) and g+8 (z[.][2..3]); quad reduction.
-// Every rounding is spelled out (no FMA contraction left to the compiler): the fp16 conv backward rebuilds rstd and
-// xhat with this function and must land on the training forward's bits.
-__device__ __forceinline__ void ln16_quad(const float (&z)[2][4], float& mean0, float& rstd0, float& mean1,
-                                          float& rstd1) {
-  float s0 = z[0][0] + z[0][1] + z[1][0] + z[1][1];
-  float q0 = fmaf(z[1][1], z[1][1], fmaf(z[1][0], z[1][0], fmaf(z[0][0], z[0][0], __fmul_rn(z[0][1], z[0][1]))));
-  float s1 = z[0][2] + z[0][3] + z[1][2] + z[1][3];
-  float q1 = fmaf(z[1][3], z[1][3], fmaf(z[1][2], z[1][2], fmaf(z[0][2], z[0][2], __fmul_rn(z[0][3], z[0][3]))));
-#pragma unroll
-  for (int o = 1; o <= 2; o <<= 1) {
-    s0 += __shfl_xor_sync(0xffffffffu, s0, o); q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-    s1 += __shfl_xor_sync(0xffffffffu, s1, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-  }
-  mean0 = __fmul_rn(s0, 1.0f / CONV_O); mean1 = __fmul_rn(s1, 1.0f / CONV_O);
-  // MUFU.RSQ (2 ulp) instead of the IEEE 1/sqrt sequence, whose slow-path branches cost more than the conv MMAs
-  rstd0 = rsqrtf(fmaxf(fmaf(q0, 1.0f / CONV_O, -__fmul_rn(mean0, mean0)), 0.f) + LN_EPS);
-  rstd1 = rsqrtf(fmaxf(fmaf(q1, 1.0f / CONV_O, -__fmul_rn(mean1, mean1)), 0.f) + LN_EPS);
-}
 
 constexpr int CONV_MMA_WARPS = 8;
 
@@ -1378,171 +1323,6 @@ __global__ void __launch_bounds__(CONV_MMA_WARPS * 32, 3)
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// conv forward on fp16 warp-level MMA (mma.sync.m16n8k16, fp32 accumulate) -- the default conv path of round 2.
-// Same structure as conv_fwd_mma_kernel (one sample per warp, quad-level LayerNorm), but
-//   * the {0,1} im2col operand is fp16 and "exponent coded": per output pixel and k-step of 16 taps two words hold the
-//     tap bits at the exponent bits 10..13 of the low half and 26..29 of the high half; lane t of the fragment masks
-//     bit (10 + t) / (26 + t), which turns a set bit into the fp16 power of two 2^(2^t - 15) (one LOP3 per register
-//     that carries TWO k values) and row k of B is pre-multiplied by the inverse power of two (exact), so every product
-//     equals the plain 0/1 product;
-//   * weights/255 are split into fp16 hi + lo (22 significant bits, like the tf32 hi/lo pair);
-//   * K = 9C taps padded to 16 needs ceil(9C/16) k-steps (3 for C = 4) instead of ceil(9C/8) = 5 tf32 ones: 48 MMAs
-//     and 48 fragment LOP3s per sample instead of 80 / 80 (the tf32 kernel's top stall was the mma.sync pipe).
-// k order inside a k-step (free to choose, B is laid out to match): fragment column 2t <-> tap 16s + t,
-// 2t+1 <-> 16s + 4 + t, 2t+8 <-> 16s + 8 + t, 2t+9 <-> 16s + 12 + t.
-// ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mma_f16_16n8k16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <int C>
-struct Conv16 {
-  static constexpr int TAPS = 9 * C;
-  static constexpr int KS = (TAPS + 15) / 16;          // k-steps of 16 taps
-  static constexpr int ROW = 2 * KS < 8 ? 8 : 2 * KS;  // padded row: 8 or 12 words keep the 4-row LDS.64 groups apart
-};
-
-// Output channel of column n (0..7) of n-tile h.  NOT the natural 8h + n: with 4 (n / 2) + 2h + (n % 2) the accumulator
-// columns (2t, 2t+1) of the two n-tiles are the four CONSECUTIVE channels 4t .. 4t+3 of a pixel, so a thread stores 16
-// bytes of fp32 h1 / 8 bytes of each fp16 plane per pixel with one instruction and no lane exchange (the kernel's time
-// follows its store instructions).
-__host__ __device__ constexpr int conv16_channel(int h, int n) { return 4 * (n >> 1) + 2 * h + (n & 1); }
-
-// tap of fragment column kk (0..15) of k-step s, see the k order above
-__host__ __device__ constexpr int conv16_tap(int s, int kk) {
-  return 16 * s + (kk < 8 ? 0 : 8) + ((kk & 1) ? 4 : 0) + ((kk & 7) >> 1);
-}
-
-// B fragments of weights/255 as fp16 (hi, lo), pre-scaled by the inverse of the A coding: wb[s][h][lane] = uint4
-// {b0_hi, b1_hi, b0_lo, b1_lo} (b0 = columns k = 2t, 2t+1; b1 = k = 2t+8, 2t+9; n = 8h + g)
-template <int C>
-__device__ __forceinline__ void conv16_load_weights(const float* __restrict__ prm, const pqn_net_layout_t& L, uint4* wb,
-                                                    float* cb, float* sc, float* bi) {
-  using M = Conv16<C>;
-  const float inv255 = 1.0f / 255.0f;
-  for (int i = threadIdx.x; i < M::KS * 2 * 32; i += blockDim.x) {
-    const int ln = i & 31, h = (i >> 5) & 1, s = i >> 6;
-    const int gg = ln >> 2, tt = ln & 3;
-    const int o = conv16_channel(h, gg);
-    const float scale = __uint_as_float((uint32_t)(127 + 15 - (1 << tt)) << 23);   // 2^(15 - 2^t), exact
-    float v[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {   // q: 0 -> k=2t, 1 -> 2t+1, 2 -> 2t+8, 3 -> 2t+9
-      const int tap = conv16_tap(s, 2 * tt + (q & 1) + (q >> 1) * 8);
-      v[q] = tap < M::TAPS ? __ldg(prm + L.conv_w + tap * CONV_O + o) * inv255 * scale : 0.f;
-      v[q] = fminf(fmaxf(v[q], -65000.f), 65000.f);
-    }
-    const __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-    const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-    const __half2 l0 = __floats2half2_rn(v[0] - f0.x, v[1] - f0.y), l1 = __floats2half2_rn(v[2] - f1.x, v[3] - f1.y);
-    wb[i] = make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
-                       *reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
-  }
-  if (threadIdx.x < CONV_O) {
-    cb[threadIdx.x] = __ldg(prm + L.conv_b + threadIdx.x);
-    sc[threadIdx.x] = __ldg(prm + L.ln0_scale + threadIdx.x);
-    bi[threadIdx.x] = __ldg(prm + L.ln0_bias + threadIdx.x);
-  }
-}
-
-// exponent-coded fp16 patch words of one output pixel: out[2s], out[2s+1] for k-step s (taps 16s..16s+7, 16s+8..16s+15).
-// Only bits 10..13 and 26..29 are meaningful (the fragment mask picks one of them per half); tap 16s+j, j<4 sits at bit
-// 10+j and tap 16s+4+j at bit 26+j.
-template <int C>
-__device__ __forceinline__ void build_patch16(const uint32_t* __restrict__ so, int pix, uint32_t* __restrict__ out) {
-  constexpr int W = PatchCfg<C>::WORDS;
-  uint32_t w[W];
-  patch_bits<C>(so, pix, w);
-#pragma unroll
-  for (int b = 0; b < 2 * Conv16<C>::KS; ++b) {
-    const int o = 8 * b;                                   // bit offset of this byte in the patch string
-    uint32_t v = (o >> 5) < W ? w[(o >> 5) < W ? (o >> 5) : 0] : 0u;
-    const int sh = o & 31;
-    const uint32_t lo = sh >= 10 ? v >> (sh - 10) : v << (10 - sh);          // bits sh..sh+3   -> 10..13
-    const uint32_t hi = sh + 4 <= 26 ? v << (26 - sh - 4) : v >> (sh + 4 - 26);  // bits sh+4..sh+7 -> 26..29
-    out[b] = __byte_perm(lo, hi, 0x7610);                  // low half from lo, high half from hi
-  }
-}
-
-// patch row of one pixel -> shared memory with 128-bit stores (ROW is 8 or 12 words; pad words are never read)
-template <int C>
-__device__ __forceinline__ void store_patch16(const uint32_t* __restrict__ so, int pix, uint32_t* __restrict__ row) {
-  using M = Conv16<C>;
-  uint32_t w[M::ROW];
-#pragma unroll
-  for (int k = 0; k < M::ROW; ++k) w[k] = 0u;
-  build_patch16<C>(so, pix, w);
-#pragma unroll
-  for (int q = 0; q < M::ROW / 4; ++q)
-    *reinterpret_cast<uint4*>(row + 4 * q) = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-}
-
-// conv output z of the NB m-blocks mb0 .. mb0 + NB - 1 (m-block mb = pixels 16 mb .. 16 mb + 15): z[i] holds pixel
-// rows 16 (mb0 + i) + g and + 8.  The training forward runs two m-blocks at a time, the backward one; every
-// accumulator sees the same MMA sequence either way, so both get the same bits.
-template <int C, int NB>
-__device__ __forceinline__ void conv16_blocks(const uint32_t* __restrict__ xp, const uint4* __restrict__ wb,
-                                              const float* __restrict__ cb, int mb0, int lane, float (&z)[NB][2][4]) {
-  using M = Conv16<C>;
-  const int g = lane >> 2, t = lane & 3;
-  const uint32_t mask = (1u << (10 + t)) | (1u << (26 + t));
-#pragma unroll
-  for (int i = 0; i < NB; ++i)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      z[i][h][0] = z[i][h][2] = cb[4 * t + 2 * h];       // conv16_channel(h, 2t), (h, 2t + 1)
-      z[i][h][1] = z[i][h][3] = cb[4 * t + 2 * h + 1];
-    }
-  const uint32_t* r00 = xp + (16 * mb0 + g) * M::ROW;
-#pragma unroll
-  for (int s = 0; s < M::KS; ++s) {
-    uint32_t a[NB][4];
-#pragma unroll
-    for (int i = 0; i < NB; ++i) {
-      const uint2 w0 = *reinterpret_cast<const uint2*>(r00 + (16 * i) * M::ROW + 2 * s);       // pixel row g
-      const uint2 w1 = *reinterpret_cast<const uint2*>(r00 + (16 * i + 8) * M::ROW + 2 * s);   // pixel row g + 8
-      a[i][0] = w0.x & mask; a[i][1] = w1.x & mask; a[i][2] = w0.y & mask; a[i][3] = w1.y & mask;
-    }
-    uint4 b[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) b[h] = wb[(s * 2 + h) * 32 + lane];
-    // lo pass of all accumulators, then the hi pass: no back-to-back dependent MMAs
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int i = 0; i < NB; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].z, b[h].w);
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int i = 0; i < NB; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].x, b[h].y);
-  }
-}
-
-// LayerNorm of one m-block of conv16_blocks: xhat of pixel rows 16 mb + g (x0) and + 8 (x1) in the thread's channels
-// 4t .. 4t+3, and the rows' rstd.  xhat = z * rstd - mean * rstd: one FFMA per element.
-__device__ __forceinline__ void conv16_xhat(const float (&z)[2][4], float (&x0)[4], float (&x1)[4], float& rstd0,
-                                            float& rstd1) {
-  float mean0, mean1;
-  ln16_quad(z, mean0, rstd0, mean1, rstd1);
-  const float nm0 = -__fmul_rn(mean0, rstd0), nm1 = -__fmul_rn(mean1, rstd1);
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      x0[2 * h + c] = fmaf(z[h][c], rstd0, nm0);
-      x1[2 * h + c] = fmaf(z[h][2 + c], rstd1, nm1);
-    }
-}
-
-__device__ __forceinline__ uint32_t cvt_f16x2_satfinite(float lo, float hi) {
-  uint32_t r;
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
 
 // 4 warps per CTA, 5 CTAs per SM = 5 warps per scheduler: 96 registers per thread.  (With 8-warp CTAs x 3 the cap is 80
 // registers and the epilogue spilled: ncu r2e, STL = 0.7 % of the instructions but 13 % of the stall samples; the
@@ -1565,7 +1345,7 @@ __global__ void __launch_bounds__(CONV16_WARPS * 32, CONV16_CTAS_PER_SM)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   const int seed = blockIdx.y;
-  conv16_load_weights<C>(params + (int64_t)seed * P, L, wb, cb, sc, bi);
+  conv16_load_weights<C>(params + (int64_t)seed * P, L, wb, cb, sc, bi, threadIdx.x, blockDim.x);
   if (TRAIN && tid < C) s_cnt[tid] = 0.f;
   __syncthreads();
   int cnt[C];
@@ -1629,30 +1409,18 @@ __global__ void __launch_bounds__(CONV16_WARPS * 32, CONV16_CTAS_PER_SM)
 #pragma unroll
       for (int mi = 0; mi < 2; ++mi) {
         const int mb = 2 * mbp + mi;
-        float x0[4], x1[4], rstd0, rstd1;
-        conv16_xhat(z2[mi], x0, x1, rstd0, rstd1);
         uint32_t rb0 = 0u, rb1 = 0u;
         // the thread's channels of pixel rows p0 = 16 mb + g and p1 = p0 + 8: 4t .. 4t+3 (n-tile h -> 4t + 2h, + 1)
         const int p0 = 16 * mb + g, p1 = p0 + 8, o4 = 4 * t;
+        const float sc4[4] = {sc[o4], sc[o4 + 1], sc[o4 + 2], sc[o4 + 3]};
+        const float bi4[4] = {bi[o4], bi[o4 + 1], bi[o4 + 2], bi[o4 + 3]};
         float v0[4], v1[4];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          v0[c] = fmaxf(fmaf(x0[c], sc[o4 + c], bi[o4 + c]), 0.f);
-          v1[c] = fmaxf(fmaf(x1[c], sc[o4 + c], bi[o4 + c]), 0.f);
-        }
+        conv16_act(z2[mi], sc4, bi4, v0, v1);
         if (H16) {
-          // hi = fp16(h) (saturating: no inf), lo = fp16((h - hi) * 2^11); 8-byte stores
+          // 8-byte stores of the (hi, lo') planes
           uint32_t hw0[2], hw1[2], lw0[2], lw1[2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            hw0[h] = cvt_f16x2_satfinite(v0[2 * h], v0[2 * h + 1]);
-            hw1[h] = cvt_f16x2_satfinite(v1[2 * h], v1[2 * h + 1]);
-            const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&hw0[h]));
-            const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&hw1[h]));
-            const __half2 l0 = __floats2half2_rn((v0[2 * h] - f0.x) * tc::TC_LO_SCALE, (v0[2 * h + 1] - f0.y) * tc::TC_LO_SCALE);
-            const __half2 l1 = __floats2half2_rn((v1[2 * h] - f1.x) * tc::TC_LO_SCALE, (v1[2 * h + 1] - f1.y) * tc::TC_LO_SCALE);
-            lw0[h] = *reinterpret_cast<const uint32_t*>(&l0); lw1[h] = *reinterpret_cast<const uint32_t*>(&l1);
-          }
+          conv16_split(v0, hw0, lw0);
+          conv16_split(v1, hw1, lw1);
           *reinterpret_cast<uint2*>(hrow16 + p0 * CONV_O + o4) = make_uint2(hw0[0], hw0[1]);
           *reinterpret_cast<uint2*>(lrow16 + p0 * CONV_O + o4) = make_uint2(lw0[0], lw0[1]);
           *reinterpret_cast<uint2*>(hrow16 + p1 * CONV_O + o4) = make_uint2(hw1[0], hw1[1]);
@@ -2033,7 +1801,7 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
   static_assert(M::MT * 16 * CONV_O <= SM::WARP_FLOATS * SM::WARPS, "dW reduction buffer aliases the warp slices");
   static_assert(Cfg::PW <= 32, "one packed observation word per lane");
   static_assert(SM::XP % 4 == 0 && SM::WB % 4 == 0, "16-byte aligned patch rows and weight fragments");
-  conv16_load_weights<C>(params + (int64_t)seed * P, L, wb, cb, sc, bi);
+  conv16_load_weights<C>(params + (int64_t)seed * P, L, wb, cb, sc, bi, threadIdx.x, blockDim.x);
   if (tid < 3 * CONV_O) s_red[tid] = 0.f;
   __syncthreads();
   float a_dsc[4] = {0.f, 0.f, 0.f, 0.f}, a_dbi[4] = {0.f, 0.f, 0.f, 0.f}, a_dcb[4] = {0.f, 0.f, 0.f, 0.f};
@@ -2787,6 +2555,26 @@ static int tc16_dense_fwd(int epi, const float* params, int64_t P, const pqn_net
   return tc::launch_gemm16(0, 1, epi, t, gs, ep, st, epi == tc::EPI_LN_HEAD ? K_TC_FWD_HEAD : K_TC_FWD);
 }
 
+// the same product and Q-head epilogue with H1 computed in the GEMM from the packed observations (tc_conv_gemm_kernel):
+// the h1 planes are neither written nor read
+static int tc16_conv_dense_fwd(int epi, int C, const uint32_t* obs, int64_t obs_rows_per_seed, const int32_t* gather,
+                               const float* params, int64_t P, const pqn_net_layout_t& L, const Workspace& w,
+                               const Planes16& pl, int A, float* q, int S, int rows, cudaStream_t st) {
+  CUtensorMap t[2];
+  int rc;
+  if ((rc = tc::make_tmap16(&t[0], pl.w1_hi, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 64))) return rc;
+  if ((rc = tc::make_tmap16(&t[1], pl.w1_lo, HID_CNN, FLAT_CNN, S, HID_CNN, (uint64_t)FLAT_CNN * HID_CNN, 64))) return rc;
+  tc::GemmShape gs = {};
+  gs.S = S; gs.M = rows; gs.m_tiles = (rows + 127) / 128; gs.n_tiles = 1; gs.k_blocks = FLAT_CNN / tc::TC_BK16;
+  tc::EpiParams ep = {};
+  ep.params = params; ep.P = P; ep.off_b = L.d0_b; ep.off_scale = L.ln1_scale; ep.off_bias = L.ln1_bias;
+  ep.off_hw = L.head_w; ep.off_hb = L.head_b; ep.A = A; ep.rows = rows;
+  ep.H = w.h2; ep.XHAT = w.xhat2; ep.RSTD = w.rstd2; ep.Q = q;
+  tc::ConvIn ci;
+  ci.obs = obs; ci.obs_rows_per_seed = obs_rows_per_seed; ci.gather = gather; ci.L = L;
+  return tc::launch_conv_gemm16(C, epi, t, gs, ep, ci, st, epi == tc::EPI_LN_HEAD ? K_TC_FWD_HEAD : K_TC_FWD);
+}
+
 static int tc16_wgrad(float* grads, int64_t P, const pqn_net_layout_t& L, const Planes16& pl, int S, int rows,
                       float gscale, float* wg_part, cudaStream_t st) {
   CUtensorMap t[4];
@@ -3206,6 +2994,12 @@ int pqn_set_conv_mma_path(int on) {
   return PQN_OK;
 }
 
+int pqn_set_conv_fusion(int on) {
+  if (on != 0 && on != 1) return set_error(PQN_E_UNSUPPORTED, "pqn_set_conv_fusion: no mode %d", on);
+  g_conv_fuse = on;
+  return PQN_OK;
+}
+
 int pqn_set_tensor_core_path(int on) {
   if (on < 0 || on > 2) return set_error(PQN_E_UNSUPPORTED, "pqn_set_tensor_core_path: no tensor-core path %d", on);
   g_use_tc = on;
@@ -3266,10 +3060,16 @@ int pqn_qnet_forward(const pqn_net_desc_t* d, const float* params, const float* 
     const bool f16 = use_tc && g_use_tc == 2;
     const Planes16 pl = planes16(w, S, rows);
     const bool conv16 = f16 && g_conv_mma == 1;   // the mma.sync conv writes the fp16 planes itself
-    launch_conv_fwd<false>(d->in_c, dim3(cdiv(rows, 4), S), st, (const uint32_t*)obs, obs_rows_per_seed, gather, params,
-                           L.total, L, conv16 ? (float*)pl.h1_hi : w.h1, conv16 ? (float*)pl.h1_lo : nullptr, nullptr,
-                           (int)rows, nullptr, nullptr, nullptr, conv16);
-    if (f16) {
+    const bool fused = conv16 && g_conv_fuse;   // ... or runs inside the dense GEMM
+    if (!fused)
+      launch_conv_fwd<false>(d->in_c, dim3(cdiv(rows, 4), S), st, (const uint32_t*)obs, obs_rows_per_seed, gather, params,
+                             L.total, L, conv16 ? (float*)pl.h1_hi : w.h1, conv16 ? (float*)pl.h1_lo : nullptr, nullptr,
+                             (int)rows, nullptr, nullptr, nullptr, conv16);
+    if (fused) {
+      launch_split16_w1(params, L.total, L.d0_w, pl, S, st);
+      if ((rc = tc16_conv_dense_fwd(tc::EPI_LN_HEAD, d->in_c, (const uint32_t*)obs, obs_rows_per_seed, gather, params,
+                                    L.total, L, w, pl, A, q, S, (int)rows, st))) return rc;
+    } else if (f16) {
       if (!conv16) launch_split16_h1(w.h1, pl, (int64_t)S * rows * FLAT_CNN, st);
       launch_split16_w1(params, L.total, L.d0_w, pl, S, st);
       if ((rc = tc16_dense_fwd(tc::EPI_LN_HEAD, params, L.total, L, w, pl, A, q, S, (int)rows, st))) return rc;

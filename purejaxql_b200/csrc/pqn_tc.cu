@@ -22,6 +22,7 @@
 #include "../../include/pqn_b200.h"
 #include "api_common.h"
 #include "tc_common.cuh"
+#include "conv16.cuh"
 
 namespace pqn {
 namespace tc {
@@ -280,6 +281,53 @@ __device__ __forceinline__ void tf32_tile(const uint8_t* smem_al, float* tile_s,
 // staging area and one thread issues the bulk store, which runs while the warpgroup goes on to the next tile's MMAs.
 // The two warpgroups do not synchronise with each other.  Rows >= gs.M are clipped by the tensor map.
 // ---------------------------------------------------------------------------
+// Tile steps of the conv-fused kernel below, written as the fp16 path of tc_gemm_kernel writes them inline (kept
+// inline there so that its code does not change); the two must stay the same arithmetic.
+// main partial of the fp16 wgmma chain -> fp32 tile (first: store, else add); rows fr, fr + 8, columns 8 j + fc, + 1
+__device__ __forceinline__ void promote_main(float* tile_s, const float (&mainacc)[64], int fr, int fc, bool first) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float2* p = reinterpret_cast<float2*>(tile_s + (fr + 8 * h) * TC_ACC_LD + 8 * j + fc);
+      const float2 v = make_float2(mainacc[4 * j + 2 * h], mainacc[4 * j + 2 * h + 1]);
+      if (first) *p = v;
+      else { const float2 o = *p; *p = make_float2(o.x + v.x, o.y + v.y); }
+    }
+}
+
+// the correction accumulator (units of 2^-11), then the power-of-two output scale (exact)
+__device__ __forceinline__ void finish_corr(float* tile_s, const float (&corr)[64], int fr, int fc, int kbn, float osc) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float2* p = reinterpret_cast<float2*>(tile_s + (fr + 8 * h) * TC_ACC_LD + 8 * j + fc);
+      float2 o = kbn > 0 ? *p : make_float2(0.f, 0.f);
+      if (kbn > 0) {
+        o.x = fmaf(corr[4 * j + 2 * h], TC_LO_INV, o.x);
+        o.y = fmaf(corr[4 * j + 2 * h + 1], TC_LO_INV, o.y);
+      }
+      *p = make_float2(o.x * osc, o.y * osc);
+    }
+}
+
+// LayerNorm epilogues of a finished fp32 tile: thread t < 128 takes tile row t
+template <int EPI>
+__device__ __forceinline__ void ln_epilogue_tile(const EpiParams& ep, float* tile_s, float* sp_all, int t, int warp,
+                                                 int lane, int seed, int m0, int M) {
+  stage_epi_params<EPI>(ep, sp_all, seed, t);
+  float acc[128];
+  const float* row = tile_s + t * TC_ACC_LD;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float4 v = *reinterpret_cast<const float4*>(row + 4 * j);
+    acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
+  }
+  __syncwarp();   // the warp's own 32 rows of tile_s become its store staging area
+  epilogue_ln_row<EPI>(ep, acc, tile_s + warp * 32 * TC_ACC_LD, sp_all, lane, seed, m0 + warp * 32, M);
+}
+
 template <int EPI, bool F16>
 __host__ __device__ constexpr bool tma_store_epilogue() { return F16 && (EPI == EPI_RELU_MASK || EPI == EPI_RELU_BITS); }
 
@@ -574,6 +622,250 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 }
 
 // ---------------------------------------------------------------------------
+// Conv-fused dense forward: Z = H1 . W1 with H1 built in registers from the packed observations, so that h1 never goes
+// through HBM or shared memory.  The LayerNorm of the conv covers the 16 channels of one pixel, so the A operand of one
+// k-step of 16 (k = pixel * 16 + channel) is the conv output of one pixel for the warp's 16 rows (samples):
+//   * per k-block (4 pixels) lane (g, t) writes the exponent-coded patch words of pixel 4 kb + t for its warp's rows g
+//     and g + 8 (store_patch16) into the warp's patch buffer;
+//   * per pair of pixels the warp runs the conv chain of the conv kernels with samples as the MMA rows
+//     (conv16_blocks<C, 2>: bias, k-steps in order, lo pass then hi pass), the quad LayerNorm, scale / bias / ReLU and
+//     the fp16 split (conv16_act, conv16_split) -- the same instructions on the same operands as conv_fwd_mma16_kernel,
+//     so the same bits;
+//   * eight shuffles inside the quad turn lane t's channels 4t .. 4t+3 into the wgmma A layout (2t, 2t+1, 2t+8, 2t+9),
+//     and the three wgmmas of each pixel (lo.hi, hi.lo into corr; hi.hi into main) go out with A from registers, in the
+//     order and with the promotion of tc_gemm_kernel.
+// The A fragments are double-buffered: pixels p + 2, p + 3 are built while the wgmmas of p, p + 1 run
+// (wgmma.wait_group 1 before their registers are rewritten).  The producer loads only the W1 planes (32 KB per
+// k-block).  Observation rows of the next tile are copied (cp.async) into a second buffer during the current tile.
+// Rows >= gs.M read row gs.M - 1 and are never stored.
+// ---------------------------------------------------------------------------
+constexpr int CV_STAGE_BYTES = 2 * TC_TILE_BYTES;   // W1 hi, lo' of one k-block: MN-major boxes [64 k][64 n] x 2 each
+constexpr int CV_B_HI = 0, CV_B_LO = TC_TILE_BYTES;
+constexpr int CV_WARPS = TC_CONSUMERS / 32;
+// a whole producer warpgroup (warps 8-11, one thread of which issues the TMA loads), so that setmaxnreg can move its
+// registers to the consumers: 128 x 40 + 256 x 232 <= 64 K.  The consumers hold 128 accumulators, two A fragment
+// buffers and the conv chain at once.
+constexpr int CV_THREADS = TC_CONSUMERS + 128;
+constexpr int CV_PRODUCER_REGS = 40, CV_CONSUMER_REGS = 232;
+constexpr int CV_KB = FLAT_CNN / TC_BK16;           // 16 k-blocks of 4 pixels
+
+template <int C>
+struct ConvGemm {
+  static constexpr int PW = ConvCfg<C>::PW;
+  static constexpr int OLD = PW + 4;                          // words per observation row: 16-byte rows + zero pad words
+  static constexpr int PB_PIX = 16 * Conv16<C>::ROW;          // patch words of one pixel for a warp's 16 rows
+  // byte offsets from the 1024-aligned base
+  static constexpr int TILE = TC_STAGES * CV_STAGE_BYTES;
+  static constexpr int SP = TILE + 128 * TC_ACC_LD * 4;
+  static constexpr int WB = SP + TC_SP_FLOATS * 4;
+  static constexpr int CB = WB + Conv16<C>::KS * 2 * 32 * 16;
+  static constexpr int OBS = CB + 3 * CONV_O * 4;             // [2 buffers][warp][16 rows][OLD]
+  static constexpr int PB = OBS + 2 * CV_WARPS * 16 * OLD * 4;  // [warp][4 pixels][16 rows][ROW]
+  static constexpr int BAR = PB + CV_WARPS * 4 * PB_PIX * 4;
+  static constexpr int SMEM = BAR + 2 * TC_STAGES * 8 + 1024 /*align slack*/;
+  static_assert(WB % 16 == 0 && OBS % 16 == 0 && PB % 16 == 0 && BAR % 8 == 0, "aligned regions");
+  static_assert(SMEM <= 227 * 1024, "dynamic shared memory of the conv-fused GEMM exceeds the per-CTA limit");
+};
+
+__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+// keeps the registers of an A fragment alive (in the compiler's view) until here: an in-flight wgmma reads them
+__device__ __forceinline__ void fence_frag(uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+
+// x[0], x[1] = channel pairs 2t', 2t'+1 (channels 4t' .. 4t'+3) of lane t' of the quad -> pair t (lo) and pair t + 4
+// (hi) of lane t: two shuffles, each source lane sending the word its reader needs
+__device__ __forceinline__ void quad_pairs(const uint32_t (&x)[2], int lane, uint32_t& lo, uint32_t& hi) {
+  const int t = lane & 3, base = lane & ~3;
+  const uint32_t sa = (t >> 1) ? x[1] : x[0], sb = (t >> 1) ? x[0] : x[1];
+  const uint32_t ra = __shfl_sync(0xffffffffu, sa, base | ((t & 1) << 1) | (t >> 1));
+  const uint32_t rb = __shfl_sync(0xffffffffu, sb, base | (((t & 1) ^ 1) << 1) | (t >> 1));
+  lo = (t & 1) ? rb : ra;
+  hi = (t & 1) ? ra : rb;
+}
+
+template <int C, int EPI>
+__global__ void __launch_bounds__(CV_THREADS, 1)
+    tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
+                        const GemmShape gs, const EpiParams ep, const ConvIn ci) {
+  using G = ConvGemm<C>;
+  using M = Conv16<C>;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
+  float* tile_s = reinterpret_cast<float*>(smem_al + G::TILE);    // [128][TC_ACC_LD]
+  float* sp_all = reinterpret_cast<float*>(smem_al + G::SP);      // [TC_SP_FLOATS]
+  uint4* wb = reinterpret_cast<uint4*>(smem_al + G::WB);          // conv B fragments (conv16_load_weights)
+  float* cb = reinterpret_cast<float*>(smem_al + G::CB);
+  float* sc = cb + CONV_O;
+  float* bi = sc + CONV_O;
+  uint32_t* obs_s = reinterpret_cast<uint32_t*>(smem_al + G::OBS);
+  uint32_t* pb_s = reinterpret_cast<uint32_t*>(smem_al + G::PB);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_al + G::BAR);
+  uint64_t* empty = full + TC_STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 8 && lane == 0) {
+    prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
+    for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TC_CONSUMERS / 32); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const int tiles_per_seed = gs.m_tiles;   // one 128-wide n-tile, no split-K
+  const int num_tiles = tiles_per_seed * gs.S;
+
+  if (warp >= 8) {
+    // ===================== TMA producer: W1 planes only =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(CV_PRODUCER_REGS));
+    if (warp == 8 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int seed = tile / tiles_per_seed;
+        for (int kb = 0; kb < CV_KB; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1u);
+          const uint32_t sb = smem_base + stage * CV_STAGE_BYTES;
+          mbar_expect_tx(&full[stage], 2 * TC_TILE_BYTES);
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            tma_load_3d(sb + CV_B_HI + j * 8192, &tm_b_hi, &full[stage], 64 * j, kb * TC_BK16, seed);
+            tma_load_3d(sb + CV_B_LO + j * 8192, &tm_b_lo, &full[stage], 64 * j, kb * TC_BK16, seed);
+          }
+          if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers (warps 0-7): conv + wgmma =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CV_CONSUMER_REGS));
+  const int t = threadIdx.x;                   // 0..255
+  const int g = lane >> 2, tq = lane & 3;
+  const int fr = 16 * warp + g, fc = 2 * tq;   // accumulator rows fr, fr + 8 of the tile (warpgroup warp / 4)
+  uint32_t* my_pb = pb_s + warp * 4 * G::PB_PIX;
+  for (int i = t; i < 2 * CV_WARPS * 16; i += TC_CONSUMERS)
+    for (int w = G::PW; w < G::OLD; ++w) obs_s[i * G::OLD + w] = 0u;   // pad words read by the funnel shifts
+  // observation rows of this warp's 16 tile rows: lane l copies row l % 16, 16-byte chunks l / 16, + 2, ..
+  auto obs_src = [&](int tile) -> const uint32_t* {
+    const int seed = tile / tiles_per_seed;
+    int m = (tile - seed * tiles_per_seed) * 128 + 16 * warp + (lane & 15);
+    m = m < gs.M ? m : gs.M - 1;
+    const int64_t src = ci.gather ? __ldg(ci.gather + (int64_t)seed * gs.M + m) : m;
+    return ci.obs + ((int64_t)seed * ci.obs_rows_per_seed + src) * G::PW;
+  };
+  auto obs_copy = [&](const uint32_t* src, int buf) {
+    const uint32_t dst = smem_u32(obs_s + ((buf * CV_WARPS + warp) * 16 + (lane & 15)) * G::OLD);
+    for (int j = lane >> 4; j < G::PW / 4; j += 2) cp_async16(dst + 16 * j, src + 4 * j);
+    cp_async_commit();
+  };
+  if ((int)blockIdx.x < num_tiles) obs_copy(obs_src(blockIdx.x), 0);
+
+  int cur_seed = -1, buf = 0;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int seed = tile / tiles_per_seed, m0 = (tile - seed * tiles_per_seed) * 128;
+    const int next = tile + gridDim.x;
+    const uint32_t* next_src = next < num_tiles ? obs_src(next) : nullptr;   // copied after the first k-block
+    consumer_bar_sync();   // the previous epilogue is done with tile_s, every warp with the previous conv weights
+    if (seed != cur_seed) {
+      conv16_load_weights<C>(ep.params + (int64_t)seed * ep.P, ci.L, wb, cb, sc, bi, t, TC_CONSUMERS);
+      consumer_bar_sync();
+      cur_seed = seed;
+    }
+    cp_async_wait_all();
+    __syncwarp();
+    const uint32_t* my_obs = obs_s + (buf * CV_WARPS + warp) * 16 * G::OLD;
+
+    // A fragments (hi, lo') of pixels 4 kb + 2 half and + 1 for rows fr, fr + 8: the two pixels' conv chains run
+    // interleaved (conv16_blocks with two m-blocks, as in the conv kernel), which halves the latency per pixel
+    auto build_pair = [&](int kb, int half, uint32_t (&ah)[2][4], uint32_t (&al)[2][4]) {
+      if (half == 0) {
+        __syncwarp();   // the previous k-block's patch rows have been read
+        store_patch16<C>(my_obs + g * G::OLD, 4 * kb + tq, my_pb + tq * G::PB_PIX + g * M::ROW);
+        store_patch16<C>(my_obs + (g + 8) * G::OLD, 4 * kb + tq, my_pb + tq * G::PB_PIX + (g + 8) * M::ROW);
+        __syncwarp();
+      }
+      float z2[2][2][4];
+      conv16_blocks<C, 2>(my_pb, wb, cb, 2 * half, lane, z2);   // m-block i = pixel 2 half + i of the k-block
+      const float4 s4 = *reinterpret_cast<const float4*>(sc + 4 * tq), b4 = *reinterpret_cast<const float4*>(bi + 4 * tq);
+      const float sc4[4] = {s4.x, s4.y, s4.z, s4.w}, bi4[4] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float v0[4], v1[4];
+        conv16_act(z2[i], sc4, bi4, v0, v1);
+        uint32_t hw0[2], lw0[2], hw1[2], lw1[2];
+        conv16_split(v0, hw0, lw0);
+        conv16_split(v1, hw1, lw1);
+        quad_pairs(hw0, lane, ah[i][0], ah[i][2]);
+        quad_pairs(hw1, lane, ah[i][1], ah[i][3]);
+        quad_pairs(lw0, lane, al[i][0], al[i][2]);
+        quad_pairs(lw1, lane, al[i][1], al[i][3]);
+      }
+    };
+
+    float mainacc[64], corr[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { mainacc[i] = 0.f; corr[i] = 0.f; }
+    uint32_t ahi[2][2][4], alo[2][2][4];   // [pixel pair of the k-block][pixel][register]
+    build_pair(0, 0, ahi[0], alo[0]);
+    int prev_stage = 0;
+    for (int kb = 0; kb < CV_KB; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sb = smem_base + stage * CV_STAGE_BYTES;
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int nxt = half ^ 1;
+        wgmma_fence();
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int ks = 2 * half + i;
+          const uint64_t b_hi = make_gdesc16<1>(sb + CV_B_HI, ks), b_lo = make_gdesc16<1>(sb + CV_B_LO, ks);
+          wgmma_f16_m64n128_ra<1>(corr, alo[half][i], b_hi, (ks == 0 && kb == 0) ? 0u : 1u);
+          wgmma_f16_m64n128_ra<1>(corr, ahi[half][i], b_lo, 1u);
+          wgmma_f16_m64n128_ra<1>(mainacc, ahi[half][i], b_hi, (ks == 0 && kb % TC_PROMOTE == 0) ? 0u : 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous pixel pair's wgmmas have retired
+#pragma unroll
+        for (int i = 0; i < 2; ++i) { fence_frag(ahi[nxt][i]); fence_frag(alo[nxt][i]); }
+        if (half == 0 && kb > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev_stage]);   // the previous k-block's W1 slot is free
+        }
+        if (half == 0 && kb == 0 && next_src) obs_copy(next_src, buf ^ 1);
+        if (half == 0) build_pair(kb, 1, ahi[1], alo[1]);
+        else if (kb + 1 < CV_KB) build_pair(kb + 1, 0, ahi[0], alo[0]);
+      }
+      prev_stage = stage;
+      if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
+      if ((kb + 1) % TC_PROMOTE == 0) {
+        wgmma_wait<0>();
+        fence_operands(mainacc); fence_operands(corr);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) { fence_frag(ahi[0][i]); fence_frag(alo[0][i]); }
+        promote_main(tile_s, mainacc, fr, fc, kb < TC_PROMOTE);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) { fence_frag(ahi[1][i]); fence_frag(alo[1][i]); }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev_stage]);
+    finish_corr(tile_s, corr, fr, fc, CV_KB, ep.out_scale != 0.f ? ep.out_scale : 1.0f);
+    consumer_bar_sync();   // tile_s complete
+    if (t < 128) ln_epilogue_tile<EPI>(ep, tile_s, sp_all, t, warp, lane, seed, m0, gs.M);
+    buf ^= 1;
+  }
+  cp_async_wait_all();
+}
+
+// ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -631,6 +923,36 @@ static int launch_t(const CUtensorMap* t, const GemmShape& gs, const EpiParams& 
     kfn<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(t[0], t[1], t[2], t[3], tm_out, gs, ep);
   }
   return check_launch("tc_gemm");
+}
+
+template <int C, int EPI>
+static int launch_conv_t(const CUtensorMap* tb, const GemmShape& gs, const EpiParams& ep, const ConvIn& ci,
+                         cudaStream_t st, int kid) {
+  auto kfn = tc_conv_gemm_kernel<C, EPI>;
+  constexpr int smem = ConvGemm<C>::SMEM;
+  if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+    return check_launch("tc_conv_gemm(cudaFuncSetAttribute)");
+  const int tiles = gs.m_tiles * gs.S;
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  {
+    LaunchScope _ls(kid, st);
+    kfn<<<grid, CV_THREADS, smem, st>>>(tb[0], tb[1], gs, ep, ci);
+  }
+  return check_launch("tc_conv_gemm");
+}
+
+int launch_conv_gemm16(int C, int epi, const CUtensorMap* tb, const GemmShape& gs, const EpiParams& ep, const ConvIn& ci,
+                       cudaStream_t st, int kernel_id) {
+  if (gs.n_tiles != 1 || gs.k_split > 1 || gs.k_blocks != CV_KB)
+    return set_error(PQN_E_INVALID, "tc_conv_gemm16: N = 128, K = 1024 and no split-K");
+#define PQN_CONV_CASE(CC) \
+  if (C == CC && epi == EPI_LN_HEAD) return launch_conv_t<CC, EPI_LN_HEAD>(tb, gs, ep, ci, st, kernel_id);
+  PQN_CONV_CASE(4)
+  PQN_CONV_CASE(6)
+  PQN_CONV_CASE(7)
+  PQN_CONV_CASE(10)
+#undef PQN_CONV_CASE
+  return set_error(PQN_E_UNSUPPORTED, "tc_conv_gemm16: combination C=%d epi=%d not instantiated", C, epi);
 }
 
 int launch_gemm(int a_mn, int b_mn, int epi, const CUtensorMap* t, const GemmShape& gs, const EpiParams& ep,
