@@ -174,6 +174,16 @@ int pqn_rollout_act_step(int env_id, const uint32_t* step_keys, const float* q, 
                          float* reward, uint8_t* done, float* maxq, int64_t tr_seed_stride, double* info_sums,
                          int info_done_only, int32_t S, int32_t E, int32_t env_total, int32_t env_offset, int max_steps,
                          float rew_scale, int rng_mode, void* stream);
+/* pqn_rollout_act_step with per-seed hyperparameters (a grid of settings trained as one batched run):
+ *   eps:       float32[S]   device, the exploration rate of each seed
+ *   rew_scale: float32[S]   device, the reward scale of each seed
+ * Every other argument as above.  With every eps[s] and rew_scale[s] equal to the scalars of pqn_rollout_act_step the
+ * results are bit-identical to it: both run the same kernel. */
+int pqn_rollout_act_step_seeds(int env_id, const uint32_t* step_keys, const float* q, const float* eps,
+                               uint32_t* state, void* obs_next, int64_t obs_seed_stride, int32_t* action,
+                               float* reward, uint8_t* done, float* maxq, int64_t tr_seed_stride, double* info_sums,
+                               int info_done_only, int32_t S, int32_t E, int32_t env_total, int32_t env_offset,
+                               int max_steps, const float* rew_scale, int rng_mode, void* stream);
 /* keys_out[T][S][2][2], rng_inout[S][2]: the scan carry chain
  * rng, rng_a, rng_s = split(rng, 3) for T steps (pqn_minatar.py:183). */
 int pqn_rollout_keys(uint32_t* rng_inout, uint32_t* keys_out, int32_t S, int32_t T, int rng_mode, void* stream);
@@ -184,6 +194,10 @@ int pqn_rollout_keys(uint32_t* rng_inout, uint32_t* keys_out, int32_t S, int32_t
 int pqn_qlambda(const float* reward, const uint8_t* done, const float* maxq, const float* q_last,
                 float* targets, int32_t T, int32_t S, int32_t E, int32_t A, float gamma, float lambda,
                 void* stream);
+/* pqn_qlambda with gamma float32[S] and lambda float32[S] on the device: seed s uses gamma[s], lambda[s]. */
+int pqn_qlambda_seeds(const float* reward, const uint8_t* done, const float* maxq, const float* q_last,
+                      float* targets, int32_t T, int32_t S, int32_t E, int32_t A, const float* gamma,
+                      const float* lambda, void* stream);
 
 /* ---- Q-network (QNetwork/CNN pqn_minatar.py:24-69; MLP QNetwork pqn_gymnax.py:29-58)
  * All network entry points are batched over S independent seeds: parameter
@@ -305,6 +319,14 @@ int pqn_rnn_loss_grad_stats(const pqn_net_desc_t* desc_host, const float* params
                             const int32_t* action, const float* reward, const uint8_t* done, float* grads,
                             float* loss_sum, float* qsa_sum, int32_t S, int32_t T, int32_t B, float gamma, float lambda,
                             void* workspace, void* stream);
+/* pqn_rnn_loss_grad_stats with gamma float32[S] and lambda float32[S] on the device (seed s's in-loss Q(lambda) targets
+ * use gamma[s], lambda[s]).  batch_stats may be NULL for the default network, as in pqn_rnn_loss_grad_stats; then this
+ * is pqn_rnn_loss_grad with per-seed gamma and lambda. */
+int pqn_rnn_loss_grad_seeds(const pqn_net_desc_t* desc_host, const float* params, float* batch_stats, const float* hs0,
+                            const float* obs, const uint8_t* last_done, const int32_t* last_action,
+                            const int32_t* action, const float* reward, const uint8_t* done, float* grads,
+                            float* loss_sum, float* qsa_sum, int32_t S, int32_t T, int32_t B, const float* gamma,
+                            const float* lambda, void* workspace, void* stream);
 
 /* optax.chain(clip_by_global_norm(max_norm), radam(lr_t)) + apply_updates
  * (pqn_minatar.py:159-162,292).  sched: float32[num_steps][4] per optimizer step
@@ -313,6 +335,13 @@ int pqn_rnn_loss_grad_stats(const pqn_net_desc_t* desc_host, const float* params
 int pqn_radam_clip_step(float* params, const float* grads, float* mu, float* nu, const float* sched,
                         int32_t* step_counter, float* gnorm_scratch /*[S][64]*/, int32_t S, int64_t P,
                         float max_norm, float b1, float b2, float eps, void* stream);
+/* pqn_radam_clip_step with a schedule and a clipping norm per seed: seed s reads its row t at
+ * sched + s * sched_seed_stride + 4 * t (sched_seed_stride in floats; 0: one float32[num_steps][4] table shared by all
+ * seeds, else float32[S][num_steps][4] with sched_seed_stride = 4 * num_steps) and clips to max_norm[s] (float32[S],
+ * device).  Shared table and equal max_norm[s]: bit-identical to pqn_radam_clip_step (same kernels). */
+int pqn_radam_clip_step_seeds(float* params, const float* grads, float* mu, float* nu, const float* sched,
+                              int64_t sched_seed_stride, int32_t* step_counter, float* gnorm_scratch /*[S][64]*/,
+                              int32_t S, int64_t P, const float* max_norm, float b1, float b2, float eps, void* stream);
 
 /* dummy input BatchNorm running statistics (flax nn.BatchNorm momentum 0.99;
  * pqn_minatar.py:65,293-296): batch_stats float32[S][2][F] (mean, var),

@@ -71,9 +71,14 @@ _SIGS = {
     "pqn_rollout_act_step": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                      c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int32, c_int32,
                                      c_int32, c_int32, c_int, c_float, c_int, c_void_p]),
+    "pqn_rollout_act_step_seeds": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int32, c_int32,
+                                           c_int32, c_int32, c_int, c_void_p, c_int, c_void_p]),
     "pqn_rollout_keys": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int, c_void_p]),
     "pqn_qlambda": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
                             c_float, c_float, c_void_p]),
+    "pqn_qlambda_seeds": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                  c_void_p, c_void_p, c_void_p]),
     "pqn_net_layout": (c_int, [POINTER(NetDesc), POINTER(NetLayout)]),
     "pqn_net_dense_layer": (c_int, [POINTER(NetDesc), c_int32, POINTER(c_int64)]),
     "pqn_net_stats_floats": (c_int64, [POINTER(NetDesc)]),
@@ -94,8 +99,13 @@ _SIGS = {
     "pqn_rnn_loss_grad_stats": (c_int, [POINTER(NetDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
                                         c_int32, c_float, c_float, c_void_p, c_void_p]),
+    "pqn_rnn_loss_grad_seeds": (c_int, [POINTER(NetDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
+                                        c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pqn_radam_clip_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
                                     c_int64, c_float, c_float, c_float, c_float, c_void_p]),
+    "pqn_radam_clip_step_seeds": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                          c_void_p, c_int32, c_int64, c_void_p, c_float, c_float, c_float, c_void_p]),
     "pqn_bn_stats_update": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int64, c_float, c_float, c_void_p]),
     "pqn_set_tensor_core_path": (c_int, [c_int]),
     "pqn_set_conv_mma_path": (c_int, [c_int]),

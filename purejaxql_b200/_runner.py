@@ -9,7 +9,7 @@ import time
 
 import torch
 
-from . import config_loader, jaxrandom as jr
+from . import config_loader, jaxrandom as jr, sweep
 
 
 def init_distributed():
@@ -43,7 +43,8 @@ def pick_data_parallel(config, world, env_sharding=True):
     """"seeds" | "envs" for this run: DATA_PARALLEL (this repo's key, not in the reference) = "seeds" shards the
     independent seeds over the ranks (no collective); "envs" shards NUM_ENVS of every seed and all-reduces the
     gradient once per minibatch step; "auto" (default) picks "envs" when there are fewer seeds than GPUs (the
-    shipped default is NUM_SEEDS=1, config/config.yaml:2).  A script whose engine has no env-sharded mode
+    shipped default is NUM_SEEDS=1, config/config.yaml:2), counting every seed of a hyperparameter grid
+    (G points x NUM_SEEDS, sweep.Grid).  A script whose engine has no env-sharded mode
     (``env_sharding=False``: the recurrent one) always shards seeds, and refuses an explicit "envs"."""
     if world <= 1:
         return "seeds"
@@ -56,7 +57,7 @@ def pick_data_parallel(config, world, env_sharding=True):
                              "DATA_PARALLEL=seeds (one seed per GPU)")
         return "seeds"
     if dp == "auto":
-        dp = "envs" if int(config["NUM_SEEDS"]) < world else "seeds"
+        dp = "envs" if sweep.Grid(config).total_seeds < world else "seeds"
     if dp == "envs":
         ne = int(config["NUM_ENVS"])
         if ne % world or (int(config["NUM_STEPS"]) * ne // world) % int(config["NUM_MINIBATCHES"]):
@@ -67,7 +68,8 @@ def pick_data_parallel(config, world, env_sharding=True):
 
 def _shard_seeds(rngs):
     """Seeds are independent runs (jax.vmap over rngs, pqn_minatar.py:459-461):
-    under torchrun each rank trains a contiguous slice of the same split(key, NUM_SEEDS)."""
+    under torchrun each rank trains a contiguous slice of the same split(key, NUM_SEEDS) (tiled over the points of a
+    hyperparameter grid)."""
     import torch.distributed as dist
     if not (dist.is_available() and dist.is_initialized()):
         return rngs, 0, 1
@@ -87,21 +89,25 @@ def single_run(config, make_train, alg_file_name="pqn", env_sharding=True):
         wandb.init(entity=config["ENTITY"], project=config["PROJECT"],
                    tags=[alg_name.upper(), env_name.upper(), "b200_native"],
                    name=f'{config["ALG_NAME"]}_{config["ENV_NAME"]}', config=config, mode=config["WANDB_MODE"])
+    grid = sweep.Grid(config)                                         # lists of LR, GAMMA, ...: one batched sweep
     d_rank, d_world = init_distributed()
     env_sharded = pick_data_parallel(config, d_world, env_sharding) == "envs"
     rng = jr.PRNGKey(config["SEED"])                                  # :456
     t0 = time.time()
     rngs = jr.split(rng, config["NUM_SEEDS"], int(config.get("JAX_THREEFRY_PARTITIONABLE", 0)))   # :459
+    rngs = grid.tile(rngs)                                            # the same keys for every grid point
     if env_sharded:
         local_rngs, rank, world = rngs, 0, 1                          # every rank trains every seed on its env shard;
     else:                                                             # rank 0 alone saves (parameters are replicated)
         local_rngs, rank, world = _shard_seeds(rngs)
+    seed_lo = seed_slice(rngs.shape[0], rank, world)[0]               # global index of this rank's first seed
     if local_rngs.shape[0] == 0:
-        # NUM_SEEDS < world size in the seed-sharded mode: this rank has no run of its own (the env-sharded
+        # fewer seeds than ranks in the seed-sharded mode: this rank has no run of its own (the env-sharded
         # mode, DATA_PARALLEL=envs, is what uses every GPU for a single seed)
-        print(f"rank {rank}: no seeds assigned (NUM_SEEDS={config['NUM_SEEDS']} < world size {world})")
+        print(f"rank {rank}: no seeds assigned ({grid.total_seeds} seeds < world size {world})")
         return None
     train = make_train(config)
+    train.engine.seed_lo = seed_lo
     if env_sharded:
         train.engine.env_shard = (d_rank, d_world)
     outs = train(local_rngs)                                          # :460-461 (seed axis is native)
@@ -112,17 +118,20 @@ def single_run(config, make_train, alg_file_name="pqn", env_sharding=True):
         model_state = outs["runner_state"][0]
         save_dir = os.path.join(config["SAVE_PATH"], env_name)
         os.makedirs(save_dir, exist_ok=True)
+        prefix = f'{alg_name}_{env_name}_seed{config["SEED"]}'
         if rank == 0:
-            config_loader.save_yaml(
-                {k: v for k, v in config.items() if k != "alg"},
-                os.path.join(save_dir, f'{alg_name}_{env_name}_seed{config["SEED"]}_config.yaml'))
-        per = local_rngs.shape[0]
-        for i in range(per):
+            config_loader.save_yaml({k: v for k, v in config.items() if k != "alg"},
+                                    os.path.join(save_dir, f'{prefix}_config.yaml'))
+            if grid.G > 1:                                            # the values every checkpoint trained with
+                config_loader.save_yaml({"axes": {k: v for k, v in grid.axes}, "num_seeds": grid.num_seeds,
+                                         "seeds": grid.table(0, grid.total_seeds)},
+                                        os.path.join(save_dir, f'{prefix}_sweep.yaml'))
+        for i in range(local_rngs.shape[0]):
             def pick(d):
                 return {k: (pick(v) if isinstance(v, dict) else v[i]) for k, v in d.items()}
-            gi = seed_slice(config["NUM_SEEDS"], rank, world)[0] + i
-            save_params(pick(model_state.params),
-                        os.path.join(save_dir, f'{alg_name}_{env_name}_seed{config["SEED"]}_vmap{gi}.safetensors'))
+            gi = seed_lo + i
+            name = f"vmap{gi}" if grid.G == 1 else f"g{gi // grid.num_seeds}_vmap{gi % grid.num_seeds}"
+            save_params(pick(model_state.params), os.path.join(save_dir, f'{prefix}_{name}.safetensors'))
     return outs
 
 

@@ -22,6 +22,16 @@ enum KernelId : int {
   K_BITS_FWD, K_BITS_WGRAD /* Dense_0 of the MLP on packed MinAtar bits (pqn_bits.cuh) */, K_COUNT
 };
 
+// A hyperparameter that may differ between seeds: v[seed] when v is given (the *_seeds entry points), else the value c
+// every seed shares (the scalar entry points).  Passed by value to the kernel that reads it.
+struct SeedScalar {
+  const float* v;
+  float c;
+#ifdef __CUDACC__
+  __device__ __forceinline__ float at(int seed) const { return v ? __ldg(v + seed) : c; }
+#endif
+};
+
 // SM count of the CURRENT device (cached per device ordinal, not per process)
 int device_sm_count();
 

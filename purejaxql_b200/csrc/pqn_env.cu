@@ -205,11 +205,11 @@ __global__ void eps_greedy_kernel(const uint32_t* __restrict__ keys, const float
 template <class Env>
 __global__ void __launch_bounds__(ENV_BLOCK)
     rollout_act_step_kernel(const uint32_t* __restrict__ step_keys, const float* __restrict__ q,
-                            const float* __restrict__ eps_p, uint32_t* __restrict__ state,
+                            const float* __restrict__ eps_p, int eps_stride, uint32_t* __restrict__ state,
                             void* __restrict__ obs_next, int32_t* __restrict__ action_out,
                             float* __restrict__ reward_out, uint8_t* __restrict__ done_out,
                             float* __restrict__ maxq_out, double* __restrict__ info_sums, int E, int max_steps,
-                            float rew_scale, int part, int64_t obs_seed_stride, int64_t tr_seed_stride,
+                            SeedScalar rew_scale_s, int part, int64_t obs_seed_stride, int64_t tr_seed_stride,
                             int info_done_only, int E_total, int env_offset) {
   __shared__ uint32_t obs_smem[ObsScratch<Env>::WORDS];
   const int seed = blockIdx.y;
@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(ENV_BLOCK)
   if (active) {
     const Key ka{step_keys[seed * 4 + 0], step_keys[seed * 4 + 1]};
     const Key ks{step_keys[seed * 4 + 2], step_keys[seed * 4 + 3]};
-    const float eps = eps_p[0];
+    const float eps = eps_p[seed * eps_stride];   // eps_stride 0: one value for every seed
     float mq;
     // per-env keys are element (env_offset + e) of split(key, E_total): an env shard of a larger vmap (env-sharded
     // data parallelism) draws exactly the keys the unsharded run gives those envs
@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(ENV_BLOCK)
     const int64_t io = (int64_t)seed * obs_seed_stride + e;
     const int64_t it = (int64_t)seed * tr_seed_stride + e;
     action_out[it] = a;
-    reward_out[it] = rew_scale * r;
+    reward_out[it] = rew_scale_s.at(seed) * r;
     done_out[it] = d ? 1 : 0;
     maxq_out[it] = mq;
     if constexpr (Env::BINARY_OBS) {
@@ -295,13 +295,14 @@ __global__ void rollout_keys_kernel(uint32_t* __restrict__ rng_inout, uint32_t* 
 // buffers are [S][T][E]; one thread per (seed, env)
 __global__ void qlambda_kernel(const float* __restrict__ reward, const uint8_t* __restrict__ done,
                                const float* __restrict__ maxq, const float* __restrict__ q_last,
-                               float* __restrict__ targets, int T, int S, int E, int A, float gamma, float lambda) {
+                               float* __restrict__ targets, int T, int S, int E, int A, SeedScalar gamma,
+                               SeedScalar lambda) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)S * E) return;
   const int64_t s = i / E, e = i - s * E;
   const int64_t base = s * (int64_t)T * E;
-  qlambda_one(reward + base, done + base, maxq + base, q_last + i * A, targets + base, T, (int64_t)E, A, gamma, lambda,
-              e);
+  qlambda_one(reward + base, done + base, maxq + base, q_last + i * A, targets + base, T, (int64_t)E, A,
+              gamma.at((int)s), lambda.at((int)s), e);
 }
 
 __global__ void rng_split_kernel(const uint32_t* __restrict__ keys, int64_t n, int num, uint32_t* __restrict__ out,
@@ -400,6 +401,38 @@ static void fill_info(pqn_env_info_t* o) {
   }
 
 static inline unsigned blocks_for(int64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
+
+static int rollout_act_step(int env_id, const uint32_t* step_keys, const float* q, const float* eps, int eps_stride,
+                            uint32_t* state, void* obs_next, int64_t obs_seed_stride, int32_t* action, float* reward,
+                            uint8_t* done, float* maxq, int64_t tr_seed_stride, double* info_sums, int info_done_only,
+                            int32_t S, int32_t E, int32_t env_total, int32_t env_offset, int max_steps,
+                            SeedScalar rew_scale, int rng_mode, void* stream, const char* who) {
+  if (!step_keys || !q || !eps || !state || !obs_next || !action || !reward || !done || !maxq || S <= 0 || E <= 0)
+    return set_error(PQN_E_INVALID, "%s: bad argument", who);
+  if (env_total <= 0) { env_total = E; env_offset = 0; }
+  if (env_offset < 0 || env_offset + E > env_total)
+    return set_error(PQN_E_INVALID, "%s: env shard [%d, %d) outside [0, %d)", who, env_offset, env_offset + E,
+                     env_total);
+  if (S > 65535) return set_error(PQN_E_INVALID, "%s: S=%d exceeds gridDim.y", who, S);
+  PQN_ENV_DISPATCH(env_id, {
+    const int ms = max_steps > 0 ? max_steps : EnvT::DEFAULT_MAX_STEPS;
+    dim3 grid(blocks_for(E, ENV_BLOCK), (unsigned)S);
+    { LaunchScope _ls(K_ROLLOUT_ACT_STEP, (cudaStream_t)stream); rollout_act_step_kernel<EnvT><<<grid, ENV_BLOCK, 0, (cudaStream_t)stream>>>(
+        step_keys, q, eps, eps_stride, state, obs_next, action, reward, done, maxq, info_sums, E, ms, rew_scale, rng_mode,
+        obs_seed_stride, tr_seed_stride, info_done_only, env_total, env_offset); }
+  });
+  return check_launch(who);
+}
+
+static int qlambda(const float* reward, const uint8_t* done, const float* maxq, const float* q_last, float* targets,
+                   int32_t T, int32_t S, int32_t E, int32_t A, SeedScalar gamma, SeedScalar lambda, void* stream,
+                   const char* who) {
+  if (!reward || !done || !maxq || !q_last || !targets || T <= 0 || S <= 0 || E <= 0 || A <= 0)
+    return set_error(PQN_E_INVALID, "%s: bad argument", who);
+  { LaunchScope _ls(K_QLAMBDA, (cudaStream_t)stream); qlambda_kernel<<<blocks_for((int64_t)S * E, 256), 256, 0, (cudaStream_t)stream>>>(reward, done, maxq, q_last,
+                                                                                    targets, T, S, E, A, gamma, lambda); }
+  return check_launch(who);
+}
 
 }  // namespace pqn
 
@@ -521,21 +554,20 @@ int pqn_rollout_act_step(int env_id, const uint32_t* step_keys, const float* q, 
                          float* maxq, int64_t tr_seed_stride, double* info_sums, int info_done_only, int32_t S,
                          int32_t E, int32_t env_total, int32_t env_offset, int max_steps, float rew_scale, int rng_mode,
                          void* stream) {
-  if (!step_keys || !q || !eps || !state || !obs_next || !action || !reward || !done || !maxq || S <= 0 || E <= 0)
-    return set_error(PQN_E_INVALID, "pqn_rollout_act_step: bad argument");
-  if (env_total <= 0) { env_total = E; env_offset = 0; }
-  if (env_offset < 0 || env_offset + E > env_total)
-    return set_error(PQN_E_INVALID, "pqn_rollout_act_step: env shard [%d, %d) outside [0, %d)", env_offset,
-                     env_offset + E, env_total);
-  if (S > 65535) return set_error(PQN_E_INVALID, "pqn_rollout_act_step: S=%d exceeds gridDim.y", S);
-  PQN_ENV_DISPATCH(env_id, {
-    const int ms = max_steps > 0 ? max_steps : EnvT::DEFAULT_MAX_STEPS;
-    dim3 grid(blocks_for(E, ENV_BLOCK), (unsigned)S);
-    { LaunchScope _ls(K_ROLLOUT_ACT_STEP, (cudaStream_t)stream); rollout_act_step_kernel<EnvT><<<grid, ENV_BLOCK, 0, (cudaStream_t)stream>>>(
-        step_keys, q, eps, state, obs_next, action, reward, done, maxq, info_sums, E, ms, rew_scale, rng_mode,
-        obs_seed_stride, tr_seed_stride, info_done_only, env_total, env_offset); }
-  });
-  return check_launch("pqn_rollout_act_step");
+  return rollout_act_step(env_id, step_keys, q, eps, 0, state, obs_next, obs_seed_stride, action, reward, done, maxq,
+                          tr_seed_stride, info_sums, info_done_only, S, E, env_total, env_offset, max_steps,
+                          SeedScalar{nullptr, rew_scale}, rng_mode, stream, "pqn_rollout_act_step");
+}
+
+int pqn_rollout_act_step_seeds(int env_id, const uint32_t* step_keys, const float* q, const float* eps,
+                               uint32_t* state, void* obs_next, int64_t obs_seed_stride, int32_t* action, float* reward,
+                               uint8_t* done, float* maxq, int64_t tr_seed_stride, double* info_sums, int info_done_only,
+                               int32_t S, int32_t E, int32_t env_total, int32_t env_offset, int max_steps,
+                               const float* rew_scale, int rng_mode, void* stream) {
+  if (!rew_scale) return set_error(PQN_E_INVALID, "pqn_rollout_act_step_seeds: rew_scale is NULL");
+  return rollout_act_step(env_id, step_keys, q, eps, 1, state, obs_next, obs_seed_stride, action, reward, done, maxq,
+                          tr_seed_stride, info_sums, info_done_only, S, E, env_total, env_offset, max_steps,
+                          SeedScalar{rew_scale, 0.f}, rng_mode, stream, "pqn_rollout_act_step_seeds");
 }
 
 int pqn_rollout_keys(uint32_t* rng_inout, uint32_t* keys_out, int32_t S, int32_t T, int rng_mode, void* stream) {
@@ -546,11 +578,15 @@ int pqn_rollout_keys(uint32_t* rng_inout, uint32_t* keys_out, int32_t S, int32_t
 
 int pqn_qlambda(const float* reward, const uint8_t* done, const float* maxq, const float* q_last, float* targets,
                 int32_t T, int32_t S, int32_t E, int32_t A, float gamma, float lambda, void* stream) {
-  if (!reward || !done || !maxq || !q_last || !targets || T <= 0 || S <= 0 || E <= 0 || A <= 0)
-    return set_error(PQN_E_INVALID, "pqn_qlambda: bad argument");
-  { LaunchScope _ls(K_QLAMBDA, (cudaStream_t)stream); qlambda_kernel<<<blocks_for((int64_t)S * E, 256), 256, 0, (cudaStream_t)stream>>>(reward, done, maxq, q_last,
-                                                                                    targets, T, S, E, A, gamma, lambda); }
-  return check_launch("pqn_qlambda");
+  return qlambda(reward, done, maxq, q_last, targets, T, S, E, A, SeedScalar{nullptr, gamma}, SeedScalar{nullptr, lambda},
+                 stream, "pqn_qlambda");
+}
+
+int pqn_qlambda_seeds(const float* reward, const uint8_t* done, const float* maxq, const float* q_last, float* targets,
+                      int32_t T, int32_t S, int32_t E, int32_t A, const float* gamma, const float* lambda, void* stream) {
+  if (!gamma || !lambda) return set_error(PQN_E_INVALID, "pqn_qlambda_seeds: gamma / lambda is NULL");
+  return qlambda(reward, done, maxq, q_last, targets, T, S, E, A, SeedScalar{gamma, 0.f}, SeedScalar{lambda, 0.f}, stream,
+                 "pqn_qlambda_seeds");
 }
 
 }  // extern "C"

@@ -2852,7 +2852,8 @@ static int rnn_step(const pqn_net_desc_t* d, const float* params, const float* b
 static int rnn_loss_grad(const pqn_net_desc_t* d, const float* params, float* batch_stats, const float* hs0,
                          const float* obs, const uint8_t* last_done, const int32_t* last_action, const int32_t* action,
                          const float* reward, const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum, int32_t S,
-                         int32_t T, int32_t B, float gamma, float lambda, void* workspace, void* stream, const char* who) {
+                         int32_t T, int32_t B, SeedScalar gamma, SeedScalar lambda, void* workspace, void* stream,
+                         const char* who) {
   int rc;
   if (!params || !hs0 || !obs || !last_done || !last_action || !action || !reward || !done || !grads || !loss_sum ||
       !qsa_sum || !workspace || S <= 0 || T < 2 || B <= 0 || B > 1024 || S > 65535)
@@ -2974,7 +2975,8 @@ int pqn_rnn_loss_grad(const pqn_net_desc_t* d, const float* params, const float*
   if (rc) return rc;
   if ((rc = rnn::check_rnn(d, "pqn_rnn_loss_grad"))) return rc;
   return rnn_loss_grad(d, params, nullptr, hs0, obs, last_done, last_action, action, reward, done, grads, loss_sum, qsa_sum,
-                       S, T, B, gamma, lambda, workspace, stream, "pqn_rnn_loss_grad");
+                       S, T, B, SeedScalar{nullptr, gamma}, SeedScalar{nullptr, lambda}, workspace, stream,
+                       "pqn_rnn_loss_grad");
 }
 
 int pqn_rnn_loss_grad_stats(const pqn_net_desc_t* d, const float* params, float* batch_stats, const float* hs0,
@@ -2985,7 +2987,22 @@ int pqn_rnn_loss_grad_stats(const pqn_net_desc_t* d, const float* params, float*
   if (rc) return rc;
   if ((rc = rnn::check_rnn_stats(d, batch_stats, "pqn_rnn_loss_grad_stats"))) return rc;
   return rnn_loss_grad(d, params, batch_stats, hs0, obs, last_done, last_action, action, reward, done, grads, loss_sum,
-                       qsa_sum, S, T, B, gamma, lambda, workspace, stream, "pqn_rnn_loss_grad_stats");
+                       qsa_sum, S, T, B, SeedScalar{nullptr, gamma}, SeedScalar{nullptr, lambda}, workspace, stream,
+                       "pqn_rnn_loss_grad_stats");
+}
+
+int pqn_rnn_loss_grad_seeds(const pqn_net_desc_t* d, const float* params, float* batch_stats, const float* hs0,
+                            const float* obs, const uint8_t* last_done, const int32_t* last_action, const int32_t* action,
+                            const float* reward, const uint8_t* done, float* grads, float* loss_sum, float* qsa_sum,
+                            int32_t S, int32_t T, int32_t B, const float* gamma, const float* lambda, void* workspace,
+                            void* stream) {
+  int rc = check_desc(d, "pqn_rnn_loss_grad_seeds");
+  if (rc) return rc;
+  if ((rc = rnn::check_rnn_stats(d, batch_stats, "pqn_rnn_loss_grad_seeds"))) return rc;
+  if (!gamma || !lambda) return set_error(PQN_E_INVALID, "pqn_rnn_loss_grad_seeds: gamma / lambda is NULL");
+  return rnn_loss_grad(d, params, batch_stats, hs0, obs, last_done, last_action, action, reward, done, grads, loss_sum,
+                       qsa_sum, S, T, B, SeedScalar{gamma, 0.f}, SeedScalar{lambda, 0.f}, workspace, stream,
+                       "pqn_rnn_loss_grad_seeds");
 }
 
 int pqn_set_conv_mma_path(int on) {

@@ -49,17 +49,19 @@ __global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ g
 
 __global__ void __launch_bounds__(256) radam_kernel(float* __restrict__ params, const float* __restrict__ grads,
                                                     float* __restrict__ mu, float* __restrict__ nu,
-                                                    const float* __restrict__ sched,
+                                                    const float* __restrict__ sched, int64_t sched_stride,
                                                     const int32_t* __restrict__ step_counter,
-                                                    const float* __restrict__ gn, int64_t P, float max_norm, float b1,
-                                                    float b2, float eps) {
+                                                    const float* __restrict__ gn, int64_t P, SeedScalar max_norm_s,
+                                                    float b1, float b2, float eps) {
   const int seed = blockIdx.y;
   const int64_t i4 = (int64_t)blockIdx.x * 256 + threadIdx.x;
   const int t = step_counter[0];
-  const float lr = __ldg(sched + 4 * t + 0);
-  const float bc1 = __ldg(sched + 4 * t + 1);
-  const float bc2 = __ldg(sched + 4 * t + 2);
-  const float rect = __ldg(sched + 4 * t + 3);
+  const float* __restrict__ row = sched + seed * sched_stride + 4 * t;   // this seed's table (stride 0: shared)
+  const float lr = __ldg(row + 0);
+  const float bc1 = __ldg(row + 1);
+  const float bc2 = __ldg(row + 2);
+  const float rect = __ldg(row + 3);
+  const float max_norm = max_norm_s.at(seed);
   // squared gradient norm = the NORM_BLOCKS (64) block partials of sqnorm_kernel, added in a FIXED order (xor-shuffle
   // tree inside each of the first two warps, then warp 0 + warp 1) and broadcast through shared memory: deterministic,
   // and one pass over the 64 partials per block instead of one per thread
@@ -169,21 +171,37 @@ __global__ void net_init_kernel(const uint32_t* __restrict__ keys, float* __rest
 
 using namespace pqn;
 
+static int radam_clip_step(float* params, const float* grads, float* mu, float* nu, const float* sched,
+                           int64_t sched_stride, int32_t* step_counter, float* gnorm_scratch, int32_t S, int64_t P,
+                           SeedScalar max_norm, float b1, float b2, float eps, void* stream, const char* who) {
+  if (!params || !grads || !mu || !nu || !sched || sched_stride < 0 || !step_counter || !gnorm_scratch || S <= 0 ||
+      P <= 0 || (P & 3) || S > 65535)
+    return set_error(PQN_E_INVALID, "%s: bad argument (P must be a multiple of 4)", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  { LaunchScope _ls(K_SQNORM, st); sqnorm_kernel<<<dim3(NORM_BLOCKS, S), 256, 0, st>>>(grads, P, gnorm_scratch); }
+  const unsigned nb = (unsigned)((P / 4 + 255) / 256);
+  { LaunchScope _ls(K_RADAM, st); radam_kernel<<<dim3(nb, S), 256, 0, st>>>(params, grads, mu, nu, sched, sched_stride,
+                                                                           step_counter, gnorm_scratch, P, max_norm, b1,
+                                                                           b2, eps); }
+  { LaunchScope _ls(K_ADVANCE, st); advance_kernel<<<1, 1, 0, st>>>(step_counter); }
+  return check_launch(who);
+}
+
 extern "C" {
 
 int pqn_radam_clip_step(float* params, const float* grads, float* mu, float* nu, const float* sched,
                         int32_t* step_counter, float* gnorm_scratch, int32_t S, int64_t P, float max_norm, float b1,
                         float b2, float eps, void* stream) {
-  if (!params || !grads || !mu || !nu || !sched || !step_counter || !gnorm_scratch || S <= 0 || P <= 0 || (P & 3) ||
-      S > 65535)
-    return set_error(PQN_E_INVALID, "pqn_radam_clip_step: bad argument (P must be a multiple of 4)");
-  cudaStream_t st = (cudaStream_t)stream;
-  { LaunchScope _ls(K_SQNORM, st); sqnorm_kernel<<<dim3(NORM_BLOCKS, S), 256, 0, st>>>(grads, P, gnorm_scratch); }
-  const unsigned nb = (unsigned)((P / 4 + 255) / 256);
-  { LaunchScope _ls(K_RADAM, st); radam_kernel<<<dim3(nb, S), 256, 0, st>>>(params, grads, mu, nu, sched, step_counter, gnorm_scratch, P, max_norm, b1,
-                                            b2, eps); }
-  { LaunchScope _ls(K_ADVANCE, st); advance_kernel<<<1, 1, 0, st>>>(step_counter); }
-  return check_launch("pqn_radam_clip_step");
+  return radam_clip_step(params, grads, mu, nu, sched, 0, step_counter, gnorm_scratch, S, P, SeedScalar{nullptr, max_norm},
+                         b1, b2, eps, stream, "pqn_radam_clip_step");
+}
+
+int pqn_radam_clip_step_seeds(float* params, const float* grads, float* mu, float* nu, const float* sched,
+                              int64_t sched_seed_stride, int32_t* step_counter, float* gnorm_scratch, int32_t S,
+                              int64_t P, const float* max_norm, float b1, float b2, float eps, void* stream) {
+  if (!max_norm) return set_error(PQN_E_INVALID, "pqn_radam_clip_step_seeds: max_norm is NULL");
+  return radam_clip_step(params, grads, mu, nu, sched, sched_seed_stride, step_counter, gnorm_scratch, S, P,
+                         SeedScalar{max_norm, 0.f}, b1, b2, eps, stream, "pqn_radam_clip_step_seeds");
 }
 
 int pqn_net_init(const pqn_net_desc_t* d, const uint32_t* keys, float* params, int32_t S, void* stream) {

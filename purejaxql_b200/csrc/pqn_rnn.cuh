@@ -179,10 +179,11 @@ __global__ void gru_transpose_kernel(const float* __restrict__ params, int64_t P
 //   part[S][2] = (loss, mean chosen q) of this minibatch, summed over the columns in thread order
 __global__ void rnn_targets_kernel(const float* __restrict__ q, const int32_t* __restrict__ action,
                                    const float* __restrict__ reward, const uint8_t* __restrict__ done, int T, int B, int A,
-                                   float gamma, float lam, float* __restrict__ dq, float* __restrict__ loss_sum,
-                                   float* __restrict__ qsa_sum) {
+                                   SeedScalar gamma_s, SeedScalar lam_s, float* __restrict__ dq,
+                                   float* __restrict__ loss_sum, float* __restrict__ qsa_sum) {
   extern __shared__ float red[];   // [2][32] warp sums (blockDim is a multiple of 32, so at least 64 floats)
   const int seed = blockIdx.x, b = threadIdx.x;
+  const float gamma = gamma_s.at(seed), lam = lam_s.at(seed);
   float l_acc = 0.f, q_acc = 0.f;
   const float inv = 1.0f / (float)((T - 1) * B);
   if (b < B) {

@@ -24,7 +24,7 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
-from . import _lib, envs, jaxrandom as jr
+from . import _lib, envs, jaxrandom as jr, sweep
 from .networks import NET_CNN, NET_MLP, NET_MLP_BITS, QNetworkSpec
 
 INFO_KEYS = ("returned_episode_returns", "returned_episode_lengths", "timestep", "returned_episode", "discount")
@@ -67,6 +67,44 @@ def radam_schedule_table(num_steps, lr_fn, b1=0.9, b2=0.999, threshold=5.0):
     return tab
 
 
+def seed_inputs(grid: "sweep.Grid", seed_lo: int, S: int, num_updates: int, updates_decay: int,
+                grad_steps_per_update: int, lr_linear_decay: bool) -> dict:
+    """The per-seed hyperparameter tables the device reads, for the S seeds [seed_lo, seed_lo + S) of a run (numpy
+    float32; a seed takes the values of its grid point, sweep.Grid):
+
+      eps        [max(NU,1)][S]  eps_scheduler(n_updates) (pqn_minatar.py:134-139)
+      sched      RAdam rows (lr_t, 1-b1^t, 1-b2^t, rect_t): [steps][4] shared by every seed when the grid has one point,
+                 else [S][steps][4], each seed its point's table (:140-147)
+      gamma, lam, max_norm, rew_scale  [S]
+    """
+    pt = grid.point_of(seed_lo, S)
+    nud, total_grad_steps = updates_decay, num_updates * grad_steps_per_update
+    eps_pts, sched_pts = [], []
+    for g in range(grid.G):
+        c = grid.config(g)
+        eps_pts.append([linear_schedule(c["EPS_START"], c["EPS_FINISH"], c["EPS_DECAY"] * nud, n)
+                        for n in range(max(num_updates, 1))])
+        if lr_linear_decay:
+            lr_fn = lambda i, lr=c["LR"]: linear_schedule(lr, 1e-20, nud * grad_steps_per_update, i)
+        else:
+            lr_fn = lambda i, lr=c["LR"]: _f32(lr)
+        sched_pts.append(radam_schedule_table(total_grad_steps, lr_fn))
+    eps = np.ascontiguousarray(np.asarray(eps_pts, np.float32).T[:, pt])
+    sched = sched_pts[0] if grid.G == 1 else np.stack([sched_pts[g] for g in pt])
+
+    def per_seed(key):
+        return np.array([grid.value(int(g), key) for g in pt], np.float32)
+    return dict(eps=eps, sched=sched, gamma=per_seed("GAMMA"), lam=per_seed("LAMBDA"),
+                max_norm=per_seed("MAX_GRAD_NORM"), rew_scale=per_seed("REW_SCALE"))
+
+
+def seed_tensors(inputs: dict, dev):
+    """seed_inputs on the device, and the RAdam schedule's per-seed stride in floats (0: one shared table)."""
+    t = {k: torch.from_numpy(v).to(dev) for k, v in inputs.items()}
+    sched = t["sched"]
+    return t, (0 if sched.dim() == 2 else sched.shape[1] * 4)
+
+
 class TrainState(SimpleNamespace):
     """Mirror of CustomTrainState (pqn_minatar.py:82-86): params / batch_stats
     nested dicts with a leading seed axis, plus timesteps, n_updates, grad_steps
@@ -95,6 +133,8 @@ def network_spec(env, network: str, c: dict):
 class PQNEngine:
     def __init__(self, config: dict, network: str, flatten_obs: bool, device=None):
         self.cfg = config
+        self.grid = sweep.Grid(config)       # per-seed hyperparameters: a grid of G points x NUM_SEEDS
+        self.seed_lo = 0            # global index of this run's first seed (a seed-sharded rank trains a slice)
         self.device = torch.device(device or "cuda")
         if self.device.type != "cuda" or not torch.cuda.is_available():
             raise _lib.PqnError("purejaxql_b200 needs a CUDA device: there is no CPU fallback")
@@ -113,9 +153,6 @@ class PQNEngine:
         self.nmb = int(c["NUM_MINIBATCHES"])
         self.epochs = int(c["NUM_EPOCHS"])
         self.mb = self.T * self.E // self.nmb
-        self.gamma = float(c["GAMMA"])
-        self.lam = float(c["LAMBDA"])
-        self.rew_scale = float(c.get("REW_SCALE", 1))
         self.test = bool(c.get("TEST_DURING_TRAINING", False))
         self._ws = None
 
@@ -167,16 +204,10 @@ class PQNEngine:
         spec, P = self.spec, self.spec.total
         W = self.row_words
 
-        # ---- schedules (pqn_minatar.py:134-147)
-        nud = c["NUM_UPDATES_DECAY"]
-        eps_table = torch.tensor([linear_schedule(c["EPS_START"], c["EPS_FINISH"], c["EPS_DECAY"] * nud, n)
-                                  for n in range(max(NU, 1))], dtype=torch.float32, device=dev)
-        total_grad_steps = NU * self.nmb * self.epochs
-        if c.get("LR_LINEAR_DECAY", False):
-            lr_fn = lambda i: linear_schedule(c["LR"], 1e-20, nud * self.nmb * self.epochs, i)
-        else:
-            lr_fn = lambda i: _f32(c["LR"])
-        sched = torch.from_numpy(radam_schedule_table(total_grad_steps, lr_fn)).to(dev)
+        # ---- schedules (pqn_minatar.py:134-147) and the other per-seed hyperparameters
+        hp, sched_stride = seed_tensors(seed_inputs(self.grid, self.seed_lo, S, NU, c["NUM_UPDATES_DECAY"],
+                                                    self.nmb * self.epochs, c.get("LR_LINEAR_DECAY", False)), dev)
+        eps_table, sched = hp["eps"], hp["sched"]
 
         # ---- key chain (SURVEY Appendix B; pqn_minatar.py:172-173,415-423)
         k = jr.split(keys, 2, mode)
@@ -209,7 +240,7 @@ class PQNEngine:
         loss_sum = torch.zeros(S, device=dev)
         qsa_sum = torch.zeros(S, device=dev)
         step_keys = torch.zeros((T, S, 2, 2), dtype=torch.int32, device=dev)
-        eps_dev = torch.zeros(1, device=dev)
+        eps_dev = torch.zeros((1, S), device=dev)                   # eps of every seed for this update
         # ---- reset (vmap_reset, :107-109,419)
         reset_keys = jr.split(kR, E_total, mode)[:, env_lo:env_lo + E].reshape(S * E, 2).contiguous()
         state = torch.empty((self.env.state_words, S * E), dtype=torch.int32, device=dev)
@@ -259,18 +290,19 @@ class PQNEngine:
             info_sums.zero_()
             for t in range(T):
                 self.forward(params, obs_buf[:, t], S, E, seed_stride_obs, q_buf)
-                _lib.check(L.pqn_rollout_act_step(
+                _lib.check(L.pqn_rollout_act_step_seeds(
                     self.env.env_id, _lib.p(step_keys[t]), _lib.p(q_buf), _lib.p(eps_dev), _lib.p(state),
                     _lib.raw(obs_buf[:, t + 1]), seed_stride_obs,
                     _lib.raw(act_buf[:, t]), _lib.raw(rew_buf[:, t]),
                     _lib.raw(done_buf[:, t]), _lib.raw(maxq_buf[:, t]),
-                    seed_stride_tr, _lib.p(info_sums), 0, S, E, E_total, env_lo, self.max_steps, self.rew_scale, mode,
-                    sp()), "pqn_rollout_act_step")
+                    seed_stride_tr, _lib.p(info_sums), 0, S, E, E_total, env_lo, self.max_steps, _lib.p(hp["rew_scale"]),
+                    mode, sp()), "pqn_rollout_act_step_seeds")
             r = carry                                                # scan's final carry (:214)
             # ================= bootstrap + Q(lambda) (:227-260)
             self.forward(params, obs_buf[:, T], S, E, seed_stride_obs, q_buf)
-            _lib.check(L.pqn_qlambda(_lib.p(rew_buf), _lib.p(done_buf), _lib.p(maxq_buf), _lib.p(q_buf),
-                                     _lib.p(targets), T, S, E, A, self.gamma, self.lam, sp()), "pqn_qlambda")
+            _lib.check(L.pqn_qlambda_seeds(_lib.p(rew_buf), _lib.p(done_buf), _lib.p(maxq_buf), _lib.p(q_buf),
+                                           _lib.p(targets), T, S, E, A, _lib.p(hp["gamma"]), _lib.p(hp["lam"]), sp()),
+                       "pqn_qlambda_seeds")
             # ================= NETWORKS UPDATE (:263-327)
             r = jr.split(r, 2, mode)[:, 0].contiguous()              # :324
             loss_sum.zero_()
@@ -290,10 +322,10 @@ class PQNEngine:
                         _lib.p(qsa_sum), _lib.p(bn_sums), S, mb, _lib.p(ws), sp()), "pqn_qnet_loss_grad")
                     allreduce_(grads, True)                          # the ONE collective of the data path
                     allreduce_(bn_sums, False)
-                    _lib.check(L.pqn_radam_clip_step(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu),
-                                                     _lib.p(sched), _lib.p(step_counter), _lib.p(gnorm), S, P,
-                                                     float(c["MAX_GRAD_NORM"]), 0.9, 0.999, 1e-8, sp()),
-                               "pqn_radam_clip_step")
+                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu),
+                                                           _lib.p(sched), sched_stride, _lib.p(step_counter),
+                                                           _lib.p(gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
+                                                           1e-8, sp()), "pqn_radam_clip_step_seeds")
                     _lib.check(L.pqn_bn_stats_update(_lib.p(batch_stats), _lib.p(bn_sums), S, F, spec.stats_total,
                                                      bn_count, 0.99, sp()), "pqn_bn_stats_update")
             if self.test:                                            # :341  rng, _rng = split(rng)
@@ -387,7 +419,8 @@ class PQNEngine:
             timesteps=torch.full((S,), timesteps, dtype=torch.int64), n_updates=torch.full((S,), NU),
             grad_steps=torch.full((S,), grad_steps))
         expl_state = (self._final_obs(obs_buf, S), state)
-        return {"runner_state": (train_state, expl_state, test_metrics, rng), "metrics": out_metrics}
+        return {"runner_state": (train_state, expl_state, test_metrics, rng), "metrics": out_metrics,
+                "sweep": self.grid.table(self.seed_lo, S)}
 
     # ------------------------------------------------------------------ #
     def _write_obs(self, state, obs_buf, t, S):

@@ -2,10 +2,11 @@
 purejaxql/pqn_rnn_gymnax.py:117-560 with the seed axis taken natively.
 
 All compute is libpqn_b200 kernels: ``pqn_rnn_step`` (one step of the recurrent Q-network for the rollout, the memory
-warm-up and the evaluation), ``pqn_rollout_act_step`` (eps-greedy + env step + LogWrapper, shared with the feed-forward
-engine), ``pqn_rnn_loss_grad`` (window forward, in-loss Q(lambda) targets, BPTT) and ``pqn_radam_clip_step``.  The
-NORM_TYPE / NORM_INPUT variants other than (layer_norm, False) call ``pqn_rnn_step_stats`` / ``pqn_rnn_loss_grad_stats``
-with a static ``batch_stats`` buffer: the loss updates the running statistics in place (:362-369), the steps read them
+warm-up and the evaluation), ``pqn_rollout_act_step_seeds`` (eps-greedy + env step + LogWrapper, shared with the
+feed-forward engine), ``pqn_rnn_loss_grad_seeds`` (window forward, in-loss Q(lambda) targets, BPTT) and
+``pqn_radam_clip_step_seeds``; the ``_seeds`` entries read eps, the reward scale, gamma, lambda, the clipping norm and
+the RAdam schedule per seed (a hyperparameter grid, sweep.py).  The NORM_TYPE / NORM_INPUT variants other than
+(layer_norm, False) call ``pqn_rnn_step_stats`` and pass a static ``batch_stats`` buffer to the loss: the loss updates the running statistics in place (:362-369), the steps read them
 (train=False), so the update stays capturable in a CUDA graph.  This
 module owns the buffers, walks the reference's PRNG key chain — including its re-bindings of ``rng`` to the final
 carry of the rollout scans (:222-228, :531-537) — and keeps the memory of the last MEMORY_WINDOW + NUM_STEPS
@@ -20,14 +21,16 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
-from . import _lib, envs, jaxrandom as jr
-from .engine import INFO_KEYS, TrainState, linear_schedule, radam_schedule_table, _f32
+from . import _lib, envs, jaxrandom as jr, sweep
+from .engine import INFO_KEYS, TrainState, seed_inputs, seed_tensors
 from .networks import NET_RNN, QNetworkSpec
 
 
 class PQNRnnEngine:
     def __init__(self, config: dict, device=None, env_params: envs.EnvParams | None = None):
         self.cfg = c = config
+        self.grid = sweep.Grid(config)       # per-seed hyperparameters: a grid of G points x NUM_SEEDS
+        self.seed_lo = 0            # global index of this run's first seed (a seed-sharded rank trains a slice)
         self.device = torch.device(device or "cuda")
         self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
         self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=True, rng_mode=self.rng_mode)
@@ -52,8 +55,6 @@ class PQNRnnEngine:
         self.nmb, self.epochs = int(c["NUM_MINIBATCHES"]), int(c["NUM_EPOCHS"])
         assert self.E % self.nmb == 0, "NUM_MINIBATCHES must divide NUM_ENVS (minibatches are whole env trajectories)"
         self.Bm = self.E // self.nmb
-        self.gamma, self.lam = float(c["GAMMA"]), float(c["LAMBDA"])
-        self.rew_scale = float(c.get("REW_SCALE", 1))
         self.test = bool(c.get("TEST_DURING_TRAINING", False))
         self._ws = None
 
@@ -77,11 +78,13 @@ class PQNRnnEngine:
                                       _lib.p(last_action), _lib.p(q), S, N, _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_step")
 
     def _act_step(self, S, N, step_keys, q, eps, state, obs_next, action, reward, done, maxq, sums, done_only, rew_scale):
+        """eps and rew_scale: float32[S] device values of each seed."""
         L = _lib.lib()
-        _lib.check(L.pqn_rollout_act_step(self.env.env_id, _lib.p(step_keys), _lib.p(q), _lib.p(eps), _lib.p(state),
-                                          _lib.p(obs_next), N, _lib.p(action), _lib.p(reward), _lib.p(done), _lib.p(maxq), N,
-                                          _lib.p(sums), done_only, S, N, 0, 0, self.max_steps, rew_scale, self.rng_mode,
-                                          _lib.stream_ptr()), "pqn_rollout_act_step")
+        _lib.check(L.pqn_rollout_act_step_seeds(self.env.env_id, _lib.p(step_keys), _lib.p(q), _lib.p(eps),
+                                                _lib.p(state), _lib.p(obs_next), N, _lib.p(action), _lib.p(reward),
+                                                _lib.p(done), _lib.p(maxq), N, _lib.p(sums), done_only, S, N, 0, 0,
+                                                self.max_steps, _lib.p(rew_scale), self.rng_mode, _lib.stream_ptr()),
+                   "pqn_rollout_act_step_seeds")
 
     def _reset(self, key, S, N):
         """vmap_reset(N)(key): obs [S,N,D], state."""
@@ -100,15 +103,9 @@ class PQNRnnEngine:
         keys = jr.as_key_tensor(rngs, dev)
         S = keys.shape[0]
         spec, P = self.spec, self.spec.total
-        nud = c["NUM_UPDATES_DECAY"]
-        eps_table = torch.tensor([linear_schedule(c["EPS_START"], c["EPS_FINISH"], c["EPS_DECAY"] * nud, n)
-                                  for n in range(max(NU, 1))], dtype=torch.float32, device=dev)
-        total_grad_steps = NU * self.nmb * self.epochs
-        if c.get("LR_LINEAR_DECAY", False):
-            lr_fn = lambda i: linear_schedule(c["LR"], 1e-20, nud * self.nmb * self.epochs, i)
-        else:
-            lr_fn = lambda i: _f32(c["LR"])
-        sched = torch.from_numpy(radam_schedule_table(total_grad_steps, lr_fn)).to(dev)
+        hp, sched_stride = seed_tensors(seed_inputs(self.grid, self.seed_lo, S, NU, c["NUM_UPDATES_DECAY"],
+                                                    self.nmb * self.epochs, c.get("LR_LINEAR_DECAY", False)), dev)
+        eps_table, sched = hp["eps"], hp["sched"]                   # [NU][S], RAdam rows (sweep layout)
 
         # ---- key chain (:255-256, :505-543)
         k = jr.split(keys, 2, mode)
@@ -138,8 +135,8 @@ class PQNRnnEngine:
         maxq = torch.zeros((S, E), device=dev)
         info_sums = torch.zeros((S, 5), dtype=torch.float64, device=dev)
         new_obs = torch.empty_like(last_obs)
-        eps_one = torch.ones(1, device=dev)
-        eps_dev = torch.zeros(1, device=dev)
+        eps_one = torch.ones(S, device=dev)                          # random actions of the memory warm-up
+        eps_dev = torch.zeros((1, S), device=dev)                    # eps of every seed for this update
 
         act_t = torch.empty((S, E), dtype=torch.int32, device=dev)
         rew_t = torch.empty((S, E), device=dev)
@@ -159,7 +156,7 @@ class PQNRnnEngine:
                 mem.last_done[:, s].copy_(last_done); mem.last_action[:, s].copy_(last_action)
                 self.step(params, hs, last_obs, last_done, last_action, q, S, E)
                 self._act_step(S, E, step_keys[t], q, eps, state, new_obs, act_t, rew_t, done_t, maxq, info_sums, 0,
-                               self.rew_scale)
+                               hp["rew_scale"])
                 mem.action[:, s].copy_(act_t); mem.reward[:, s].copy_(rew_t); mem.done[:, s].copy_(done_t)
                 last_obs.copy_(new_obs)
                 last_done.copy_(done_t); last_action.copy_(act_t)
@@ -214,20 +211,16 @@ class PQNRnnEngine:
                     obs_mb = mem.obs.gather(2, i3[..., None].expand(S, Tm, Bm, D)).contiguous()
                     hs0 = mem.hs[:, 0].gather(1, idx[:, :, None].expand(S, Bm, H)).contiguous()
                     ld, la, ac, rw, dn = g3(mem.last_done), g3(mem.last_action), g3(mem.action), g3(mem.reward), g3(mem.done)
-                    if self.with_stats:                              # batch_stats = updates["batch_stats"] (:362-369)
-                        _lib.check(L.pqn_rnn_loss_grad_stats(
-                            spec.desc, _lib.p(params), _lib.p(self.batch_stats), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
-                            _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads), _lib.p(loss_sum),
-                            _lib.p(qsa_sum), S, Tm, Bm, self.gamma, self.lam, _lib.p(ws), _lib.stream_ptr()),
-                            "pqn_rnn_loss_grad_stats")
-                    else:
-                        _lib.check(L.pqn_rnn_loss_grad(spec.desc, _lib.p(params), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
-                                                       _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads),
-                                                       _lib.p(loss_sum), _lib.p(qsa_sum), S, Tm, Bm, self.gamma, self.lam,
-                                                       _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_loss_grad")
-                    _lib.check(L.pqn_radam_clip_step(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu), _lib.p(sched),
-                                                     _lib.p(step_counter), _lib.p(gnorm), S, P, float(c["MAX_GRAD_NORM"]),
-                                                     0.9, 0.999, 1e-8, _lib.stream_ptr()), "pqn_radam_clip_step")
+                    # batch_stats = updates["batch_stats"] (:362-369); None for the default network
+                    _lib.check(L.pqn_rnn_loss_grad_seeds(
+                        spec.desc, _lib.p(params), _lib.p(self.batch_stats), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
+                        _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads), _lib.p(loss_sum),
+                        _lib.p(qsa_sum), S, Tm, Bm, _lib.p(hp["gamma"]), _lib.p(hp["lam"]), _lib.p(ws),
+                        _lib.stream_ptr()), "pqn_rnn_loss_grad_seeds")
+                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu),
+                                                           _lib.p(sched), sched_stride, _lib.p(step_counter),
+                                                           _lib.p(gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
+                                                           1e-8, _lib.stream_ptr()), "pqn_radam_clip_step_seeds")
             if self.test:                                            # :398  rng, _rng = split(rng)
                 k = jr.split(r, 2, mode)
                 r = k[:, 0].contiguous()
@@ -293,7 +286,8 @@ class PQNRnnEngine:
             timesteps=torch.full((S,), timesteps, dtype=torch.int64), n_updates=torch.full((S,), NU),
             grad_steps=torch.full((S,), grad_steps))
         expl_state = (hs, last_obs, last_done, last_action, state)
-        return {"runner_state": (train_state, mem, expl_state, test_metrics, rng), "metrics": out_metrics}
+        return {"runner_state": (train_state, mem, expl_state, test_metrics, rng), "metrics": out_metrics,
+                "sweep": self.grid.table(self.seed_lo, S)}
 
     # ------------------------------------------------------------------ #
     def get_test_metrics(self, params, rng):
@@ -313,13 +307,14 @@ class PQNRnnEngine:
         act = torch.zeros((S, N), dtype=torch.int32, device=dev)
         dn = torch.zeros((S, N), dtype=torch.uint8, device=dev)
         sums = torch.zeros((S, 5), dtype=torch.float64, device=dev)
-        eps = torch.full((1,), float(c["EPS_TEST"]), device=dev)
+        eps = torch.full((S,), float(c["EPS_TEST"]), device=dev)
+        ones = torch.ones(S, device=dev)                             # the evaluation's rewards are not scaled
         step_keys = torch.zeros((steps, S, 2, 2), dtype=torch.int32, device=dev)
         carry = kr.clone()
         _lib.check(L.pqn_rollout_keys(_lib.p(carry), _lib.p(step_keys), S, steps, mode, _lib.stream_ptr()), "pqn_rollout_keys")
         for t in range(steps):
             self.step(params, hs, obs, ld, la, q, S, N)
-            self._act_step(S, N, step_keys[t], q, eps, state, nxt, act, rw, dn, mq, sums, 1, 1.0)
+            self._act_step(S, N, step_keys[t], q, eps, state, nxt, act, rw, dn, mq, sums, 1, ones)
             obs, nxt = nxt, obs
             ld.copy_(dn); la.copy_(act)
         cnt = sums[:, 3]

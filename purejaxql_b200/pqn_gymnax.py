@@ -25,11 +25,12 @@ from the config, and there is REW_SCALE.
 """
 from __future__ import annotations
 
-from . import _runner, envs
+from . import _runner, envs, sweep
 from .engine import PQNEngine, prepare_config
 
 
 def make_train(config):
+    sweep.Grid(config)                       # refuses lists it cannot train before anything is built
     env, env_params = envs.make(config["ENV_NAME"], flatten_obs=True)      # :92-94
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=True)    # :80-97
     engine = PQNEngine(config, network="mlp", flatten_obs=True)

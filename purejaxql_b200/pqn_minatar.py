@@ -12,11 +12,12 @@ test_metrics, rng), "metrics": {name: [S, NUM_UPDATES]}}``.
 """
 from __future__ import annotations
 
-from . import _runner, envs
+from . import _runner, envs, sweep
 from .engine import PQNEngine, prepare_config
 
 
 def make_train(config):
+    sweep.Grid(config)                       # refuses lists it cannot train before anything is built
     env, env_params = envs.make(config["ENV_NAME"])                  # :103-104
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=False)   # :91-105
     engine = PQNEngine(config, network="cnn", flatten_obs=False)

@@ -22,12 +22,13 @@ scripts ``train(rngs)`` takes the ``[NUM_SEEDS, 2]`` key array natively.
 """
 from __future__ import annotations
 
-from . import _runner, envs
+from . import _runner, envs, sweep
 from .engine import prepare_config
 from .engine_rnn import PQNRnnEngine
 
 
 def make_train(config):
+    sweep.Grid(config)                       # refuses lists it cannot train before anything is built
     env, env_params = envs.make(config["ENV_NAME"], flatten_obs=True)      # :134-139
     if config["ENV_NAME"] == "MemoryChain-bsuite":
         # :134-136 -- EnvParams(memory_length=ENV_KWARGS.get("memory_length", 10)): the script's default is 10, not
