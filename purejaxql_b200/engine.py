@@ -18,7 +18,6 @@ Appendix B) and sequences the launches:
 """
 from __future__ import annotations
 
-import time
 from types import SimpleNamespace
 
 import numpy as np
@@ -130,44 +129,205 @@ def network_spec(env, network: str, c: dict):
     return spec, env.obs_dim, torch.float32
 
 
-class PQNEngine:
-    def __init__(self, config: dict, network: str, flatten_obs: bool, device=None):
-        self.cfg = config
+class EngineBase:
+    """What the feed-forward and the recurrent engine share: the config, the per-seed hyperparameter tables, the
+    optimiser and update-step buffers, the fused act step, the update loop (eager, then a captured CUDA graph), the
+    metrics, the evaluation means and the assembly of train()'s result.  A subclass owns its network, its key chain
+    and its ``update_body``."""
+
+    def __init__(self, config: dict, flatten_obs: bool, device=None, env_params: envs.EnvParams | None = None):
+        self.cfg = c = config
         self.grid = sweep.Grid(config)       # per-seed hyperparameters: a grid of G points x NUM_SEEDS
         self.seed_lo = 0            # global index of this run's first seed (a seed-sharded rank trains a slice)
+        self.env_shard = None       # (rank, world): train envs [rank*E/world, (rank+1)*E/world) of every seed
         self.device = torch.device(device or "cuda")
         if self.device.type != "cuda" or not torch.cuda.is_available():
             raise _lib.PqnError("purejaxql_b200 needs a CUDA device: there is no CPU fallback")
-        _lib.lib()
-        c = config
         self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
         self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=flatten_obs, rng_mode=self.rng_mode)
+        if env_params is not None:                                   # e.g. MemoryChain's memory_length
+            self.env_params = env_params
         self.max_steps = int(self.env_params.max_steps_in_episode)
-        self.T = int(c["NUM_STEPS"])
-        self.E = int(c["NUM_ENVS"])
-        self.NU = int(c["NUM_UPDATES"])
+        self.T, self.E, self.NU = int(c["NUM_STEPS"]), int(c["NUM_ENVS"]), int(c["NUM_UPDATES"])
         self.A = self.env.num_actions
-        self.binary = self.env.binary_obs
-        self.network = network
-        self.spec, self.row_words, self.obs_dtype = network_spec(self.env, network, c)
-        self.nmb = int(c["NUM_MINIBATCHES"])
-        self.epochs = int(c["NUM_EPOCHS"])
-        self.mb = self.T * self.E // self.nmb
+        self.nmb, self.epochs = int(c["NUM_MINIBATCHES"]), int(c["NUM_EPOCHS"])
         self.test = bool(c.get("TEST_DURING_TRAINING", False))
+        self.batch_stats = None     # [S][stats_total] running statistics; train() sets them
+        # hooks (bench / tests), called on the host outside the captured region so they do not prevent graph replay:
+        # on_update_begin(n) before update n, on_update_end(n, payload) with the engine's static buffers after it
+        self.on_update_begin = None
+        self.on_update_end = None
+        self.graph_captured = False
+        self.graph_replays = 0
+        self.graph_launches_per_replay = 0
         self._ws = None
 
-    # ------------------------------------------------------------------ #
     def _workspace(self, S, rows):
         need = int(_lib.lib().pqn_net_workspace_bytes(self.spec.desc, S, rows))
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         return self._ws
 
+    def _seed_tables(self, S):
+        """seed_tensors of this run's S seeds: ({eps, sched, gamma, lam, max_norm, rew_scale}, sched stride)."""
+        c = self.cfg
+        return seed_tensors(seed_inputs(self.grid, self.seed_lo, S, self.NU, c["NUM_UPDATES_DECAY"],
+                                        self.nmb * self.epochs, c.get("LR_LINEAR_DECAY", False)), self.device)
+
+    def _update_buffers(self, params, rng):
+        """The optimiser state and the static buffers every update reads and writes (so that it can be replayed
+        from a CUDA graph): the runner key, the evaluation key and the update index on the device, and the sums
+        the metrics are taken from."""
+        S, dev = rng.shape[0], self.device
+        return SimpleNamespace(
+            mu=torch.zeros_like(params), nu=torch.zeros_like(params), grads=torch.zeros_like(params),
+            step_counter=torch.zeros(1, dtype=torch.int32, device=dev),
+            gnorm=torch.zeros(S * 64, device=dev),                   # block partials of the squared gradient norm
+            rng=rng.clone(),                                          # runner rng, updated in place
+            kT=torch.zeros((S, 2), dtype=torch.int32, device=dev),    # eval key of this update
+            idx=torch.zeros(1, dtype=torch.int64, device=dev),        # n_updates on the device
+            m=torch.zeros((S, 7), dtype=torch.float64, device=dev),   # td_loss, qvals, 5 info means
+            loss_sum=torch.zeros(S, device=dev), qsa_sum=torch.zeros(S, device=dev))
+
+    def _end_update(self, u, r, info_sums):
+        """The end of every update body: the evaluation key (rng, _rng = split(rng)), the runner key and the
+        update's means."""
+        if self.test:
+            k = jr.split(r, 2, self.rng_mode)
+            r = k[:, 0].contiguous()
+            u.kT.copy_(k[:, 1])
+        u.rng.copy_(r)
+        denom = float(self.epochs * self.nmb)
+        u.m[:, 0] = u.loss_sum.double() / denom
+        u.m[:, 1] = u.qsa_sum.double() / denom
+        u.m[:, 2:7] = info_sums / float(self.T * self.E)
+        u.idx.add_(1)
+
+    def _act_step(self, S, N, step_keys, q, eps, state, obs_next, action, reward, done, maxq, sums, done_only,
+                  rew_scale, obs_stride, tr_stride, env_total, env_offset):
+        """Fused eps-greedy + env step + stores (pqn_rollout_act_step_seeds) for S seeds x N envs.  eps and
+        rew_scale are float32[S] device values of each seed; obs_next and the transition buffers may be strided
+        views (obs_stride / tr_stride rows per seed); the N envs are [env_offset, env_offset + N) of env_total."""
+        _lib.check(_lib.lib().pqn_rollout_act_step_seeds(
+            self.env.env_id, _lib.p(step_keys), _lib.p(q), _lib.p(eps), _lib.p(state), _lib.raw(obs_next), obs_stride,
+            _lib.raw(action), _lib.raw(reward), _lib.raw(done), _lib.raw(maxq), tr_stride, _lib.p(sums), done_only,
+            S, N, env_total, env_offset, self.max_steps, _lib.p(rew_scale), self.rng_mode, _lib.stream_ptr()),
+            "pqn_rollout_act_step_seeds")
+
+    @staticmethod
+    def _episode_means(sums):
+        """INFO_KEYS means over the episodes that ended (sums[:, 3] of them); NaN where none did."""
+        cnt = sums[:, 3]
+        return {kk: torch.where(cnt > 0, sums[:, j] / cnt.clamp(min=1), torch.full_like(cnt, float("nan")))
+                for j, kk in enumerate(INFO_KEYS)}
+
+    def _run_updates(self, keys, params, u, update_body, payload, graph_auto, test_metrics, frame_channels=None):
+        """NUM_UPDATES x update_body, with the metrics (pqn_minatar.py:329-338), the evaluation (:340-350) and the
+        wandb log (:353-365) of every update.  The first update runs eagerly (it warms every code path); when
+        CUDA_GRAPH is true, or "auto" and graph_auto holds, later updates replay a graph captured after it.
+        Returns (metrics, test_hist, test_metrics): [S, NU] float64 columns and the last evaluation."""
+        c, dev, L, NU = self.cfg, self.device, _lib.lib(), self.NU
+        S = keys.shape[0]
+        # pqn_minatar.py:330-338 reports env_frame; pqn_gymnax.py:324-331 and pqn_rnn_gymnax.py:401-408 do not
+        metric_names = ["env_step", "update_steps", *(["env_frame"] if frame_channels else []), "grad_steps",
+                        "td_loss", "qvals", *INFO_KEYS]
+        metrics = {m: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for m in metric_names}
+        test_hist = None
+        if self.test:
+            test_every = int(NU * c["TEST_INTERVAL"])
+            test_hist = {kk: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for kk in INFO_KEYS}
+        want_graph = c.get("CUDA_GRAPH", "auto")
+        use_graph = (graph_auto if want_graph == "auto" else bool(want_graph)) and NU > 2
+        graph = None
+        self.graph_captured = False
+        self.graph_replays = 0
+        self.graph_launches_per_replay = 0
+        for col in range(NU):
+            if self.on_update_begin is not None:
+                self.on_update_begin(col)
+            if graph is not None:
+                graph.replay()
+                self.graph_replays += 1
+            else:
+                update_body()
+                if use_graph and col == 0:
+                    try:
+                        torch.cuda.synchronize(dev)
+                        g = torch.cuda.CUDAGraph()
+                        l0 = L.pqn_launch_count()
+                        with torch.cuda.graph(g):
+                            update_body()
+                        self.graph_launches_per_replay = int(L.pqn_launch_count() - l0)
+                        graph = g
+                        self.graph_captured = True
+                    except Exception as e:                            # capture is an optimisation only
+                        import warnings
+                        warnings.warn(f"CUDA graph capture of the update step failed ({e!r}); running eagerly")
+                        graph = None
+                        use_graph = False
+                        torch.cuda.synchronize(dev)
+            n_done = col + 1
+            timesteps = n_done * self.T * self.E                      # :222-225
+            metrics["env_step"][:, col] = timesteps
+            metrics["update_steps"][:, col] = n_done
+            if frame_channels:
+                metrics["env_frame"][:, col] = timesteps * frame_channels
+            metrics["grad_steps"][:, col] = n_done * self.nmb * self.epochs
+            metrics["td_loss"][:, col] = u.m[:, 0]
+            metrics["qvals"][:, col] = u.m[:, 1]
+            for j, kk in enumerate(INFO_KEYS):
+                metrics[kk][:, col] = u.m[:, 2 + j]
+            if self.on_update_end is not None:
+                self.on_update_end(col, payload)
+            if self.test:
+                if test_every > 0 and n_done % test_every == 0:
+                    test_metrics = self.get_test_metrics(params, u.kT.clone())
+                for kk in INFO_KEYS:
+                    test_hist[kk][:, col] = test_metrics[kk]
+            if c.get("WANDB_MODE", "disabled") != "disabled":
+                self._wandb_log(metrics, test_hist, col, jr.to_numpy_u32(keys)[:, 0])
+        torch.cuda.synchronize(dev)
+        return metrics, test_hist, test_metrics
+
+    def _wandb_log(self, metrics, test_hist, col, seed_labels):
+        import wandb
+        S = metrics["td_loss"].shape[0]
+        row = {m: v[:, col].mean().item() for m, v in metrics.items()}
+        if test_hist is not None:
+            row.update({f"test/{kk}": v[:, col].nanmean().item() for kk, v in test_hist.items()})
+        if self.cfg.get("WANDB_LOG_ALL_SEEDS", False):
+            for s in range(S):
+                for m, v in metrics.items():
+                    row[f"rng{int(seed_labels[s])}/{m}"] = v[s, col].item()
+        wandb.log(row, step=int(row["update_steps"]))
+
+    def _result(self, params, batch_stats, u, metrics, test_hist, runner_tail):
+        """train()'s result: {"runner_state": (TrainState, *runner_tail), "metrics", "sweep"}."""
+        NU, spec, S = self.NU, self.spec, params.shape[0]
+        out_metrics = {m: v[:, :NU].float() if m in ("td_loss", "qvals", *INFO_KEYS) else v[:, :NU].to(torch.int64)
+                       for m, v in metrics.items()}
+        if test_hist is not None:
+            out_metrics.update({f"test/{kk}": v[:, :NU].float() for kk, v in test_hist.items()})
+        timesteps, grad_steps = NU * self.T * self.E, NU * self.nmb * self.epochs
+        train_state = TrainState(
+            params=spec.unflatten(params), params_flat=params,
+            batch_stats=spec.unflatten_stats(batch_stats), batch_stats_flat=batch_stats,
+            opt_state=SimpleNamespace(mu=u.mu, nu=u.nu, count=grad_steps),
+            timesteps=torch.full((S,), timesteps, dtype=torch.int64), n_updates=torch.full((S,), NU),
+            grad_steps=torch.full((S,), grad_steps))
+        return {"runner_state": (train_state, *runner_tail), "metrics": out_metrics,
+                "sweep": self.grid.table(self.seed_lo, S)}
+
+
+class PQNEngine(EngineBase):
+    def __init__(self, config: dict, network: str, flatten_obs: bool, device=None):
+        super().__init__(config, flatten_obs, device)
+        self.network = network
+        self.spec, self.row_words, self.obs_dtype = network_spec(self.env, network, config)
+
     def forward(self, params, obs, S, rows, obs_rows_per_seed, q_out, gather=None, batch_stats=None):
         """network.apply({"params", "batch_stats"}, obs, train=False) (pqn_minatar.py:184-191)."""
         ws = self._workspace(S, rows)
-        if batch_stats is None:
-            batch_stats = getattr(self, "_cur_stats", None)
         _lib.check(_lib.lib().pqn_qnet_forward(self.spec.desc, _lib.p(params), _lib.p(batch_stats), _lib.raw(obs),
                                                _lib.p(gather),
                                                obs_rows_per_seed, _lib.p(q_out), S, rows, _lib.p(ws),
@@ -176,8 +336,8 @@ class PQNEngine:
 
     # ------------------------------------------------------------------ #
     def train(self, rngs):
-        c, dev, L = self.cfg, self.device, _lib.lib()
-        T, E, A, NU = self.T, self.E, self.A, self.NU
+        dev, L = self.device, _lib.lib()
+        T, E, A = self.T, self.E, self.A
         keys = jr.as_key_tensor(rngs, dev)
         assert keys.dim() == 2 and keys.shape[1] == 2, "train(rngs) takes the [NUM_SEEDS, 2] key array"
         S = keys.shape[0]
@@ -187,7 +347,7 @@ class PQNEngine:
         # minibatch step all-reduces (mean) the flat [S][P] gradient once before clip + RAdam, so parameters stay
         # bit-identical across ranks.  The minibatch permutation is per rank (statistically equivalent to the
         # reference's global shuffle, not sample-identical).
-        shard = getattr(self, "env_shard", None)
+        shard = self.env_shard
         E_total, env_lo, world, rank = E, 0, 1, 0
         if shard is not None and shard[1] > 1:
             import torch.distributed as dist
@@ -205,23 +365,17 @@ class PQNEngine:
         W = self.row_words
 
         # ---- schedules (pqn_minatar.py:134-147) and the other per-seed hyperparameters
-        hp, sched_stride = seed_tensors(seed_inputs(self.grid, self.seed_lo, S, NU, c["NUM_UPDATES_DECAY"],
-                                                    self.nmb * self.epochs, c.get("LR_LINEAR_DECAY", False)), dev)
+        hp, sched_stride = self._seed_tables(S)
         eps_table, sched = hp["eps"], hp["sched"]
 
         # ---- key chain (SURVEY Appendix B; pqn_minatar.py:172-173,415-423)
         k = jr.split(keys, 2, mode)
         K1 = k[:, 0].contiguous()                                   # :172 rng (also the init key, :173)
         params = spec.init(K1, dev)                                 # :156-170
-        mu = torch.zeros_like(params)
-        nu = torch.zeros_like(params)
-        grads = torch.zeros_like(params)
         F = spec.in_c
         batch_stats = spec.init_stats(S, dev)                       # flax BatchNorm running statistics: mean 0, var 1
-        self._cur_stats = batch_stats                               # read by forward() (train=False => running stats)
+        self.batch_stats = batch_stats                              # read by get_test_metrics (train=False)
         bn_sums = torch.zeros(S, 2 * F, device=dev)
-        step_counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        gnorm = torch.zeros(S * 64, device=dev)                     # block partials of the squared gradient norm
 
         k = jr.split(K1, 2, mode)
         K2, kT0 = k[:, 0].contiguous(), k[:, 1].contiguous()        # :415
@@ -237,8 +391,6 @@ class PQNEngine:
         targets = torch.zeros((S, T, E), dtype=torch.float32, device=dev)
         q_buf = torch.zeros((S * E, A), dtype=torch.float32, device=dev)
         info_sums = torch.zeros((S, 5), dtype=torch.float64, device=dev)
-        loss_sum = torch.zeros(S, device=dev)
-        qsa_sum = torch.zeros(S, device=dev)
         step_keys = torch.zeros((T, S, 2, 2), dtype=torch.int32, device=dev)
         eps_dev = torch.zeros((1, S), device=dev)                   # eps of every seed for this update
         # ---- reset (vmap_reset, :107-109,419)
@@ -248,29 +400,12 @@ class PQNEngine:
         self._write_obs(state, obs_buf, T, S)                        # update_body moves row T to row 0
         rng = jr.split(K3, 2, mode)[:, 1].contiguous()              # :422-423 runner rng
 
-        # pqn_minatar.py:330-338 reports env_frame; pqn_gymnax.py:324-331 does not
-        metric_names = ["env_step", "update_steps", *(["env_frame"] if self.network == "cnn" else []), "grad_steps",
-                        "td_loss", "qvals", *INFO_KEYS]
-        metrics = {m: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for m in metric_names}
-        test_hist = None
-        test_every = None
-        if self.test:
-            test_every = int(NU * c["TEST_INTERVAL"])
-            test_hist = {kk: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for kk in INFO_KEYS}
-        obs_channels = self.env.observation_space().shape[-1]
         sp = _lib.stream_ptr
-        timesteps = 0
-        grad_steps = 0
         seed_stride_obs = (T + 1) * E
         seed_stride_tr = T * E
-        # ---- static buffers of the update step (the whole step is CUDA-graph capturable)
-        rng_buf = rng.clone()                                        # runner rng, updated in place
-        kT_buf = torch.zeros((S, 2), dtype=torch.int32, device=dev)  # eval key of this update (:341)
-        upd_idx = torch.zeros(1, dtype=torch.int64, device=dev)      # n_updates on the device
-        m_cur = torch.zeros((S, 7), dtype=torch.float64, device=dev)  # td_loss, qvals, 5 info means
+        u = self._update_buffers(params, rng)                        # the whole step is CUDA-graph capturable
         ws = self._workspace(S, max(mb, E))
         perm_ws = jr.permutation_workspace(T * E, S, dev)
-        denom = float(self.epochs * self.nmb)
         bn_count = float(mb * world * (100 if self.network == "cnn" else 1))   # CNN: per channel over 10x10 pixels
 
         def allreduce_(t, avg):
@@ -283,30 +418,26 @@ class PQNEngine:
             """One `_update_step` (pqn_minatar.py:176-350) on the current stream; reads/writes only the static
             buffers above, so it can be replayed from a CUDA graph."""
             # ================= SAMPLE PHASE (:181-219)
-            eps_dev.copy_(eps_table.index_select(0, upd_idx))
+            eps_dev.copy_(eps_table.index_select(0, u.idx))
             obs_buf[:, 0].copy_(obs_buf[:, T])                       # last_obs of this rollout = last next_obs
-            carry = jr.split(rng_buf, 2, mode)[:, 1].contiguous()    # :213  `_rng`
+            carry = jr.split(u.rng, 2, mode)[:, 1].contiguous()      # :213  `_rng`
             _lib.check(L.pqn_rollout_keys(_lib.p(carry), _lib.p(step_keys), S, T, mode, sp()), "pqn_rollout_keys")
             info_sums.zero_()
             for t in range(T):
-                self.forward(params, obs_buf[:, t], S, E, seed_stride_obs, q_buf)
-                _lib.check(L.pqn_rollout_act_step_seeds(
-                    self.env.env_id, _lib.p(step_keys[t]), _lib.p(q_buf), _lib.p(eps_dev), _lib.p(state),
-                    _lib.raw(obs_buf[:, t + 1]), seed_stride_obs,
-                    _lib.raw(act_buf[:, t]), _lib.raw(rew_buf[:, t]),
-                    _lib.raw(done_buf[:, t]), _lib.raw(maxq_buf[:, t]),
-                    seed_stride_tr, _lib.p(info_sums), 0, S, E, E_total, env_lo, self.max_steps, _lib.p(hp["rew_scale"]),
-                    mode, sp()), "pqn_rollout_act_step_seeds")
+                self.forward(params, obs_buf[:, t], S, E, seed_stride_obs, q_buf, batch_stats=batch_stats)
+                self._act_step(S, E, step_keys[t], q_buf, eps_dev, state, obs_buf[:, t + 1], act_buf[:, t],
+                               rew_buf[:, t], done_buf[:, t], maxq_buf[:, t], info_sums, 0, hp["rew_scale"],
+                               seed_stride_obs, seed_stride_tr, E_total, env_lo)
             r = carry                                                # scan's final carry (:214)
             # ================= bootstrap + Q(lambda) (:227-260)
-            self.forward(params, obs_buf[:, T], S, E, seed_stride_obs, q_buf)
+            self.forward(params, obs_buf[:, T], S, E, seed_stride_obs, q_buf, batch_stats=batch_stats)
             _lib.check(L.pqn_qlambda_seeds(_lib.p(rew_buf), _lib.p(done_buf), _lib.p(maxq_buf), _lib.p(q_buf),
                                            _lib.p(targets), T, S, E, A, _lib.p(hp["gamma"]), _lib.p(hp["lam"]), sp()),
                        "pqn_qlambda_seeds")
             # ================= NETWORKS UPDATE (:263-327)
             r = jr.split(r, 2, mode)[:, 0].contiguous()              # :324
-            loss_sum.zero_()
-            qsa_sum.zero_()
+            u.loss_sum.zero_()
+            u.qsa_sum.zero_()
             for _ in range(self.epochs):
                 k = jr.split(r, 2, mode)                             # :309
                 r, kperm = k[:, 0].contiguous(), k[:, 1].contiguous()
@@ -318,109 +449,29 @@ class PQNEngine:
                     _lib.check(L.pqn_qnet_loss_grad(
                         spec.desc, _lib.p(params), _lib.p(batch_stats), _lib.p(obs_buf), _lib.p(perm_view[mbi]),
                         seed_stride_obs,
-                        _lib.p(act_buf), _lib.p(targets), seed_stride_tr, _lib.p(grads), _lib.p(loss_sum),
-                        _lib.p(qsa_sum), _lib.p(bn_sums), S, mb, _lib.p(ws), sp()), "pqn_qnet_loss_grad")
-                    allreduce_(grads, True)                          # the ONE collective of the data path
+                        _lib.p(act_buf), _lib.p(targets), seed_stride_tr, _lib.p(u.grads), _lib.p(u.loss_sum),
+                        _lib.p(u.qsa_sum), _lib.p(bn_sums), S, mb, _lib.p(ws), sp()), "pqn_qnet_loss_grad")
+                    allreduce_(u.grads, True)                        # the ONE collective of the data path
                     allreduce_(bn_sums, False)
-                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu),
-                                                           _lib.p(sched), sched_stride, _lib.p(step_counter),
-                                                           _lib.p(gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
+                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(u.grads), _lib.p(u.mu), _lib.p(u.nu),
+                                                           _lib.p(sched), sched_stride, _lib.p(u.step_counter),
+                                                           _lib.p(u.gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
                                                            1e-8, sp()), "pqn_radam_clip_step_seeds")
                     _lib.check(L.pqn_bn_stats_update(_lib.p(batch_stats), _lib.p(bn_sums), S, F, spec.stats_total,
                                                      bn_count, 0.99, sp()), "pqn_bn_stats_update")
-            if self.test:                                            # :341  rng, _rng = split(rng)
-                k = jr.split(r, 2, mode)
-                r = k[:, 0].contiguous()
-                kT_buf.copy_(k[:, 1])
-            rng_buf.copy_(r)
-            allreduce_(loss_sum, True)
-            allreduce_(qsa_sum, True)
+            allreduce_(u.loss_sum, True)
+            allreduce_(u.qsa_sum, True)
             allreduce_(info_sums, False)
-            m_cur[:, 0] = loss_sum.double() / denom
-            m_cur[:, 1] = qsa_sum.double() / denom
-            m_cur[:, 2:7] = info_sums / float(T * E_total)
-            upd_idx.add_(1)
+            self._end_update(u, r, info_sums)                        # :341
 
-        # CUDA graph: "auto" captures the update when the run is launch-bound (small S*E); the first update runs
-        # eagerly (warms every code path), later updates replay the captured graph.
-        want_graph = c.get("CUDA_GRAPH", "auto")
-        use_graph = (S * E * T <= (1 << 21) and world == 1) if want_graph == "auto" else bool(want_graph)
-        use_graph = use_graph and NU > 2
-        graph = None
-        self.graph_captured = False
-        self.graph_replays = 0
-        self.graph_launches_per_replay = 0
-
-        # hooks (bench / tests): both are called on the host OUTSIDE the captured region, so they do not prevent
-        # CUDA-graph replay.  on_update_end receives the static rollout buffers of the update that just ran.
-        on_update_begin = getattr(self, "on_update_begin", None)
-        on_update_end = getattr(self, "on_update_end", None)
-        dbg = dict(obs=obs_buf, action=act_buf, reward=rew_buf, done=done_buf, maxq=maxq_buf, targets=targets,
-                   params=params, state=state, rng=rng_buf)
-        for n_updates in range(NU):
-            if on_update_begin is not None:
-                on_update_begin(n_updates)
-            if graph is not None:
-                graph.replay()
-                self.graph_replays += 1
-            else:
-                update_body()
-                if use_graph and n_updates == 0:
-                    try:
-                        torch.cuda.synchronize(dev)
-                        g = torch.cuda.CUDAGraph()
-                        l0 = L.pqn_launch_count()
-                        with torch.cuda.graph(g):
-                            update_body()
-                        self.graph_launches_per_replay = int(L.pqn_launch_count() - l0)
-                        graph = g
-                        self.graph_captured = True
-                    except Exception as e:                            # capture is an optimisation only
-                        import warnings
-                        warnings.warn(f"CUDA graph capture of the update step failed ({e!r}); running eagerly")
-                        graph = None
-                        use_graph = False
-                        torch.cuda.synchronize(dev)
-            if on_update_end is not None:
-                on_update_end(n_updates, dbg)
-            timesteps += T * E_total                                 # :222-225
-            grad_steps += self.nmb * self.epochs
-            # ================= metrics (:329-338)
-            n_done = n_updates + 1
-            col = n_updates
-            metrics["env_step"][:, col] = timesteps
-            metrics["update_steps"][:, col] = n_done
-            if "env_frame" in metrics:
-                metrics["env_frame"][:, col] = timesteps * obs_channels
-            metrics["grad_steps"][:, col] = grad_steps
-            metrics["td_loss"][:, col] = m_cur[:, 0]
-            metrics["qvals"][:, col] = m_cur[:, 1]
-            for j, kk in enumerate(INFO_KEYS):
-                metrics[kk][:, col] = m_cur[:, 2 + j]
-            # ================= evaluation (:340-350)
-            if self.test:
-                if test_every > 0 and n_done % test_every == 0:
-                    test_metrics = self.get_test_metrics(params, kT_buf.clone())
-                for kk in INFO_KEYS:
-                    test_hist[kk][:, col] = test_metrics[kk]
-            if c.get("WANDB_MODE", "disabled") != "disabled":
-                self._wandb_log(metrics, test_hist, col, jr.to_numpy_u32(keys)[:, 0])
-        rng = rng_buf
-
-        torch.cuda.synchronize(dev)
-        out_metrics = {m: v[:, :NU].float() if m in ("td_loss", "qvals", *INFO_KEYS) else v[:, :NU].to(torch.int64)
-                       for m, v in metrics.items()}
-        if self.test:
-            out_metrics.update({f"test/{kk}": v[:, :NU].float() for kk, v in test_hist.items()})
-        train_state = TrainState(
-            params=spec.unflatten(params), params_flat=params,
-            batch_stats=spec.unflatten_stats(batch_stats), batch_stats_flat=batch_stats,
-            opt_state=SimpleNamespace(mu=mu, nu=nu, count=grad_steps),
-            timesteps=torch.full((S,), timesteps, dtype=torch.int64), n_updates=torch.full((S,), NU),
-            grad_steps=torch.full((S,), grad_steps))
-        expl_state = (self._final_obs(obs_buf, S), state)
-        return {"runner_state": (train_state, expl_state, test_metrics, rng), "metrics": out_metrics,
-                "sweep": self.grid.table(self.seed_lo, S)}
+        # "auto" captures the update when the run is launch-bound (small S*E)
+        payload = dict(obs=obs_buf, action=act_buf, reward=rew_buf, done=done_buf, maxq=maxq_buf, targets=targets,
+                       params=params, state=state, rng=u.rng)
+        metrics, test_hist, test_metrics = self._run_updates(
+            keys, params, u, update_body, payload, S * E * T <= (1 << 21) and world == 1, test_metrics,
+            frame_channels=self.env.observation_space().shape[-1] if self.network == "cnn" else None)
+        expl_state = (obs_buf[:, -1].contiguous(), state)
+        return self._result(params, batch_stats, u, metrics, test_hist, (expl_state, test_metrics, u.rng))
 
     # ------------------------------------------------------------------ #
     def _write_obs(self, state, obs_buf, t, S):
@@ -428,7 +479,7 @@ class PQNEngine:
         L = _lib.lib()
         E = obs_buf.shape[2]
         tmp = torch.empty((S * E, self.row_words), dtype=self.obs_dtype, device=self.device)
-        if self.binary:
+        if self.env.binary_obs:
             _lib.check(L.pqn_env_obs_packed(self.env.env_id, _lib.p(state), _lib.p(tmp), S * E, _lib.stream_ptr()),
                        "pqn_env_obs_packed")
         else:
@@ -436,16 +487,12 @@ class PQNEngine:
                        "pqn_env_obs")
         obs_buf[:, t] = tmp.view(S, E, self.row_words)
 
-    def _final_obs(self, obs_buf, S):
-        st_obs = obs_buf[:, -1]
-        return st_obs.contiguous()
-
     # ------------------------------------------------------------------ #
     def get_test_metrics(self, params, rng):
         """Greedy evaluation rollout (pqn_minatar.py:371-413), incl. its key quirks:
         the scan carry starts at the reset key `_rng`, and each step uses the same
-        sub-key for the action keys and the env keys."""
-        c, dev, L, mode = self.cfg, self.device, _lib.lib(), self.rng_mode
+        sub-key for the action keys and the env keys.  The network reads ``self.batch_stats``."""
+        c, dev, mode = self.cfg, self.device, self.rng_mode
         S = rng.shape[0]
         N = int(c["TEST_NUM_ENVS"])
         steps = int(c["TEST_NUM_STEPS"])
@@ -463,36 +510,18 @@ class PQNEngine:
         scratch_f2 = torch.zeros((S, N), dtype=torch.float32, device=dev)
         scratch_b = torch.zeros((S, N), dtype=torch.uint8, device=dev)
         sums = torch.zeros((S, 5), dtype=torch.float64, device=dev)
-        eps = torch.full((1,), float(c["EPS_TEST"]), device=dev)
+        eps = torch.full((S,), float(c["EPS_TEST"]), device=dev)
+        ones = torch.ones(S, device=dev)                             # the evaluation's rewards are not scaled
         carry = kr                                                   # :399-401
         for t in range(steps):
             k = jr.split(carry, 2, mode)                             # :378
             carry, ku = k[:, 0].contiguous(), k[:, 1].contiguous()
             sk = torch.stack([ku, ku], 1).contiguous()               # same key for actions and env (:388-393)
             cur, nxt = t & 1, (t + 1) & 1
-            self.forward(params, obs[:, cur], S, N, 2 * N, q)
-            _lib.check(L.pqn_rollout_act_step(
-                self.env.env_id, _lib.p(sk), _lib.p(q), _lib.p(eps), _lib.p(state),
-                _lib.raw(obs[:, nxt]), 2 * N, _lib.p(scratch_i), _lib.p(scratch_f), _lib.p(scratch_b),
-                _lib.p(scratch_f2), N, _lib.p(sums), 1, S, N, 0, 0, self.max_steps, 1.0, mode, _lib.stream_ptr()),
-                "pqn_rollout_act_step")
-        cnt = sums[:, 3]
-        out = {}
-        for j, kk in enumerate(INFO_KEYS):
-            out[kk] = torch.where(cnt > 0, sums[:, j] / cnt.clamp(min=1), torch.full_like(cnt, float("nan")))
-        return out
-
-    def _wandb_log(self, metrics, test_hist, col, seed_labels):
-        import wandb
-        S = metrics["td_loss"].shape[0]
-        row = {m: v[:, col].mean().item() for m, v in metrics.items()}
-        if test_hist is not None:
-            row.update({f"test/{kk}": v[:, col].nanmean().item() for kk, v in test_hist.items()})
-        if self.cfg.get("WANDB_LOG_ALL_SEEDS", False):
-            for s in range(S):
-                for m, v in metrics.items():
-                    row[f"rng{int(seed_labels[s])}/{m}"] = v[s, col].item()
-        wandb.log(row, step=int(row["update_steps"]))
+            self.forward(params, obs[:, cur], S, N, 2 * N, q, batch_stats=self.batch_stats)
+            self._act_step(S, N, sk, q, eps, state, obs[:, nxt], scratch_i, scratch_f, scratch_b, scratch_f2, sums, 1,
+                           ones, 2 * N, N, N, 0)
+        return self._episode_means(sums)
 
 
 def prepare_config(config: dict, env_max_steps: int, allow_test_steps_override: bool):

@@ -18,53 +18,31 @@ from __future__ import annotations
 
 from types import SimpleNamespace
 
-import numpy as np
 import torch
 
-from . import _lib, envs, jaxrandom as jr, sweep
-from .engine import INFO_KEYS, TrainState, seed_inputs, seed_tensors
+from . import _lib, envs, jaxrandom as jr
+from .engine import EngineBase
 from .networks import NET_RNN, QNetworkSpec
 
 
-class PQNRnnEngine:
+class PQNRnnEngine(EngineBase):
     def __init__(self, config: dict, device=None, env_params: envs.EnvParams | None = None):
-        self.cfg = c = config
-        self.grid = sweep.Grid(config)       # per-seed hyperparameters: a grid of G points x NUM_SEEDS
-        self.seed_lo = 0            # global index of this run's first seed (a seed-sharded rank trains a slice)
-        self.device = torch.device(device or "cuda")
-        self.rng_mode = int(c.get("JAX_THREEFRY_PARTITIONABLE", 0))
-        self.env, self.env_params = envs.make(c["ENV_NAME"], flatten_obs=True, rng_mode=self.rng_mode)
-        if self.env.binary_obs:   # its memory buffer stores float observation rows
+        if config["ENV_NAME"] in envs.MINATAR_GAMES:                 # its memory buffer stores float observation rows
             raise NotImplementedError("the recurrent script is built for the float-observation envs "
                                       "(classic control, MemoryChain-bsuite)")
-        if self.device.type != "cuda" or not torch.cuda.is_available():
-            raise _lib.PqnError("purejaxql_b200 needs a CUDA device: there is no CPU fallback")
-        _lib.lib()
-        if env_params is not None:                                   # e.g. MemoryChain's memory_length (:134-136)
-            self.env_params = env_params
-        self.max_steps = int(self.env_params.max_steps_in_episode)
-        self.T, self.E, self.NU = int(c["NUM_STEPS"]), int(c["NUM_ENVS"]), int(c["NUM_UPDATES"])
+        super().__init__(config, True, device, env_params)           # env_params: MemoryChain's memory_length (:134-136)
+        c = config
         self.W = int(c["MEMORY_WINDOW"])
-        self.A, self.D = self.env.num_actions, self.env.obs_dim
+        self.D = self.env.obs_dim
         self.H = int(c.get("HIDDEN_SIZE", 128))
         self.spec = QNetworkSpec(NET_RNN, self.D, self.A, self.H, int(c.get("NUM_LAYERS", 2)),
                                  norm_type=c.get("NORM_TYPE", "layer_norm"), norm_input=bool(c.get("NORM_INPUT", False)))
         # the default network keeps the entry points without running statistics (its BatchNorm_0 output is discarded)
         self.with_stats = self.spec.norm_type != "layer_norm" or self.spec.norm_input
-        self.batch_stats = None                                      # [S][stats_total] running statistics (with_stats)
-        self.nmb, self.epochs = int(c["NUM_MINIBATCHES"]), int(c["NUM_EPOCHS"])
         assert self.E % self.nmb == 0, "NUM_MINIBATCHES must divide NUM_ENVS (minibatches are whole env trajectories)"
         self.Bm = self.E // self.nmb
-        self.test = bool(c.get("TEST_DURING_TRAINING", False))
-        self._ws = None
 
     # ------------------------------------------------------------------ #
-    def _workspace(self, S, rows):
-        need = int(_lib.lib().pqn_net_workspace_bytes(self.spec.desc, S, rows))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        return self._ws
-
     def step(self, params, hs, obs, last_done, last_action, q, S, N):
         """network.apply(params, hs, obs[None], done[None], last_action[None], train=False) for S x N envs; hs in place.
         The BatchNorm variants normalise with ``self.batch_stats``."""
@@ -77,15 +55,6 @@ class PQNRnnEngine:
             _lib.check(L.pqn_rnn_step(self.spec.desc, _lib.p(params), _lib.p(hs), _lib.p(obs), N, _lib.p(last_done),
                                       _lib.p(last_action), _lib.p(q), S, N, _lib.p(ws), _lib.stream_ptr()), "pqn_rnn_step")
 
-    def _act_step(self, S, N, step_keys, q, eps, state, obs_next, action, reward, done, maxq, sums, done_only, rew_scale):
-        """eps and rew_scale: float32[S] device values of each seed."""
-        L = _lib.lib()
-        _lib.check(L.pqn_rollout_act_step_seeds(self.env.env_id, _lib.p(step_keys), _lib.p(q), _lib.p(eps),
-                                                _lib.p(state), _lib.p(obs_next), N, _lib.p(action), _lib.p(reward),
-                                                _lib.p(done), _lib.p(maxq), N, _lib.p(sums), done_only, S, N, 0, 0,
-                                                self.max_steps, _lib.p(rew_scale), self.rng_mode, _lib.stream_ptr()),
-                   "pqn_rollout_act_step_seeds")
-
     def _reset(self, key, S, N):
         """vmap_reset(N)(key): obs [S,N,D], state."""
         dev, mode = self.device, self.rng_mode
@@ -97,14 +66,13 @@ class PQNRnnEngine:
 
     # ------------------------------------------------------------------ #
     def train(self, rngs):
-        c, dev, L, mode = self.cfg, self.device, _lib.lib(), self.rng_mode
-        T, E, A, NU, W, H, D, Bm = self.T, self.E, self.A, self.NU, self.W, self.H, self.D, self.Bm
+        dev, L, mode = self.device, _lib.lib(), self.rng_mode
+        T, E, A, W, H, D, Bm = self.T, self.E, self.A, self.W, self.H, self.D, self.Bm
         Tm = W + T
         keys = jr.as_key_tensor(rngs, dev)
         S = keys.shape[0]
         spec, P = self.spec, self.spec.total
-        hp, sched_stride = seed_tensors(seed_inputs(self.grid, self.seed_lo, S, NU, c["NUM_UPDATES_DECAY"],
-                                                    self.nmb * self.epochs, c.get("LR_LINEAR_DECAY", False)), dev)
+        hp, sched_stride = self._seed_tables(S)
         eps_table, sched = hp["eps"], hp["sched"]                   # [NU][S], RAdam rows (sweep layout)
 
         # ---- key chain (:255-256, :505-543)
@@ -112,9 +80,6 @@ class PQNRnnEngine:
         rng = k[:, 0].contiguous()                                   # :255  rng, _rng = split(rng)
         params = spec.init(rng, dev)                                 # :256  create_agent(rng)  (the CARRIED key)
         self.batch_stats = spec.init_stats(S, dev) if self.with_stats else None   # mean 0, var 1
-        mu, nu, grads = torch.zeros_like(params), torch.zeros_like(params), torch.zeros_like(params)
-        step_counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        gnorm = torch.zeros(S * 64, device=dev)
         k = jr.split(rng, 2, mode)
         rng, kT = k[:, 0].contiguous(), k[:, 1].contiguous()         # :505
         test_metrics = self.get_test_metrics(params, kT) if self.test else None
@@ -156,7 +121,7 @@ class PQNRnnEngine:
                 mem.last_done[:, s].copy_(last_done); mem.last_action[:, s].copy_(last_action)
                 self.step(params, hs, last_obs, last_done, last_action, q, S, E)
                 self._act_step(S, E, step_keys[t], q, eps, state, new_obs, act_t, rew_t, done_t, maxq, info_sums, 0,
-                               hp["rew_scale"])
+                               hp["rew_scale"], E, E, E, 0)
                 mem.action[:, s].copy_(act_t); mem.reward[:, s].copy_(rew_t); mem.done[:, s].copy_(done_t)
                 last_obs.copy_(new_obs)
                 last_done.copy_(done_t); last_action.copy_(act_t)
@@ -168,33 +133,21 @@ class PQNRnnEngine:
         k = jr.split(rng, 2, mode)                                   # :541
         rng = k[:, 1].contiguous()                                   # runner rng = _rng
 
-        metric_names = ["env_step", "update_steps", "grad_steps", "td_loss", "qvals", *INFO_KEYS]
-        metrics = {m: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for m in metric_names}
-        test_hist = {kk: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for kk in INFO_KEYS} if self.test else None
-        test_every = int(NU * c["TEST_INTERVAL"]) if self.test else None
-        loss_sum, qsa_sum = torch.zeros(S, device=dev), torch.zeros(S, device=dev)
+        u = self._update_buffers(params, rng)                        # static buffers of the update step
         ws = self._workspace(S, max(Tm * Bm, E))
         perm_ws = jr.permutation_workspace(E, S, dev)
-        timesteps = grad_steps = 0
-        denom = float(self.epochs * self.nmb)
-        on_update_end = getattr(self, "on_update_end", None)
-        # static buffers of the update step (graph capturable, like engine.PQNEngine)
-        rng_buf = rng.clone()
-        kT_buf = torch.zeros((S, 2), dtype=torch.int32, device=dev)
-        upd_idx = torch.zeros(1, dtype=torch.int64, device=dev)
-        m_cur = torch.zeros((S, 7), dtype=torch.float64, device=dev)
 
         def update_body():
             # ================= SAMPLE PHASE (:190-236)
-            eps_dev.copy_(eps_table.index_select(0, upd_idx))
-            k = jr.split(rng_buf, 2, mode)                           # :222
+            eps_dev.copy_(eps_table.index_select(0, u.idx))
+            k = jr.split(u.rng, 2, mode)                             # :222
             info_sums.zero_()
             for name in ("hs", "obs", "action", "reward", "done", "last_done", "last_action"):   # :239-243 shift the memory
                 buf = getattr(mem, name)
                 buf[:, :W].copy_(buf[:, T:T + W].clone())
             rng = rollout(k[:, 1].contiguous(), T, W, eps_dev)       # rng := final carry of the scan (:223-228)
             # ================= NETWORKS UPDATE (:246-386)
-            loss_sum.zero_(); qsa_sum.zero_()
+            u.loss_sum.zero_(); u.qsa_sum.zero_()
             k = jr.split(rng, 2, mode)                               # :381  (the scan carry starts at `rng`)
             r = k[:, 0].contiguous()
             for _ in range(self.epochs):
@@ -214,80 +167,23 @@ class PQNRnnEngine:
                     # batch_stats = updates["batch_stats"] (:362-369); None for the default network
                     _lib.check(L.pqn_rnn_loss_grad_seeds(
                         spec.desc, _lib.p(params), _lib.p(self.batch_stats), _lib.p(hs0), _lib.p(obs_mb), _lib.p(ld),
-                        _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(grads), _lib.p(loss_sum),
-                        _lib.p(qsa_sum), S, Tm, Bm, _lib.p(hp["gamma"]), _lib.p(hp["lam"]), _lib.p(ws),
+                        _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(u.grads), _lib.p(u.loss_sum),
+                        _lib.p(u.qsa_sum), S, Tm, Bm, _lib.p(hp["gamma"]), _lib.p(hp["lam"]), _lib.p(ws),
                         _lib.stream_ptr()), "pqn_rnn_loss_grad_seeds")
-                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(grads), _lib.p(mu), _lib.p(nu),
-                                                           _lib.p(sched), sched_stride, _lib.p(step_counter),
-                                                           _lib.p(gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
+                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(u.grads), _lib.p(u.mu), _lib.p(u.nu),
+                                                           _lib.p(sched), sched_stride, _lib.p(u.step_counter),
+                                                           _lib.p(u.gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
                                                            1e-8, _lib.stream_ptr()), "pqn_radam_clip_step_seeds")
-            if self.test:                                            # :398  rng, _rng = split(rng)
-                k = jr.split(r, 2, mode)
-                r = k[:, 0].contiguous()
-                kT_buf.copy_(k[:, 1])
-            rng_buf.copy_(r)
-            m_cur[:, 0] = loss_sum.double() / denom
-            m_cur[:, 1] = qsa_sum.double() / denom
-            m_cur[:, 2:7] = info_sums / float(T * E)
-            upd_idx.add_(1)
+            self._end_update(u, r, info_sums)                        # :398
 
-        # CUDA graph: these runs are launch-bound (32 envs x 64 steps: thousands of small launches per update), so the
-        # update is captured after the first eager one and replayed unless CUDA_GRAPH is false
-        want_graph = c.get("CUDA_GRAPH", "auto")
-        use_graph = (True if want_graph == "auto" else bool(want_graph)) and NU > 2
-        graph = None
-        self.graph_captured = False
-        for n_updates in range(NU):
-            if graph is not None:
-                graph.replay()
-            else:
-                update_body()
-                if use_graph and n_updates == 0:
-                    try:
-                        torch.cuda.synchronize(dev)
-                        g = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(g):
-                            update_body()
-                        graph = g
-                        self.graph_captured = True
-                    except Exception as e:                            # capture is an optimisation only
-                        import warnings
-                        warnings.warn(f"CUDA graph capture of the recurrent update failed ({e!r}); running eagerly")
-                        graph, use_graph = None, False
-                        torch.cuda.synchronize(dev)
-            timesteps += T * E
-            grad_steps += self.nmb * self.epochs
-            col = n_updates
-            metrics["env_step"][:, col] = timesteps
-            metrics["update_steps"][:, col] = n_updates + 1
-            metrics["grad_steps"][:, col] = grad_steps
-            metrics["td_loss"][:, col] = m_cur[:, 0]
-            metrics["qvals"][:, col] = m_cur[:, 1]
-            for j, kk in enumerate(INFO_KEYS):
-                metrics[kk][:, col] = m_cur[:, 2 + j]
-            if on_update_end is not None:
-                on_update_end(n_updates, dict(mem=mem, params=params, rng=rng_buf, batch_stats=self.batch_stats))
-            if self.test:                                            # :398-408
-                if test_every > 0 and (n_updates + 1) % test_every == 0:
-                    test_metrics = self.get_test_metrics(params, kT_buf.clone())
-                for kk in INFO_KEYS:
-                    test_hist[kk][:, col] = test_metrics[kk]
-        rng = rng_buf
-        torch.cuda.synchronize(dev)
-        out_metrics = {m: v[:, :NU].float() if m in ("td_loss", "qvals", *INFO_KEYS) else v[:, :NU].to(torch.int64)
-                       for m, v in metrics.items()}
-        if self.test:
-            out_metrics.update({f"test/{kk}": v[:, :NU].float() for kk, v in test_hist.items()})
-        F = spec.in_c
+        # these runs are launch-bound (32 envs x 64 steps: thousands of small launches per update), so "auto" always
+        # captures the update
+        metrics, test_hist, test_metrics = self._run_updates(
+            keys, params, u, update_body, dict(mem=mem, params=params, rng=u.rng, batch_stats=self.batch_stats), True,
+            test_metrics)
         bs = self.batch_stats if self.with_stats else spec.init_stats(S, dev)
-        train_state = TrainState(
-            params=spec.unflatten(params), params_flat=params, batch_stats=spec.unflatten_stats(bs), batch_stats_flat=bs,
-            opt_state=SimpleNamespace(mu=mu, nu=nu, count=grad_steps),
-            timesteps=torch.full((S,), timesteps, dtype=torch.int64), n_updates=torch.full((S,), NU),
-            grad_steps=torch.full((S,), grad_steps))
         expl_state = (hs, last_obs, last_done, last_action, state)
-        return {"runner_state": (train_state, mem, expl_state, test_metrics, rng), "metrics": out_metrics,
-                "sweep": self.grid.table(self.seed_lo, S)}
+        return self._result(params, bs, u, metrics, test_hist, (mem, expl_state, test_metrics, u.rng))
 
     # ------------------------------------------------------------------ #
     def get_test_metrics(self, params, rng):
@@ -314,9 +210,7 @@ class PQNRnnEngine:
         _lib.check(L.pqn_rollout_keys(_lib.p(carry), _lib.p(step_keys), S, steps, mode, _lib.stream_ptr()), "pqn_rollout_keys")
         for t in range(steps):
             self.step(params, hs, obs, ld, la, q, S, N)
-            self._act_step(S, N, step_keys[t], q, eps, state, nxt, act, rw, dn, mq, sums, 1, ones)
+            self._act_step(S, N, step_keys[t], q, eps, state, nxt, act, rw, dn, mq, sums, 1, ones, N, N, N, 0)
             obs, nxt = nxt, obs
             ld.copy_(dn); la.copy_(act)
-        cnt = sums[:, 3]
-        return {kk: torch.where(cnt > 0, sums[:, j] / cnt.clamp(min=1), torch.full_like(cnt, float("nan")))
-                for j, kk in enumerate(INFO_KEYS)}
+        return self._episode_means(sums)
