@@ -3227,7 +3227,8 @@ int pqn_qnet_loss_grad(const pqn_net_desc_t* d, const float* params, float* batc
       // dz of the conv is rstd times a dense-layer-sized gradient, and rstd reaches 1 / sqrt(LN_EPS) = 1000 on the empty
       // 3x3 patches of the initial parameters (conv bias 0: z = 0, var = 0).  One sixteenth of the dense gradient scale,
       // 2^ceil(log2 rows), keeps it above the subnormals; the headroom below the fp16 maximum (conversions saturate) is
-      // small: test_gpu_cnn_grads.py measures max |dz * gs| = 3.96e4 at init with TD errors of scale 30 (1.65x below)
+      // small: test_gpu_cnn_grads.py measures max |dz * gs| = 3.96e4 at init with TD errors of scale 30 (1.65x below),
+      // test_gpu_cnn_grads_tiles.py 4.02e4 at C = 7 (1.63x below)
       const float gs16 = grad_scale((int)rows) * (1.0f / 16.0f);
       if (g_conv_mma == 1) {
         switch (d->in_c) {
