@@ -178,30 +178,38 @@ __device__ __forceinline__ void store_patch16(const uint32_t* __restrict__ so, i
     *reinterpret_cast<uint4*>(row + 4 * q) = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
 }
 
-// conv output z of the NB m-blocks mb0 .. mb0 + NB - 1 (m-block mb = pixels 16 mb .. 16 mb + 15): z[i] holds pixel
-// rows 16 (mb0 + i) + g and + 8.  The training forward runs two m-blocks at a time, the backward one; every
-// accumulator sees the same MMA sequence either way, so both get the same bits.
-template <int C, int NB>
-__device__ __forceinline__ void conv16_blocks(const uint32_t* __restrict__ xp, const uint4* __restrict__ wb,
-                                              const float* __restrict__ cb, int mb0, int lane, float (&z)[NB][2][4]) {
+// conv output z of NB blocks of 16 pixels from patch rows ra (fragment row g of block 0), rb (row g + 8 of block 0) and
+// ra / rb + i * BSTRIDE words for block i; cb4 = conv bias of the thread's channels 4t .. 4t+3.  PAIRED: the two rows
+// are interleaved per k-step at ra (words 4s, 4s+1 of row g, 4s+2, 4s+3 of row g + 8: one 16-byte load; rb unused).
+// Which pixel feeds which fragment row does not change any accumulator's MMA sequence, so every caller gets the same
+// bits per pixel.
+template <int C, int NB, int BSTRIDE, bool PAIRED = false>
+__device__ __forceinline__ void conv16_blocks_rows(const uint32_t* __restrict__ ra, const uint32_t* __restrict__ rb,
+                                                   const uint4* __restrict__ wb, const float (&cb4)[4], int lane,
+                                                   float (&z)[NB][2][4]) {
   using M = Conv16<C>;
-  const int g = lane >> 2, t = lane & 3;
+  const int t = lane & 3;
   const uint32_t mask = (1u << (10 + t)) | (1u << (26 + t));
 #pragma unroll
   for (int i = 0; i < NB; ++i)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      z[i][h][0] = z[i][h][2] = cb[4 * t + 2 * h];       // conv16_channel(h, 2t), (h, 2t + 1)
-      z[i][h][1] = z[i][h][3] = cb[4 * t + 2 * h + 1];
+      z[i][h][0] = z[i][h][2] = cb4[2 * h];       // conv16_channel(h, 2t), (h, 2t + 1)
+      z[i][h][1] = z[i][h][3] = cb4[2 * h + 1];
     }
-  const uint32_t* r00 = xp + (16 * mb0 + g) * M::ROW;
 #pragma unroll
   for (int s = 0; s < M::KS; ++s) {
     uint32_t a[NB][4];
 #pragma unroll
     for (int i = 0; i < NB; ++i) {
-      const uint2 w0 = *reinterpret_cast<const uint2*>(r00 + (16 * i) * M::ROW + 2 * s);       // pixel row g
-      const uint2 w1 = *reinterpret_cast<const uint2*>(r00 + (16 * i + 8) * M::ROW + 2 * s);   // pixel row g + 8
+      uint2 w0, w1;   // fragment rows g and g + 8
+      if (PAIRED) {
+        const uint4 v = *reinterpret_cast<const uint4*>(ra + i * BSTRIDE + 4 * s);
+        w0 = make_uint2(v.x, v.y); w1 = make_uint2(v.z, v.w);
+      } else {
+        w0 = *reinterpret_cast<const uint2*>(ra + i * BSTRIDE + 2 * s);
+        w1 = *reinterpret_cast<const uint2*>(rb + i * BSTRIDE + 2 * s);
+      }
       a[i][0] = w0.x & mask; a[i][1] = w1.x & mask; a[i][2] = w0.y & mask; a[i][3] = w1.y & mask;
     }
     uint4 b[2];
@@ -217,6 +225,19 @@ __device__ __forceinline__ void conv16_blocks(const uint32_t* __restrict__ xp, c
 #pragma unroll
       for (int i = 0; i < NB; ++i) mma_f16_16n8k16(z[i][h], a[i], b[h].x, b[h].y);
   }
+}
+
+// conv output z of the NB m-blocks mb0 .. mb0 + NB - 1 (m-block mb = pixels 16 mb .. 16 mb + 15): z[i] holds pixel
+// rows 16 (mb0 + i) + g and + 8.  The training forward runs two m-blocks at a time; every accumulator sees the same MMA
+// sequence however many blocks share a call, so the backward's rebuild (conv16_blocks_rows) gets the same bits.
+template <int C, int NB>
+__device__ __forceinline__ void conv16_blocks(const uint32_t* __restrict__ xp, const uint4* __restrict__ wb,
+                                              const float* __restrict__ cb, int mb0, int lane, float (&z)[NB][2][4]) {
+  using M = Conv16<C>;
+  const int g = lane >> 2, t = lane & 3;
+  const float cb4[4] = {cb[4 * t], cb[4 * t + 1], cb[4 * t + 2], cb[4 * t + 3]};
+  const uint32_t* r00 = xp + (16 * mb0 + g) * M::ROW;
+  conv16_blocks_rows<C, NB, 16 * M::ROW>(r00, r00 + 8 * M::ROW, wb, cb4, lane, z);
 }
 
 // LayerNorm of one m-block of conv16_blocks: xhat of pixel rows 16 mb + g (x0) and + 8 (x1) in the thread's channels

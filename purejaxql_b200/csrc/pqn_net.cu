@@ -1733,41 +1733,42 @@ __global__ void __launch_bounds__(ConvBwdSmem<C>::WARPS * 32, 2)
 //     dzT[plane][channel][pixel pair], the pairs (t, t + 4) of a k-step adjacent so that (b0, b1) is one LDS.64; the
 //     k-step block of a channel row is XOR-swizzled so that the phase-A stores and the fragment loads are conflict free.
 //   * 48 MMAs per sample (3 m-tiles x 2 n-tiles x 4 k-steps x {hi, lo}) instead of 96 tf32 ones.
-// Phase A works on the pixel pair (16 mb + 2g, + 1) per thread (it was (g, g + 8)): a thread's two dz values of one
-// channel are exactly one B word.  The DY / xhat stage has a row + column swizzle for that access pattern.
-// xhat and rstd are not read from memory: just before phase A handles m-block mb, the warp rebuilds that m-block's
-// conv output from the sample's packed observation with the training forward's own code (conv16_blocks,
-// conv16_xhat) and the same parameters, so they are bit for bit what the forward computed.  The rebuild costs the
-// forward's MMAs again (48 at C = 4, 96 at C = 10); it saves 4,352 bytes per sample of HBM writes in the forward and as
-// many reads here.
+// xhat and rstd are not read from memory: phase A reruns the training forward's conv MMAs and LayerNorm
+// (conv16_blocks_rows, conv16_xhat) from the sample's packed observation with the same parameters, two m-blocks
+// (pixels 16 mb .. 16 mb + 15) per call as the forward groups them (one at C = 10), so they are bit for bit what the
+// forward computed.
+// The rebuild's fragment row g is pixel 16 mb + 2g and row g + 8 is pixel 16 mb + 2g + 1, so thread (g, t) holds
+// xhat and rstd of the pixel pair (16 mb + 2g, + 1) -- whose two dz values of a channel are exactly one B word -- in
+// channels 4t .. 4t+3, and runs the LayerNorm backward there, in registers: only dy (one 16-byte load per pixel) and
+// the dz planes go through shared memory.  The rebuild costs the forward's MMAs again (48 at C = 4, 96 at C = 10); it
+// saves 4,352 bytes per sample of HBM writes in the forward and as many reads here.
 // ---------------------------------------------------------------------------------------------------------------
 template <int C>
 struct ConvBwd16 {
   static constexpr int MT = ConvMma<C>::MT;
   static constexpr int NG = 4 * MT;                             // tap groups of 4 per pixel pair
   static constexpr int NGP = (NG % 8 == 4) ? NG : NG + 4;       // pair stride in words: the 4 t-lanes hit distinct banks
-  static constexpr int DY = 0;                                  // [64][16] upstream gradient (swizzled)
-  static constexpr int XH = DY + FLAT_CNN;                      // [16][16] xhat of the m-block phase A is on (swizzled)
-  static constexpr int RS = XH + 16 * CONV_O;                   // [16] its rstd
-  static constexpr int DZT = RS + 16;                           // 2 planes x [16 ch][32 pair words]; aliases the obs row
+  static constexpr int DY = 0;                                  // [64][16] upstream gradient (rows swizzled, dy_off)
+  static constexpr int DZT = DY + FLAT_CNN;                     // 2 planes x [16 ch][32 pair words]; aliases the obs row
   static constexpr int PW = DZT + 2 * CONV_O * 32;              // [32 pairs][NGP] exponent-coded pair words
-  static constexpr int XP = PW + 32 * NGP;                      // [64 pixels][Conv16::ROW] the forward's patch words
-  static constexpr int WARP_FLOATS = (XP + CONV_PIX * Conv16<C>::ROW + 3) / 4 * 4;
+  static constexpr int XP = PW + 32 * NGP;                      // [32 pairs][NGP] the forward's patch words, pair-interleaved
+  static constexpr int WARP_FLOATS = XP + 32 * NGP;
   static constexpr int WARPS = (C == 4) ? 8 : 6;                // keeps two CTAs per SM for the wider observations
   static constexpr int WB = WARPS * WARP_FLOATS;                // the forward's weight fragments, Conv16::KS x 2 x 32 uint4
   static constexpr int BYTES = (WB + Conv16<C>::KS * 2 * 32 * 4 + 6 * CONV_O) * 4;  // + cb, sc, bi[16] + s_red[48]
+  // m-blocks per conv rebuild: two (the training forward's grouping, more MMAs in flight) where the registers allow
+  static constexpr int NBR = (C == 10) ? 1 : 2;
 };
 
-// float offset of (pixel row p, channel column col) in the swizzled [64][16] DY stage (and, with p < 16, the [16][16]
-// xhat stage): the rows 2g of one fragment group would all start on bank 0, so odd (p / 4) swaps the two rows of a pair
-// and odd (p / 2) swaps the column halves -- the four g of a half-warp then cover the 32 banks once
-__device__ __forceinline__ int cswz16(int p, int col) {
-  return ((p ^ ((p >> 2) & 1)) << 4) + (col ^ (((p >> 1) & 1) << 3));
-}
-// word offset of (channel ch, k-step ks, position pos) in a dzT plane [16][32]
+// float offset of the 16-byte chunk (pixel p, channels 4q .. 4q+3) in the [64][16] DY stage: rows 4i+2 and 4i+3 are
+// swapped, so that the even pixels 2g (and the odd ones) that a quarter-warp reads cover the 32 banks once
+__device__ __forceinline__ int dy_off(int p, int q) { return ((p ^ ((p >> 1) & 1)) << 4) + 4 * q; }
+// word offset of (channel ch, k-step ks, position pos) in a dzT plane [16][32].  The k-step block of a channel row is
+// swizzled by (ch / 4) ^ (ch % 4), which differs between the channels 4t + k of a phase-A store (t = 0..3) and between
+// the channels 8h + g of a fragment load (g = 0..3 or 4..7); it sits in bits 3..4, so a thread reaches every block it
+// stores or loads from one base word by XOR-ing a constant
 __device__ __forceinline__ int dzt_word(int ch, int ks, int pos) {
-  const int c7 = ch & 7;
-  return (ch << 5) + ((ks ^ ((c7 + (c7 >> 2)) & 3)) << 3) + pos;
+  return (ch << 5) + ((ks ^ (ch >> 2) ^ (ch & 3)) << 3) + pos;
 }
 
 template <int C>
@@ -1785,8 +1786,6 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
   const int seed = blockIdx.y;
   float* my = smem_bwd + warp * SM::WARP_FLOATS;
   float* my_dy = my + SM::DY;
-  float* my_xh = my + SM::XH;
-  float* my_rs = my + SM::RS;
   uint32_t* my_dzt = reinterpret_cast<uint32_t*>(my + SM::DZT);   // plane 0 = hi, plane 1 = lo: 512 words each
   uint32_t* my_so = reinterpret_cast<uint32_t*>(my + SM::DZT);    // packed obs row: only needed until the patch words exist
   uint32_t* my_pw = reinterpret_cast<uint32_t*>(my + SM::PW);
@@ -1801,6 +1800,7 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
   static_assert(M::MT * 16 * CONV_O <= SM::WARP_FLOATS * SM::WARPS, "dW reduction buffer aliases the warp slices");
   static_assert(Cfg::PW <= 32, "one packed observation word per lane");
   static_assert(SM::XP % 4 == 0 && SM::WB % 4 == 0, "16-byte aligned patch rows and weight fragments");
+  static_assert(SM::NG == 4 * Conv16<C>::KS, "a pixel's patch words are exactly the pair words' tap groups");
   conv16_load_weights<C>(params + (int64_t)seed * P, L, wb, cb, sc, bi, threadIdx.x, blockDim.x);
   if (tid < 3 * CONV_O) s_red[tid] = 0.f;
   __syncthreads();
@@ -1813,7 +1813,16 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
 #pragma unroll
       for (int j = 0; j < 4; ++j) wrun[mt][h][j] = 0.f;
   const uint32_t amask = (1u << (10 + (g & 3))) | (1u << (26 + (g & 3)));
+  // per-lane offsets, computed once: the k-steps and the m-blocks of one rebuild add compile-time constants (or XOR
+  // them, for the dzT swizzle)
   const int pos_g = g < 4 ? 2 * g : 2 * (g - 4) + 1;   // pair g of a k-step sits next to pair g + 4
+  const uint32_t* xpg = my_xp + g * SM::NGP;   // rebuild fragment rows g, g + 8: pixel pair g of each m-block
+  const float* dy0 = my_dy + dy_off(2 * g, t);
+  const float* dy1 = my_dy + dy_off(2 * g + 1, t);
+  // dzt_word(4t + k, mb, pos_g) = (dzs ^ ((k ^ mb) << 3)) + 32 k, dzt_word(8h + g, ks, 2t) = (dzl ^ ((ks ^ 2h) << 3)) + 256 h
+  const int dzs = dzt_word(4 * t, 0, pos_g), dzl = dzt_word(g, 0, 2 * t);
+  const uint32_t* pa = my_pw + t * SM::NGP + 2 * (g >> 2);   // pixel pair 8ks + t: A rows (g, g + 8)
+  const uint32_t* pb = pa + 4 * SM::NGP;                     // pixel pair 8ks + t + 4
 
   const int row_stride = gridDim.x * SM::WARPS;
   // unconditional loads from clamped addresses (rows past the end re-read the last row, lanes past the packed width
@@ -1832,8 +1841,8 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
       const float* dsrc = DY1 + ((int64_t)seed * rows + r) * FLAT_CNN;
 #pragma unroll
       for (int i = 0; i < FLAT_CNN / 4 / 32; ++i) {
-        const int q = i * 32 + lane, prow = q >> 2;              // 16-byte chunk q = (pixel row, column quad)
-        cp_async16(my_dy + cswz16(prow, (q & 3) * 4), dsrc + q * 4);   // the swizzles move whole chunks
+        const int q = i * 32 + lane;                             // 16-byte chunk q = (pixel row, column quad)
+        cp_async16(my_dy + dy_off(q >> 2, q & 3), dsrc + q * 4);
       }
     }
     cp_async_commit();
@@ -1849,12 +1858,22 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
     __syncwarp();
     pre = fetch_obs(src_next);
     src_next = fetch_index(row + 2 * row_stride);
-    store_patch16<C>(my_so, lane, my_xp + lane * Conv16<C>::ROW);   // the forward's patch words, for the xhat rebuild
-    store_patch16<C>(my_so, lane + 32, my_xp + (lane + 32) * Conv16<C>::ROW);
-    {  // exponent-coded pair words of pixel pair `lane`
+    {  // exponent-coded pair words of pixel pair `lane`, and from them the forward's patch words of its two pixels
       uint32_t w0[PWD], w1[PWD];
       patch_bits<C>(my_so, 2 * lane, w0);
       patch_bits<C>(my_so, 2 * lane + 1, w1);
+      uint32_t gw[SM::NG];   // tap group q: taps 4q .. 4q+3 of pixel 2 lane at bits 10..13, of pixel 2 lane + 1 at 26..29
+#pragma unroll
+      for (int q = 0; q < SM::NG; ++q) {
+        const int bit = 4 * q, wi = bit >> 5, sh = bit & 31;
+        gw[q] = 0u;
+        if (wi < PWD) {
+          const uint32_t v0 = w0[wi < PWD ? wi : 0], v1 = w1[wi < PWD ? wi : 0];
+          const uint32_t lo = sh >= 10 ? v0 >> (sh >= 10 ? sh - 10 : 0) : v0 << (sh < 10 ? 10 - sh : 0);
+          const uint32_t hi = sh <= 26 ? v1 << (sh <= 26 ? 26 - sh : 0) : v1 >> (sh > 26 ? sh - 26 : 0);
+          gw[q] = __byte_perm(lo, hi, 0x7610);
+        }
+      }
       uint32_t pw[SM::NGP];
 #pragma unroll
       for (int k = 0; k < SM::NGP; ++k) pw[k] = 0u;
@@ -1862,87 +1881,95 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
       for (int q = 0; q < SM::NG; ++q) {
         // memory order inside an m-tile: groups (0, 2, 1, 3), so the words of fragment rows g and g + 8 are adjacent
         const int ql = q & 3, slot = (q & ~3) + (ql == 1 ? 2 : (ql == 2 ? 1 : ql));
-        const int bit = 4 * q, wi = bit >> 5, sh = bit & 31;
-        if (wi < PWD) {
-          const uint32_t v0 = w0[wi < PWD ? wi : 0], v1 = w1[wi < PWD ? wi : 0];
-          const uint32_t lo = sh >= 10 ? v0 >> (sh >= 10 ? sh - 10 : 0) : v0 << (sh < 10 ? 10 - sh : 0);
-          const uint32_t hi = sh <= 26 ? v1 << (sh <= 26 ? 26 - sh : 0) : v1 >> (sh > 26 ? sh - 26 : 0);
-          pw[slot] = __byte_perm(lo, hi, 0x7610);
-        }
+        pw[slot] = gw[q];
       }
       uint32_t* dstw = my_pw + lane * SM::NGP;
 #pragma unroll
       for (int k = 0; k < SM::NGP / 4; ++k)
         *reinterpret_cast<uint4*>(dstw + 4 * k) = make_uint4(pw[4 * k], pw[4 * k + 1], pw[4 * k + 2], pw[4 * k + 3]);
+      // the forward's patch word of byte b of a pixel holds taps 8b .. 8b+3 at bits 10..13 and 8b+4 .. 8b+7 at 26..29
+      // (build_patch16): groups 2b and 2b+1, the low halves of their pair words for pixel 2 lane, the high halves for
+      // 2 lane + 1.  Row `lane` of XP: per k-step s (bytes 2s, 2s+1) pixel 2 lane's two words, then 2 lane + 1's.
+      uint32_t* dstx = my_xp + lane * SM::NGP;
+#pragma unroll
+      for (int s = 0; s < Conv16<C>::KS; ++s)
+        *reinterpret_cast<uint4*>(dstx + 4 * s) =
+            make_uint4(__byte_perm(gw[4 * s], gw[4 * s + 1], 0x5410), __byte_perm(gw[4 * s + 2], gw[4 * s + 3], 0x5410),
+                       __byte_perm(gw[4 * s], gw[4 * s + 1], 0x7632), __byte_perm(gw[4 * s + 2], gw[4 * s + 3], 0x7632));
     }
     cp_async_wait_all();
     __syncwarp();
-    // ---- phase A: LayerNorm backward of the pixel pair (16 mb + 2g, + 1); dz * gs -> fp16 (hi, lo) planes
-#pragma unroll 1
-    for (int mb = 0; mb < 4; ++mb) {
-      {  // xhat / rstd of m-block mb, rebuilt as the forward computed them, into the [16][16] stage
-        float zc[1][2][4], x0[4], x1[4], rs0, rs1;
-        conv16_blocks<C, 1>(my_xp, wb, cb, mb, lane, zc);
-        conv16_xhat(zc[0], x0, x1, rs0, rs1);
-        __syncwarp();   // phase A of the previous m-block is done with the stage
-        *reinterpret_cast<float4*>(my_xh + cswz16(g, 4 * t)) = make_float4(x0[0], x0[1], x0[2], x0[3]);
-        *reinterpret_cast<float4*>(my_xh + cswz16(g + 8, 4 * t)) = make_float4(x1[0], x1[1], x1[2], x1[3]);
-        if (t == 0) { my_rs[g] = rs0; my_rs[g + 8] = rs1; }
-        __syncwarp();
-      }
-      const int p0 = 16 * mb + 2 * g, p1 = p0 + 1;
-      float z[2][4];
-      float2 dyv[2][2];
+    // ---- phase A: LayerNorm backward of the pixel pair (16 mb + 2g, + 1) in channels 4t .. 4t+3; dz * gs -> fp16
+    // (hi, lo) planes.  Every rounding is the one the former [pixel pair][channels 2t, 2t+1, 8+2t, 9+2t] layout made,
+    // and the per-channel sums add the same pixels in the same order, so dz and all gradients keep their bits.
+#pragma unroll 1   // unrolled, ptxas hoists the next rebuild's loads and spills
+    for (int mp = 0; mp < 4 / SM::NBR; ++mp) {
+      float zc[SM::NBR][2][4];
+      const float4 cbv = *reinterpret_cast<const float4*>(cb + 4 * t);   // conv bias of channels 4t .. 4t+3
+      const float cb4[4] = {cbv.x, cbv.y, cbv.z, cbv.w};
+      conv16_blocks_rows<C, SM::NBR, 8 * SM::NGP, true>(xpg + 8 * SM::NBR * mp * SM::NGP, nullptr, wb, cb4, lane, zc);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        dyv[h][0] = *reinterpret_cast<const float2*>(my_dy + cswz16(p0, 8 * h + 2 * t));
-        dyv[h][1] = *reinterpret_cast<const float2*>(my_dy + cswz16(p1, 8 * h + 2 * t));
-        const float2 a0 = *reinterpret_cast<const float2*>(my_xh + cswz16(2 * g, 8 * h + 2 * t));
-        const float2 a1 = *reinterpret_cast<const float2*>(my_xh + cswz16(2 * g + 1, 8 * h + 2 * t));
-        z[h][0] = a0.x; z[h][1] = a0.y; z[h][2] = a1.x; z[h][3] = a1.y;
-      }
-      // rstd * gs: dz comes out pre-scaled for the fp16 planes (gs is a power of two; the conv-bias sum is unscaled at
-      // the end), which saves a multiplication per element
-      const float rstd0 = my_rs[2 * g] * gs, rstd1 = my_rs[2 * g + 1] * gs;
-      float dxh[2][4];
-      float m1a = 0.f, m2a = 0.f, m1b = 0.f, m2b = 0.f;
+      for (int i = 0; i < SM::NBR; ++i) {
+        const int mb = SM::NBR * mp + i;
+        float x[2][4], rs[2];   // [pixel 16 mb + 2g + p][channel 4t + k]
+        conv16_xhat(zc[i], x[0], x[1], rs[0], rs[1]);
+        const float4 d0 = *reinterpret_cast<const float4*>(dy0 + 256 * mb);
+        const float4 d1 = *reinterpret_cast<const float4*>(dy1 + 256 * mb);
+        const float dy[2][4] = {{d0.x, d0.y, d0.z, d0.w}, {d1.x, d1.y, d1.z, d1.w}};
+        const float4 scv = *reinterpret_cast<const float4*>(sc + 4 * t);   // LayerNorm scale of channels 4t .. 4t+3
+        const float sc4[4] = {scv.x, scv.y, scv.z, scv.w};
+        float dxh[2][4];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int o = 8 * h + 2 * t;
-        const float dy4[4] = {dyv[h][0].x, dyv[h][0].y, dyv[h][1].x, dyv[h][1].y};
+        for (int p = 0; p < 2; ++p)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int col = 2 * h + (j & 1);
-          a_dsc[col] = fmaf(dy4[j], z[h][j], a_dsc[col]);
-          a_dbi[col] += dy4[j];
-          dxh[h][j] = dy4[j] * sc[o + (j & 1)];
-          if (j < 2) { m1a += dxh[h][j]; m2a = fmaf(dxh[h][j], z[h][j], m2a); }
-          else { m1b += dxh[h][j]; m2b = fmaf(dxh[h][j], z[h][j], m2b); }
+          for (int k = 0; k < 4; ++k) {
+            a_dsc[k] = fmaf(dy[p][k], x[p][k], a_dsc[k]);
+            a_dbi[k] = __fadd_rn(a_dbi[k], dy[p][k]);
+            dxh[p][k] = __fmul_rn(dy[p][k], sc4[k]);
+          }
+        // m1 = sum_ch dxh, m2 = sum_ch dxh * xhat over the 16 channels of each pixel, associated as
+        // (P0 + P1) + (P2 + P3) with P_u = ((ch 2u + ch 2u+1) + ch 8+2u) + ch 9+2u: lanes 0, 1 start the chains of
+        // their channel pairs, lanes 2, 3 (channels 8 .. 15) continue them, add P_2v + P_2v+1 and swap the result
+        float m1[2], m2[2];
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+          float s1[2], s2[2];
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            s1[j] = __fadd_rn(__fadd_rn(0.f, dxh[p][2 * j]), dxh[p][2 * j + 1]);
+            s2[j] = fmaf(dxh[p][2 * j + 1], x[p][2 * j + 1], fmaf(dxh[p][2 * j], x[p][2 * j], 0.f));
+          }
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const float r1 = __shfl_xor_sync(0xffffffffu, s1[j], 2), r2 = __shfl_xor_sync(0xffffffffu, s2[j], 2);
+            s1[j] = __fadd_rn(__fadd_rn(r1, dxh[p][2 * j]), dxh[p][2 * j + 1]);
+            s2[j] = fmaf(dxh[p][2 * j + 1], x[p][2 * j + 1], fmaf(dxh[p][2 * j], x[p][2 * j], r2));
+          }
+          float q1 = __fadd_rn(s1[0], s1[1]), q2 = __fadd_rn(s2[0], s2[1]);
+          q1 = __fadd_rn(q1, __shfl_xor_sync(0xffffffffu, q1, 1));
+          q2 = __fadd_rn(q2, __shfl_xor_sync(0xffffffffu, q2, 1));
+          m1[p] = __shfl_sync(0xffffffffu, q1, lane | 2);
+          m2[p] = __fmul_rn(__shfl_sync(0xffffffffu, q2, lane | 2), 1.0f / CONV_O);
         }
-      }
+        // dz = rstd gs (dxh - m1 / 16 - xhat m2 / 16): rstd * gs makes dz come out pre-scaled for the fp16 planes (gs
+        // is a power of two; the conv-bias sum is unscaled at the end)
+        float dz[2][4];
 #pragma unroll
-      for (int o = 1; o <= 2; o <<= 1) {
-        m1a += __shfl_xor_sync(0xffffffffu, m1a, o); m2a += __shfl_xor_sync(0xffffffffu, m2a, o);
-        m1b += __shfl_xor_sync(0xffffffffu, m1b, o); m2b += __shfl_xor_sync(0xffffffffu, m2b, o);
-      }
-      m1a *= (1.0f / CONV_O); m2a *= (1.0f / CONV_O); m1b *= (1.0f / CONV_O); m2b *= (1.0f / CONV_O);
+        for (int p = 0; p < 2; ++p) {
+          const float rsg = __fmul_rn(rs[p], gs);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float dzv[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float rstd = j < 2 ? rstd0 : rstd1, m1 = j < 2 ? m1a : m1b, m2 = j < 2 ? m2a : m2b;
-          dzv[j] = rstd * (dxh[h][j] - m1 - z[h][j] * m2);
-          a_dcb[2 * h + (j & 1)] += dzv[j];
+          for (int k = 0; k < 4; ++k) {
+            dz[p][k] = __fmul_rn(rsg, fmaf(-x[p][k], m2[p], fmaf(m1[p], -1.0f / CONV_O, dxh[p][k])));
+            a_dcb[k] = __fadd_rn(a_dcb[k], dz[p][k]);
+          }
         }
-        // B words: (pixel p0, pixel p1) of channel o (j = 0, 2) and of channel o + 1 (j = 1, 3); k-step mb, pair g
+        // B words: (pixel 16 mb + 2g, + 1) of channel 4t + k; k-step mb, pair g
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const float v0 = dzv[c], v1 = dzv[2 + c];
-          const uint32_t hw = cvt_f16x2_satfinite(v0, v1);
+        for (int k = 0; k < 4; ++k) {
+          const uint32_t hw = cvt_f16x2_satfinite(dz[0][k], dz[1][k]);
           const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw));
-          const __half2 lw = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
-          const int wd = dzt_word(8 * h + 2 * t + c, mb, pos_g);
+          const __half2 lw = __floats2half2_rn(dz[0][k] - hf.x, dz[1][k] - hf.y);
+          const int wd = (dzs ^ ((k ^ mb) << 3)) + 32 * k;
           my_dzt[wd] = hw;
           my_dzt[CONV_O * 32 + wd] = *reinterpret_cast<const uint32_t*>(&lw);
         }
@@ -1958,23 +1985,22 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int j = 0; j < 4; ++j) wacc[mt][h][j] = 0.f;
-#pragma unroll 1
+#pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
       // B fragments: b0 = dz[pixels 16ks + 2t, + 1][o = 8h + g], b1 = the same of pixels + 8: one LDS.64 per plane
       uint2 bhi[2], blo[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int wd = dzt_word(8 * h + g, ks, 2 * t);
+        const int wd = (dzl ^ ((ks ^ 2 * h) << 3)) + 256 * h;
         bhi[h] = *reinterpret_cast<const uint2*>(my_dzt + wd);
         blo[h] = *reinterpret_cast<const uint2*>(my_dzt + CONV_O * 32 + wd);
       }
-      const uint32_t* pa = my_pw + (8 * ks + t) * SM::NGP + 2 * (g >> 2);   // pixel pair 8ks + t: rows (g, g + 8)
-      const uint32_t* pb = pa + 4 * SM::NGP;                               // pixel pair 8ks + t + 4
 #pragma unroll
       for (int mt = 0; mt < M::MT; ++mt) {
-        const uint2 wa = *reinterpret_cast<const uint2*>(pa + 4 * mt), wb = *reinterpret_cast<const uint2*>(pb + 4 * mt);
+        const uint2 wa = *reinterpret_cast<const uint2*>(pa + 8 * ks * SM::NGP + 4 * mt);
+        const uint2 wb2 = *reinterpret_cast<const uint2*>(pb + 8 * ks * SM::NGP + 4 * mt);
         uint32_t a[4];
-        a[0] = wa.x & amask; a[1] = wa.y & amask; a[2] = wb.x & amask; a[3] = wb.y & amask;
+        a[0] = wa.x & amask; a[1] = wa.y & amask; a[2] = wb2.x & amask; a[3] = wb2.y & amask;
         // lo pass of both column halves, then the hi pass: no back-to-back MMAs on one accumulator
         mma_f16_16n8k16(wacc[mt][0], a, blo[0].x, blo[0].y);
         mma_f16_16n8k16(wacc[mt][1], a, blo[1].x, blo[1].y);
@@ -2010,25 +2036,27 @@ __global__ void __launch_bounds__(ConvBwd16<C>::WARPS * 32, 2)
     }
     __syncthreads();
   }
+  // per-channel sums: lanes with the same t hold the same channels 4t .. 4t+3 -> xor-shuffle tree over g (fixed),
+  // then warps in order
 #pragma unroll
-  for (int col = 0; col < 4; ++col) {
-    float v0 = a_dsc[col], v1 = a_dbi[col], v2 = a_dcb[col];
+  for (int k = 0; k < 4; ++k) {
+    float v0 = a_dsc[k], v1 = a_dbi[k], v2 = a_dcb[k];
 #pragma unroll
     for (int sft = 4; sft <= 16; sft <<= 1) {
       v0 += __shfl_xor_sync(0xffffffffu, v0, sft);
       v1 += __shfl_xor_sync(0xffffffffu, v1, sft);
       v2 += __shfl_xor_sync(0xffffffffu, v2, sft);
     }
-    a_dsc[col] = v0; a_dbi[col] = v1; a_dcb[col] = v2;
+    a_dsc[k] = v0; a_dbi[k] = v1; a_dcb[k] = v2;
   }
   for (int w = 0; w < SM::WARPS; ++w) {
     if (warp == w && g == 0) {
 #pragma unroll
-      for (int col = 0; col < 4; ++col) {
-        const int o = 8 * (col >> 1) + 2 * t + (col & 1);
-        s_red[o] = (w == 0 ? 0.f : s_red[o]) + a_dsc[col];
-        s_red[CONV_O + o] = (w == 0 ? 0.f : s_red[CONV_O + o]) + a_dbi[col];
-        s_red[2 * CONV_O + o] = (w == 0 ? 0.f : s_red[2 * CONV_O + o]) + a_dcb[col] * inv_gs;
+      for (int k = 0; k < 4; ++k) {
+        const int o = 4 * t + k;
+        s_red[o] = (w == 0 ? 0.f : s_red[o]) + a_dsc[k];
+        s_red[CONV_O + o] = (w == 0 ? 0.f : s_red[CONV_O + o]) + a_dbi[k];
+        s_red[2 * CONV_O + o] = (w == 0 ? 0.f : s_red[2 * CONV_O + o]) + a_dcb[k] * inv_gs;
       }
     }
     __syncthreads();
