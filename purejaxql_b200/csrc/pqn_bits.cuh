@@ -24,7 +24,7 @@
 namespace bits {
 
 constexpr int KC = 8;                            // k-steps per MMA accumulation chain (forward)
-constexpr int FWD_WARPS = 4, FWD_ROWS = 32 * FWD_WARPS, FWD_COLS = 64;   // forward CTA tile: 128 rows x 64 columns
+constexpr int FWD_WARPS = 4, FWD_ROWS = 32 * FWD_WARPS;   // forward CTA tile: 128 rows x 8 * NT columns
 constexpr int WG_ROWS = 64;                      // rows (4 k-steps) per staged chunk of the weight gradient
 constexpr int WG_FEAT = 128;                     // features per weight-gradient CTA
 constexpr int CNT_BLOCKS = 64;                   // row chunks per seed of the two-stage popcount
@@ -71,27 +71,30 @@ __global__ void wfrag_kernel(const float* __restrict__ params, int64_t P, int64_
   wf[(int64_t)seed * n_per + i] = make_uint4(h2u(h0), h2u(h1), h2u(l0), h2u(l1));
 }
 
-// Z[s][r][n0 .. n0+63] = bits(row r) . W0' + bias.  CTA = 4 warps; its 64-column slice of the B fragments (all k-steps)
-// stays in shared memory while the CTA walks row tiles of 128 (grid-stride); warp = 32 rows x 64 columns.
-// grid = (row-tile CTAs, H / 64, S), dynamic shared memory fwd_smem(KS)
+// Z[s][r][n0 .. n0+8NT-1] = bits(row r) . W0' + bias.  CTA = 4 warps; its 8NT-column slice of the B fragments (all
+// k-steps) stays in shared memory while the CTA walks row tiles of 128 (grid-stride); warp = 32 rows x 8NT columns.
+// NT = 8 (64 columns) up to 44 k-steps (D = 700); NT = 4 (32 columns) at D = 1000, whose 63 k-steps of 64-column B
+// fragments (252 KB) would not fit in shared memory.  Same MMA chains and fp32 adds per column either way.
+// grid = (row-tile CTAs, H / (8NT), S), dynamic shared memory fwd_smem(KS, NT)
+template <int NT>
 __global__ void __launch_bounds__(FWD_WARPS * 32, 1)
     fwd_kernel(const uint32_t* __restrict__ obs, int64_t orps, const int32_t* __restrict__ gather, int rows, int D,
                int KS, const uint4* __restrict__ wf, int H, const float* __restrict__ bias, int64_t bias_stride,
                const uint32_t* __restrict__ flip, float* __restrict__ Z) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint4* sB = reinterpret_cast<uint4*>(smem_raw);                      // [KS][8 n-tiles][32 lanes]
-  uint2* sA = reinterpret_cast<uint2*>(sB + (int64_t)KS * 256);        // [128 rows][LDA] spread k-chunks
+  uint2* sA = reinterpret_cast<uint2*>(sB + (int64_t)KS * NT * 32);    // [128 rows][LDA] spread k-chunks
   const int LDA = KS | 1;                                              // odd: conflict-free fragment loads
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
-  const int seed = blockIdx.z, nt0 = blockIdx.y * (FWD_COLS / 8);
+  const int seed = blockIdx.z, nt0 = blockIdx.y * NT;
   const int PW = packed_words(D);
   const uint4* __restrict__ wsrc = wf + (int64_t)seed * KS * (H / 8) * 32;
-  for (int i = tid; i < KS * 256; i += blockDim.x)
-    sB[i] = __ldg(wsrc + ((int64_t)(i >> 8) * (H / 8) + nt0 + ((i >> 5) & 7)) * 32 + (i & 31));
+  for (int i = tid; i < KS * NT * 32; i += blockDim.x)
+    sB[i] = __ldg(wsrc + ((int64_t)(i / (NT * 32)) * (H / 8) + nt0 + ((i >> 5) % NT)) * 32 + (i & 31));
   const float* __restrict__ bv = bias + (int64_t)seed * bias_stride + nt0 * 8;
-  float2 bcol[8];
+  float2 bcol[NT];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) bcol[j] = make_float2(bv[8 * j + 2 * t], bv[8 * j + 2 * t + 1]);
+  for (int j = 0; j < NT; ++j) bcol[j] = make_float2(bv[8 * j + 2 * t], bv[8 * j + 2 * t + 1]);
 
   for (int r0 = blockIdx.x * FWD_ROWS; r0 < rows; r0 += gridDim.x * FWD_ROWS) {
     __syncthreads();   // sB is loaded / the previous tile's sA is consumed
@@ -120,20 +123,20 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, 1)
       }
     }
     __syncthreads();
-    float tot[2][8][4];
+    float tot[2][NT][4];
 #pragma unroll
     for (int m = 0; m < 2; ++m)
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
+      for (int j = 0; j < NT; ++j)
 #pragma unroll
         for (int q = 0; q < 4; ++q) tot[m][j][q] = 0.f;
     const uint2* __restrict__ arow = sA + (warp * 32 + g) * LDA;
     for (int c0 = 0; c0 < KS; c0 += KC) {
-      float acc[2][8][4];
+      float acc[2][NT][4];
 #pragma unroll
       for (int m = 0; m < 2; ++m)
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int j = 0; j < NT; ++j)
 #pragma unroll
           for (int q = 0; q < 4; ++q) acc[m][j][q] = 0.f;
       const int c1 = min(KS, c0 + KC);
@@ -142,8 +145,8 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, 1)
 #pragma unroll
         for (int m = 0; m < 2; ++m) a_frag(arow[(16 * m) * LDA + ks], arow[(16 * m + 8) * LDA + ks], t, alo[m], ahi[m]);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 b = sB[(ks * 8 + j) * 32 + lane];
+        for (int j = 0; j < NT; ++j) {
+          const uint4 b = sB[(ks * NT + j) * 32 + lane];
 #pragma unroll
           for (int m = 0; m < 2; ++m) {
             mma_f16_16n8k16(acc[m][j], ahi[m], b.x, b.y);
@@ -154,7 +157,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, 1)
 #pragma unroll
       for (int m = 0; m < 2; ++m)
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int j = 0; j < NT; ++j)
 #pragma unroll
           for (int q = 0; q < 4; ++q) tot[m][j][q] += acc[m][j][q];
     }
@@ -162,7 +165,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, 1)
     for (int m = 0; m < 2; ++m) {
       const int row = r0 + warp * 32 + 16 * m + g;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < NT; ++j) {
         const int col = (nt0 + j) * 8 + 2 * t;
         if (row < rows)
           *reinterpret_cast<float2*>(Z + ((int64_t)seed * rows + row) * H + col) =
@@ -174,7 +177,10 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, 1)
     }
   }
 }
-static size_t fwd_smem(int KS) { return (size_t)KS * 256 * sizeof(uint4) + (size_t)FWD_ROWS * (KS | 1) * sizeof(uint2); }
+static size_t fwd_smem(int KS, int NT) {
+  return (size_t)KS * NT * 32 * sizeof(uint4) + (size_t)FWD_ROWS * (KS | 1) * sizeof(uint2);
+}
+static int fwd_ntiles(int KS) { return fwd_smem(KS, 8) <= 227u * 1024u ? 8 : 4; }
 
 // G[f][n] = sum_r bit[r][f] * dz[r][n] over this CTA's row split, for 128 features x BNC columns: the bits of a 64-row
 // chunk are transposed to feature-major spread words with warp ballots, dz * gscale is split into fp16 (hi, lo') B
@@ -476,16 +482,17 @@ static void launch_wfrag(const float* params, int64_t P, int64_t off_w, const fl
 // Z[S][rows][H] = bits . Dense_0' + bias (bias + seed * bias_stride, [H])
 static int launch_fwd(const uint32_t* obs, int64_t orps, const int32_t* gather, int rows, int D, int H, const uint4* wf,
                       const float* bias, int64_t bias_stride, const uint32_t* flip, float* Z, int S, cudaStream_t st) {
-  const int KS = ksteps(D);
-  const size_t sm = fwd_smem(KS);
-  if (cudaFuncSetAttribute(fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm) != cudaSuccess)
+  const int KS = ksteps(D), NT = fwd_ntiles(KS);
+  const size_t sm = fwd_smem(KS, NT);
+  auto kfn = NT == 8 ? fwd_kernel<8> : fwd_kernel<4>;
+  if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm) != cudaSuccess)
     return check_launch("bits fwd(cudaFuncSetAttribute)");
-  const int tiles = (rows + FWD_ROWS - 1) / FWD_ROWS, slices = H / FWD_COLS;
+  const int tiles = (rows + FWD_ROWS - 1) / FWD_ROWS, slices = H / (8 * NT);
   int per = (device_sm_count() + slices * S - 1) / (slices * S);   // one CTA per SM over all seeds and slices
   if (per > tiles) per = tiles;
   if (per < 1) per = 1;
   LaunchScope _ls(K_BITS_FWD, st);
-  fwd_kernel<<<dim3(per, slices, S), FWD_WARPS * 32, sm, st>>>(obs, orps, gather, rows, D, KS, wf, H, bias, bias_stride, flip, Z);
+  kfn<<<dim3(per, slices, S), FWD_WARPS * 32, sm, st>>>(obs, orps, gather, rows, D, KS, wf, H, bias, bias_stride, flip, Z);
   return 0;
 }
 

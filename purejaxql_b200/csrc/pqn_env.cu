@@ -21,6 +21,7 @@
 #include "env_classic.cuh"
 #include "env_minatar_more.cuh"
 #include "env_misc.cuh"
+#include "env_seaquest.cuh"
 #include "rollout_logic.cuh"
 
 namespace pqn {
@@ -384,6 +385,7 @@ static void fill_info(pqn_env_info_t* o) {
     case ENV_ASTERIX: { using EnvT = AsterixEnv; __VA_ARGS__; } break;          \
     case ENV_FREEWAY: { using EnvT = FreewayEnv; __VA_ARGS__; } break;          \
     case ENV_SPACE_INVADERS: { using EnvT = SpaceInvadersEnv; __VA_ARGS__; } break; \
+    case ENV_SEAQUEST: { using EnvT = SeaquestEnv; __VA_ARGS__; } break;        \
     case ENV_CARTPOLE: { using EnvT = CartPoleEnv; __VA_ARGS__; } break;        \
     case ENV_ACROBOT: { using EnvT = AcrobotEnv; __VA_ARGS__; } break;          \
     case ENV_MOUNTAIN_CAR: { using EnvT = MountainCarEnv; __VA_ARGS__; } break; \

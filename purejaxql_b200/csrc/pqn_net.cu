@@ -118,9 +118,9 @@ static int check_desc(const pqn_net_desc_t* d, const char* who) {
     return PQN_OK;
   }
   if (d->kind == PQN_NET_MLP_BITS) {
-    if (d->in_c != 400 && d->in_c != 600 && d->in_c != 700)
+    if (d->in_c != 400 && d->in_c != 600 && d->in_c != 700 && d->in_c != 1000)
       return set_error(PQN_E_UNSUPPORTED, "%s: MLP on packed MinAtar observations with in_c=%d (100 * C: 400, 600 or 700 "
-                       "built)", who, d->in_c);
+                       "built, and 1000 for Seaquest)", who, d->in_c);
     return PQN_OK;
   }
   if (d->kind == PQN_NET_MLP || d->kind == PQN_NET_RNN) {

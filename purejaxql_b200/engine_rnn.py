@@ -27,7 +27,7 @@ from .networks import NET_RNN, QNetworkSpec
 
 class PQNRnnEngine(EngineBase):
     def __init__(self, config: dict, device=None, env_params: envs.EnvParams | None = None):
-        if config["ENV_NAME"] in envs.MINATAR_GAMES:                 # its memory buffer stores float observation rows
+        if config["ENV_NAME"] in envs.MINATAR_GAMES + envs.MINATAR_UNREGISTERED:                 # its memory buffer stores float observation rows
             raise NotImplementedError("the recurrent script is built for the float-observation envs "
                                       "(classic control, MemoryChain-bsuite)")
         super().__init__(config, True, device, env_params)           # env_params: MemoryChain's memory_length (:134-136)

@@ -29,6 +29,7 @@ ENV_IDS = {
     "Asterix-MinAtar": 1,
     "SpaceInvaders-MinAtar": 2,
     "Freeway-MinAtar": 3,
+    "Seaquest-MinAtar": 4,
     "CartPole-v1": 16,
     "Acrobot-v1": 17,
     "MountainCar-v0": 18,
@@ -45,9 +46,16 @@ ENV_IDS = {
 }
 # float-observation envs whose gymnax observation is 2-D although pqn_env_info's (rows, cols) = (1, 1) cannot say so
 _2D_OBS = {"SimpleBandit-bsuite"}
-# PQN_ENV_SEAQUEST (4) is reserved in include/pqn_b200.h but not built: gymnax 0.0.6 (the reference's pin) does not
-# register "Seaquest-MinAtar" in gymnax.make either (DESIGN.md section 8), so the reference cannot run it.
+# the MinAtar games gymnax 0.0.6 (the reference's pin) registers in gymnax.make
 MINATAR_GAMES = ("Breakout-MinAtar", "Asterix-MinAtar", "SpaceInvaders-MinAtar", "Freeway-MinAtar")
+# MinAtar games built here that gymnax 0.0.6 does not register (DESIGN.md section 8): restated from MinAtar itself
+MINATAR_UNREGISTERED = ("Seaquest-MinAtar",)
+# Seaquest-MinAtar's lists (bullets, fish, subs, divers): (capacity, first state word, entry fields)
+_SQ_LISTS = (("f_bullets", 2, 4, ("x", "y", "lr")), ("e_fish", 8, 5, ("x", "y", "lr", "move_timer")),
+             ("e_subs", 8, 9, ("x", "y", "lr", "move_timer", "shot_timer")),
+             ("e_bullets", 8, 13, ("x", "y", "lr")), ("divers", 4, 17, ("x", "y", "lr", "move_timer")))
+_SQ_FIELD_BITS = {"x": (0, 15), "y": (4, 15), "lr": (8, 1), "move_timer": (9, 7), "shot_timer": (12, 15)}
+_SQ_LEN_BITS = {"f_bullets": (0, 3), "e_fish": (2, 15), "e_subs": (6, 15), "e_bullets": (10, 15), "divers": (14, 7)}
 
 LOG_FIELDS = ("episode_returns", "episode_lengths", "returned_episode_returns",
               "returned_episode_lengths", "timestep")
@@ -145,6 +153,31 @@ def state_to_fields(env_name: str, state: torch.Tensor) -> dict:
             bits = (words[p >> 5] >> (p & 31).unsqueeze(1)) & 1
             f[name] = bits.t().reshape(n, 10, 10).to(torch.int32)
         core = 14
+    elif env_name == "Seaquest-MinAtar":
+        w, w1, w2 = st[0], st[1], st[2]
+        f["sub_x"] = w & 15
+        f["sub_y"] = (w >> 4) & 15
+        f["sub_or"] = ((w >> 8) & 1).bool()
+        f["shot_timer"] = (w >> 9) & 7
+        f["diver_count"] = (w >> 12) & 7
+        f["surface"] = ((w >> 15) & 1).bool()
+        f["terminal"] = ((w >> 16) & 1).bool()
+        f["move_speed"] = (w >> 17) & 7
+        f["ramp_index"] = (w >> 20) & 31
+        f["oxygen"] = (w1 & 255) - 1
+        f["e_spawn_speed"] = (w1 >> 8) & 31
+        f["e_spawn_timer"] = (w1 >> 13) & 31
+        f["d_spawn_timer"] = (w1 >> 18) & 63
+        f["time"] = st[3]
+        for name, cap, w0, fields in _SQ_LISTS:
+            sh, m = _SQ_LEN_BITS[name]
+            f["n_" + name] = (w2 >> sh) & m
+            ents = []
+            for k in range(cap):
+                v = (st[w0 + k // 2] >> (16 * (k % 2))) & 0xFFFF
+                ents.append(torch.stack([(v >> _SQ_FIELD_BITS[c][0]) & _SQ_FIELD_BITS[c][1] for c in fields], -1))
+            f[name] = torch.stack(ents, 1)                                  # [N, capacity, fields], zero past n_<name>
+        core = 19
     elif env_name == "CartPole-v1":
         for j, k in enumerate(("x", "x_dot", "theta", "theta_dot")):
             f[k] = _u2f(st[j])
@@ -305,6 +338,24 @@ def fields_to_state(env_name: str, f: dict) -> torch.Tensor:
                 sh = torch.arange(hi - lo, device=bm.device)
                 v = (bm[:, lo:hi] << sh).sum(1)
                 core.append(torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32))
+    elif env_name == "Seaquest-MinAtar":
+        w = (i32(f["sub_x"]) | (i32(f["sub_y"]) << 4) | (i32(f["sub_or"]) << 8) | (i32(f["shot_timer"]) << 9)
+             | (i32(f["diver_count"]) << 12) | (i32(f["surface"]) << 15) | (i32(f["terminal"]) << 16)
+             | (i32(f["move_speed"]) << 17) | (i32(f["ramp_index"]) << 20))
+        w1 = ((i32(f["oxygen"]) + 1) | (i32(f["e_spawn_speed"]) << 8) | (i32(f["e_spawn_timer"]) << 13)
+              | (i32(f["d_spawn_timer"]) << 18))
+        w2 = torch.zeros_like(w)
+        words = []
+        for name, cap, _, fields in _SQ_LISTS:
+            w2 = w2 | (i32(f["n_" + name]) << _SQ_LEN_BITS[name][0])
+            ent = i32(f[name])
+            for k in range(0, cap, 2):
+                v = torch.zeros_like(w)
+                for h in range(2):
+                    for j, c in enumerate(fields):
+                        v = v | (ent[:, k + h, j] << (_SQ_FIELD_BITS[c][0] + 16 * h))
+                words.append(v)
+        core = [w, w1, w2, i32(f["time"])] + words
     elif env_name == "CartPole-v1":
         core = [_f2u(torch.as_tensor(f[k])) for k in ("x", "x_dot", "theta", "theta_dot")] + [i32(f["time"])]
     elif env_name == "Acrobot-v1":

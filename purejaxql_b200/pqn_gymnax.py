@@ -3,6 +3,7 @@ purejaxql/pqn_gymnax.py.
 
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole NUM_SEEDS=8
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=Breakout-MinAtar
+    python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=Seaquest-MinAtar
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=MountainCar-v0
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=Catch-bsuite
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=DeepSea-bsuite
@@ -13,7 +14,8 @@ Every env of ``envs.ENV_IDS`` runs with its gymnax default ``EnvParams``: CartPo
 (200 steps), MemoryChain-bsuite, Catch-bsuite (its 10 x 5 board flattened to 50 inputs), DeepSea-bsuite (its 8 x 8
 board flattened to 64 inputs), UmbrellaChain-bsuite, DiscountingChain-bsuite (5 actions), SimpleBandit-bsuite (one
 constant input, 11 actions: HIDDEN_SIZE 512 is refused), BernoulliBandit-misc, GaussianBandit-misc, FourRooms-misc,
-MetaMaze-misc and the MinAtar games.
+MetaMaze-misc and the MinAtar games (Seaquest-MinAtar included: restated from MinAtar, as gymnax 0.0.6 does not
+register it; its board flattens to 1000 inputs).
 
 On a MinAtar game the flattened (10,10,C) observation feeds the MLP as in the reference; the rollout keeps it as
 packed bits and Dense_0 reads those directly (PQN_NET_MLP_BITS).

@@ -1,6 +1,11 @@
 """PQN on MinAtar with the CNN Q-network — drop-in for purejaxql/pqn_minatar.py.
 
     python -m purejaxql_b200.pqn_minatar +alg=pqn_minatar alg.ENV_NAME=Breakout-MinAtar NUM_SEEDS=16
+    python -m purejaxql_b200.pqn_minatar +alg=pqn_minatar alg.ENV_NAME=Seaquest-MinAtar NUM_SEEDS=4
+
+Runs the four MinAtar games gymnax registers (``envs.MINATAR_GAMES``) and Seaquest-MinAtar, which gymnax 0.0.6 does
+not register and which is restated here from MinAtar's own game (``envs.MINATAR_UNREGISTERED``; 10 channels, 6
+actions).
 
 ``make_train(config)`` keeps the reference's contract (pqn_minatar.py:89-431):
 it mutates ``config`` (NUM_UPDATES, NUM_UPDATES_DECAY, TEST_NUM_STEPS), asserts
