@@ -18,13 +18,15 @@ Appendix B) and sequences the launches:
 """
 from __future__ import annotations
 
+import dataclasses
+import os
 from types import SimpleNamespace
 
 import numpy as np
 import torch
 
-from . import _lib, envs, jaxrandom as jr, sweep
-from .networks import NET_CNN, NET_MLP, NET_MLP_BITS, QNetworkSpec
+from . import _lib, envs, jaxrandom as jr, state as runstate, sweep
+from .networks import NET_CNN, NET_MLP, NET_MLP_BITS, NET_RNN, QNetworkSpec
 
 INFO_KEYS = ("returned_episode_returns", "returned_episode_lengths", "timestep", "returned_episode", "discount")
 
@@ -161,6 +163,10 @@ class EngineBase:
         self.graph_replays = 0
         self.graph_launches_per_replay = 0
         self._ws = None
+        # training state (purejaxql_b200.state): written after every state_every-th update (0: never); `resume`, which
+        # make_train loads from RESUME_FROM, is copied into the static buffers before the first update this run runs
+        self.state_every = runstate.save_interval(c)
+        self.resume = None
 
     def _workspace(self, S, rows):
         need = int(_lib.lib().pqn_net_workspace_bytes(self.spec.desc, S, rows))
@@ -221,11 +227,15 @@ class EngineBase:
         return {kk: torch.where(cnt > 0, sums[:, j] / cnt.clamp(min=1), torch.full_like(cnt, float("nan")))
                 for j, kk in enumerate(INFO_KEYS)}
 
-    def _run_updates(self, keys, params, u, update_body, payload, graph_auto, test_metrics, frame_channels=None):
+    def _run_updates(self, keys, params, u, update_body, payload, graph_auto, test_metrics, frame_channels=None,
+                     live=None):
         """NUM_UPDATES x update_body, with the metrics (pqn_minatar.py:329-338), the evaluation (:340-350) and the
-        wandb log (:353-365) of every update.  The first update runs eagerly (it warms every code path); when
-        CUDA_GRAPH is true, or "auto" and graph_auto holds, later updates replay a graph captured after it.
-        Returns (metrics, test_hist, test_metrics): [S, NU] float64 columns and the last evaluation."""
+        wandb log (:353-365) of every update.  The first update this process runs is eager (it warms every code
+        path); when CUDA_GRAPH is true, or "auto" and graph_auto holds, later updates replay a graph captured after it.
+        `live` names the engine's buffers that carry a run from one update to the next besides ``u``'s: they are what
+        the training state holds.  On resume the state is copied into them and into the metric columns first, and
+        the loop starts at the column after the saved update.  Returns (metrics, test_hist, test_metrics): [S, NU]
+        float64 columns and the last evaluation."""
         c, dev, L, NU = self.cfg, self.device, _lib.lib(), self.NU
         S = keys.shape[0]
         # pqn_minatar.py:330-338 reports env_frame; pqn_gymnax.py:324-331 and pqn_rnn_gymnax.py:401-408 do not
@@ -236,13 +246,17 @@ class EngineBase:
         if self.test:
             test_every = int(NU * c["TEST_INTERVAL"])
             test_hist = {kk: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for kk in INFO_KEYS}
+        live = {**(live or {}), "mu": u.mu, "nu": u.nu, "step_counter": u.step_counter, "rng": u.rng, "idx": u.idx}
+        n0 = 0
+        if self.resume is not None:
+            n0, test_metrics = self._restore_state(live, metrics, test_hist)
         want_graph = c.get("CUDA_GRAPH", "auto")
-        use_graph = (graph_auto if want_graph == "auto" else bool(want_graph)) and NU > 2
+        use_graph = (graph_auto if want_graph == "auto" else bool(want_graph)) and NU - n0 > 2
         graph = None
         self.graph_captured = False
         self.graph_replays = 0
         self.graph_launches_per_replay = 0
-        for col in range(NU):
+        for col in range(n0, NU):
             if self.on_update_begin is not None:
                 self.on_update_begin(col)
             if graph is not None:
@@ -250,7 +264,7 @@ class EngineBase:
                 self.graph_replays += 1
             else:
                 update_body()
-                if use_graph and col == 0:
+                if use_graph and col == n0:
                     try:
                         torch.cuda.synchronize(dev)
                         g = torch.cuda.CUDAGraph()
@@ -286,8 +300,93 @@ class EngineBase:
                     test_hist[kk][:, col] = test_metrics[kk]
             if c.get("WANDB_MODE", "disabled") != "disabled":
                 self._wandb_log(metrics, test_hist, col, jr.to_numpy_u32(keys)[:, 0])
+            if self.state_every and n_done % self.state_every == 0:
+                self._save_state(keys, live, metrics, test_hist, test_metrics, n_done)
         torch.cuda.synchronize(dev)
         return metrics, test_hist, test_metrics
+
+    # ---- training state (purejaxql_b200.state) ------------------------------------------------------------------ #
+    def _placement(self):
+        """(data-parallel mode, rank, world) of this engine's run."""
+        shard = self.env_shard
+        if shard is not None and shard[1] > 1:
+            return "envs", int(shard[0]), int(shard[1])
+        return ("seeds", *runstate.dist_placement())
+
+    def _resume_begin(self, keys):
+        """Whether this train() resumes from ``self.resume``; refuses keys, a seed slice or a data-parallel mode other
+        than the saved run's before anything is allocated."""
+        rs = self.resume
+        if rs is None:
+            return False
+        runstate.check_placement(rs["meta"], self._placement()[0], self.seed_lo, keys.shape[0], rs["path"])
+        if not torch.equal(keys.cpu(), rs["tensors"]["keys"]):
+            raise ValueError(f"train(rngs): the keys differ from those the run in {rs['path']} was trained with")
+        return True
+
+    def _save_state(self, keys, live, metrics, test_hist, test_metrics, n_done):
+        """Write the state after update n_done to runstate.state_file (host-side, outside any graph capture)."""
+        from .utils.save_load import save_state
+        dp, rank, world = self._placement()
+        S, spec = keys.shape[0], self.spec
+        t = {"keys": keys, **live}
+        t.update({f"metrics/{m}": v[:, :n_done] for m, v in metrics.items()})
+        if test_hist is not None:
+            t.update({f"test_hist/{kk}": v[:, :n_done] for kk, v in test_hist.items()})
+        if test_metrics is not None:
+            t.update({f"test_metrics/{kk}": v for kk, v in test_metrics.items()})
+        kind = {NET_CNN: "cnn", NET_MLP: "mlp", NET_MLP_BITS: "mlp_bits", NET_RNN: "rnn"}[spec.kind]
+        meta = dict(format=runstate.FORMAT_VERSION, script=self.script, env=self.cfg["ENV_NAME"],
+                    env_params=dataclasses.asdict(self.env_params),
+                    network=dict(kind=kind, D=spec.in_c, A=spec.num_actions, H=spec.hidden, L=spec.layers,
+                                 norm_type=spec.norm_type, norm_input=spec.norm_input),
+                    n_done=n_done, num_updates=self.NU, rng_mode=self.rng_mode, sweep=self.grid.table(self.seed_lo, S),
+                    seed_lo=self.seed_lo, num_seeds_local=S, data_parallel=dp, rank=rank, world=world,
+                    config=runstate.run_keys(self.cfg))
+        path = runstate.state_file(self.cfg, rank, world)
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        save_state(path, {"tensors": t, "meta": meta})
+
+    def _restore_state(self, live, metrics, test_hist):
+        """Copy the state of ``self.resume`` into the freshly built buffers and metric columns.  Returns (n0,
+        test_metrics): the first update to run and the last evaluation."""
+        rs = self.resume
+        t, n0 = rs["tensors"], int(rs["meta"]["n_done"])
+
+        def put(dst, name):
+            src = t.get(name)
+            if src is None or src.shape != dst.shape or src.dtype != dst.dtype:
+                got = "missing" if src is None else f"{src.dtype}{list(src.shape)}"
+                raise ValueError(f"{rs['path']}: {name} is {got}; this run's is {dst.dtype}{list(dst.shape)}")
+            dst.copy_(src)
+        for name, buf in live.items():
+            put(buf, name)
+        for m, v in metrics.items():
+            put(v[:, :n0], f"metrics/{m}")
+        test_metrics = None
+        if test_hist is not None:
+            for kk, v in test_hist.items():
+                put(v[:, :n0], f"test_hist/{kk}")
+            test_metrics = {kk: t[f"test_metrics/{kk}"].to(self.device) for kk in INFO_KEYS}
+        if self._placement()[0] == "envs":
+            self._check_replicated(t)
+        return n0, test_metrics
+
+    def _check_replicated(self, t):
+        """Env-sharded ranks hold replicas of the parameters and optimiser state: refuse files that disagree."""
+        import hashlib
+        import torch.distributed as dist
+        h = hashlib.sha256()
+        for name in ("params", "batch_stats", "mu", "nu", "step_counter", "rng", "idx"):
+            if name in t:
+                h.update(t[name].numpy().tobytes())
+        d = torch.tensor(list(h.digest()), dtype=torch.int64, device=self.device)
+        hi, lo = d.clone(), d.clone()
+        dist.all_reduce(hi, op=dist.ReduceOp.MAX)
+        dist.all_reduce(lo, op=dist.ReduceOp.MIN)
+        if not torch.equal(hi, lo):
+            raise ValueError(f"{self.resume['path']}: the replicated parameters and optimiser state of the env-sharded "
+                             f"ranks' state files differ")
 
     def _wandb_log(self, metrics, test_hist, col, seed_labels):
         import wandb
@@ -324,6 +423,11 @@ class PQNEngine(EngineBase):
         super().__init__(config, flatten_obs, device)
         self.network = network
         self.spec, self.row_words, self.obs_dtype = network_spec(self.env, network, config)
+
+    @property
+    def script(self):
+        """The training script of this engine, as a state file records it."""
+        return "pqn_minatar" if self.network == "cnn" else "pqn_gymnax"
 
     def forward(self, params, obs, S, rows, obs_rows_per_seed, q_out, gather=None, batch_stats=None):
         """network.apply({"params", "batch_stats"}, obs, train=False) (pqn_minatar.py:184-191)."""
@@ -368,20 +472,27 @@ class PQNEngine(EngineBase):
         hp, sched_stride = self._seed_tables(S)
         eps_table, sched = hp["eps"], hp["sched"]
 
-        # ---- key chain (SURVEY Appendix B; pqn_minatar.py:172-173,415-423)
-        k = jr.split(keys, 2, mode)
-        K1 = k[:, 0].contiguous()                                   # :172 rng (also the init key, :173)
-        params = spec.init(K1, dev)                                 # :156-170
+        # ---- key chain (SURVEY Appendix B; pqn_minatar.py:172-173,415-423).  A resumed run (RESUME_FROM) skips the
+        # initialiser, the first evaluation and the reset: the saved state is copied over the buffers below
+        resume = self._resume_begin(keys)
+        if not resume:
+            k = jr.split(keys, 2, mode)
+            K1 = k[:, 0].contiguous()                               # :172 rng (also the init key, :173)
+            params = spec.init(K1, dev)                             # :156-170
+        else:
+            params = torch.empty((S, P), device=dev)
         F = spec.in_c
         batch_stats = spec.init_stats(S, dev)                       # flax BatchNorm running statistics: mean 0, var 1
         self.batch_stats = batch_stats                              # read by get_test_metrics (train=False)
         bn_sums = torch.zeros(S, 2 * F, device=dev)
 
-        k = jr.split(K1, 2, mode)
-        K2, kT0 = k[:, 0].contiguous(), k[:, 1].contiguous()        # :415
-        test_metrics = self.get_test_metrics(params, kT0) if self.test else None
-        k = jr.split(K2, 2, mode)
-        K3, kR = k[:, 0].contiguous(), k[:, 1].contiguous()         # :418
+        test_metrics = None
+        if not resume:
+            k = jr.split(K1, 2, mode)
+            K2, kT0 = k[:, 0].contiguous(), k[:, 1].contiguous()    # :415
+            test_metrics = self.get_test_metrics(params, kT0) if self.test else None
+            k = jr.split(K2, 2, mode)
+            K3, kR = k[:, 0].contiguous(), k[:, 1].contiguous()     # :418
         # ---- rollout buffers: obs rows [S][T+1][E], transitions [S][T][E]
         obs_buf = torch.zeros((S, T + 1, E, W), dtype=self.obs_dtype, device=dev)
         act_buf = torch.zeros((S, T, E), dtype=torch.int32, device=dev)
@@ -394,11 +505,15 @@ class PQNEngine(EngineBase):
         step_keys = torch.zeros((T, S, 2, 2), dtype=torch.int32, device=dev)
         eps_dev = torch.zeros((1, S), device=dev)                   # eps of every seed for this update
         # ---- reset (vmap_reset, :107-109,419)
-        reset_keys = jr.split(kR, E_total, mode)[:, env_lo:env_lo + E].reshape(S * E, 2).contiguous()
+        if not resume:
+            reset_keys = jr.split(kR, E_total, mode)[:, env_lo:env_lo + E].reshape(S * E, 2).contiguous()
         state = torch.empty((self.env.state_words, S * E), dtype=torch.int32, device=dev)
-        envs.reset_into(self.env.env_id, reset_keys, state, None, S * E, self.env_params, mode)
-        self._write_obs(state, obs_buf, T, S)                        # update_body moves row T to row 0
-        rng = jr.split(K3, 2, mode)[:, 1].contiguous()              # :422-423 runner rng
+        if not resume:
+            envs.reset_into(self.env.env_id, reset_keys, state, None, S * E, self.env_params, mode)
+            self._write_obs(state, obs_buf, T, S)                    # update_body moves row T to row 0
+            rng = jr.split(K3, 2, mode)[:, 1].contiguous()          # :422-423 runner rng
+        else:
+            rng = torch.empty_like(keys)
 
         sp = _lib.stream_ptr
         seed_stride_obs = (T + 1) * E
@@ -469,7 +584,8 @@ class PQNEngine(EngineBase):
                        params=params, state=state, rng=u.rng)
         metrics, test_hist, test_metrics = self._run_updates(
             keys, params, u, update_body, payload, S * E * T <= (1 << 21) and world == 1, test_metrics,
-            frame_channels=self.env.observation_space().shape[-1] if self.network == "cnn" else None)
+            frame_channels=self.env.observation_space().shape[-1] if self.network == "cnn" else None,
+            live=dict(params=params, batch_stats=batch_stats, env_state=state, last_obs=obs_buf[:, T]))
         expl_state = (obs_buf[:, -1].contiguous(), state)
         return self._result(params, batch_stats, u, metrics, test_hist, (expl_state, test_metrics, u.rng))
 

@@ -42,6 +42,11 @@ class PQNRnnEngine(EngineBase):
         assert self.E % self.nmb == 0, "NUM_MINIBATCHES must divide NUM_ENVS (minibatches are whole env trajectories)"
         self.Bm = self.E // self.nmb
 
+    @property
+    def script(self):
+        """The training script of this engine, as a state file records it."""
+        return "pqn_rnn_gymnax"
+
     # ------------------------------------------------------------------ #
     def step(self, params, hs, obs, last_done, last_action, q, S, N):
         """network.apply(params, hs, obs[None], done[None], last_action[None], train=False) for S x N envs; hs in place.
@@ -75,17 +80,27 @@ class PQNRnnEngine(EngineBase):
         hp, sched_stride = self._seed_tables(S)
         eps_table, sched = hp["eps"], hp["sched"]                   # [NU][S], RAdam rows (sweep layout)
 
-        # ---- key chain (:255-256, :505-543)
-        k = jr.split(keys, 2, mode)
-        rng = k[:, 0].contiguous()                                   # :255  rng, _rng = split(rng)
-        params = spec.init(rng, dev)                                 # :256  create_agent(rng)  (the CARRIED key)
+        # ---- key chain (:255-256, :505-543).  A resumed run (RESUME_FROM) skips the initialiser, the first evaluation,
+        # the reset and the memory warm-up: the saved state is copied over the buffers below
+        resume = self._resume_begin(keys)
+        if not resume:
+            k = jr.split(keys, 2, mode)
+            rng = k[:, 0].contiguous()                               # :255  rng, _rng = split(rng)
+            params = spec.init(rng, dev)                             # :256  create_agent(rng)  (the CARRIED key)
+        else:
+            params = torch.empty((S, P), device=dev)
         self.batch_stats = spec.init_stats(S, dev) if self.with_stats else None   # mean 0, var 1
-        k = jr.split(rng, 2, mode)
-        rng, kT = k[:, 0].contiguous(), k[:, 1].contiguous()         # :505
-        test_metrics = self.get_test_metrics(params, kT) if self.test else None
-        k = jr.split(rng, 2, mode)
-        rng, kR = k[:, 0].contiguous(), k[:, 1].contiguous()         # :508
-        last_obs, state = self._reset(kR, S, E)                      # :509
+        test_metrics = None
+        if not resume:
+            k = jr.split(rng, 2, mode)
+            rng, kT = k[:, 0].contiguous(), k[:, 1].contiguous()     # :505
+            test_metrics = self.get_test_metrics(params, kT) if self.test else None
+            k = jr.split(rng, 2, mode)
+            rng, kR = k[:, 0].contiguous(), k[:, 1].contiguous()     # :508
+            last_obs, state = self._reset(kR, S, E)                  # :509
+        else:
+            last_obs = torch.empty((S, E, D), dtype=torch.float32, device=dev)
+            state = torch.empty((self.env.state_words, S * E), dtype=torch.int32, device=dev)
         last_done = torch.zeros((S, E), dtype=torch.uint8, device=dev)
         last_action = torch.zeros((S, E), dtype=torch.int32, device=dev)
         hs = torch.zeros((S, E, H), dtype=torch.float32, device=dev)
@@ -128,10 +143,13 @@ class PQNRnnEngine(EngineBase):
             return carry
 
         # ---- memory warm-up with random actions (:514-537); `rng` becomes the scan's final carry
-        k = jr.split(rng, 2, mode)
-        rng = rollout(k[:, 1].contiguous(), Tm, 0, eps_one)
-        k = jr.split(rng, 2, mode)                                   # :541
-        rng = k[:, 1].contiguous()                                   # runner rng = _rng
+        if not resume:
+            k = jr.split(rng, 2, mode)
+            rng = rollout(k[:, 1].contiguous(), Tm, 0, eps_one)
+            k = jr.split(rng, 2, mode)                               # :541
+            rng = k[:, 1].contiguous()                               # runner rng = _rng
+        else:
+            rng = torch.empty_like(keys)
 
         u = self._update_buffers(params, rng)                        # static buffers of the update step
         ws = self._workspace(S, max(Tm * Bm, E))
@@ -178,9 +196,13 @@ class PQNRnnEngine(EngineBase):
 
         # these runs are launch-bound (32 envs x 64 steps: thousands of small launches per update), so "auto" always
         # captures the update
+        live = dict(params=params, env_state=state, hs=hs, last_obs=last_obs, last_done=last_done,
+                    last_action=last_action, **{f"mem/{k}": v for k, v in vars(mem).items()})
+        if self.with_stats:
+            live["batch_stats"] = self.batch_stats
         metrics, test_hist, test_metrics = self._run_updates(
             keys, params, u, update_body, dict(mem=mem, params=params, rng=u.rng, batch_stats=self.batch_stats), True,
-            test_metrics)
+            test_metrics, live=live)
         bs = self.batch_stats if self.with_stats else spec.init_stats(S, dev)
         expl_state = (hs, last_obs, last_done, last_action, state)
         return self._result(params, bs, u, metrics, test_hist, (mem, expl_state, test_metrics, u.rng))

@@ -27,7 +27,7 @@ from the config, and there is REW_SCALE.
 """
 from __future__ import annotations
 
-from . import _runner, envs, sweep
+from . import _runner, envs, state, sweep
 from .engine import PQNEngine, prepare_config
 
 
@@ -35,7 +35,9 @@ def make_train(config):
     sweep.Grid(config)                       # refuses lists it cannot train before anything is built
     env, env_params = envs.make(config["ENV_NAME"], flatten_obs=True)      # :92-94
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=True)    # :80-97
+    resume = state.load_for_resume(config, "pqn_gymnax")   # RESUME_FROM, checked before anything is built
     engine = PQNEngine(config, network="mlp", flatten_obs=True)
+    engine.resume = resume
 
     def train(rngs):
         return engine.train(rngs)

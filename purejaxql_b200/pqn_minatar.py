@@ -17,7 +17,7 @@ test_metrics, rng), "metrics": {name: [S, NUM_UPDATES]}}``.
 """
 from __future__ import annotations
 
-from . import _runner, envs, sweep
+from . import _runner, envs, state, sweep
 from .engine import PQNEngine, prepare_config
 
 
@@ -25,7 +25,9 @@ def make_train(config):
     sweep.Grid(config)                       # refuses lists it cannot train before anything is built
     env, env_params = envs.make(config["ENV_NAME"])                  # :103-104
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=False)   # :91-105
+    resume = state.load_for_resume(config, "pqn_minatar")   # RESUME_FROM, checked before anything is built
     engine = PQNEngine(config, network="cnn", flatten_obs=False)
+    engine.resume = resume
 
     def train(rngs):
         return engine.train(rngs)

@@ -22,7 +22,7 @@ scripts ``train(rngs)`` takes the ``[NUM_SEEDS, 2]`` key array natively.
 """
 from __future__ import annotations
 
-from . import _runner, envs, sweep
+from . import _runner, envs, state, sweep
 from .engine import prepare_config
 from .engine_rnn import PQNRnnEngine
 
@@ -48,7 +48,9 @@ def make_train(config):
     if window < 2:
         raise ValueError(f"MEMORY_WINDOW + NUM_STEPS = {window}; the recurrent loss needs a window of at least 2 steps")
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=True)    # :119-132,140
+    resume = state.load_for_resume(config, "pqn_rnn_gymnax")   # RESUME_FROM, checked before anything is built
     engine = PQNRnnEngine(config, env_params=env_params)
+    engine.resume = resume
 
     def train(rngs):
         return engine.train(rngs)
