@@ -1,6 +1,8 @@
 """CPU tests of oracle/pqn_ref_norm.py (NORM_TYPE / NORM_INPUT variants, SURVEY section 8(f) row 4): the analytic
 backward agrees with central finite differences in fp64, the shared configuration (layer_norm, NORM_INPUT=False)
-reproduces oracle/pqn_ref.py exactly, and BatchNorm follows flax's train/eval and running-statistics rules."""
+reproduces oracle/pqn_ref.py exactly, and BatchNorm follows flax's train/eval and running-statistics rules.  The CNN
+is pinned at every channel count the library builds (CNN_SHAPES: the games' C with their action counts), since the
+GPU tests compare the variant kernels with this oracle at each of them."""
 import numpy as np
 import pytest
 
@@ -9,6 +11,8 @@ from oracle import pqn_ref_norm as N
 
 F64 = np.float64
 VARIANTS = [("layer_norm", False), ("layer_norm", True), ("batch_norm", False), ("batch_norm", True), ("none", False)]
+CNN_VARIANTS = VARIANTS + [("none", True)]
+CNN_SHAPES = [(4, 3), (6, 4), (7, 3), (10, 6)]      # (C, A): Breakout, SpaceInvaders, Freeway, Seaquest
 
 
 def _fd_check(loss_fn, p, keys, rng, n_probe=6, h=1e-6, rtol=2e-6):
@@ -27,10 +31,11 @@ def _fd_check(loss_fn, p, keys, rng, n_probe=6, h=1e-6, rtol=2e-6):
             assert abs(fd - an) <= rtol * max(1.0, abs(fd), abs(an)) + 1e-9, (k, idx, fd, an)
 
 
-@pytest.mark.parametrize("norm_type,norm_input", VARIANTS)
-def test_cnn_variant_grads_match_finite_differences(norm_type, norm_input):
-    rng = np.random.default_rng(3)
-    C, A, B = 4, 3, 6
+@pytest.mark.parametrize("norm_type,norm_input", CNN_VARIANTS)
+@pytest.mark.parametrize("C,A", CNN_SHAPES, ids=["C%dA%d" % s for s in CNN_SHAPES])
+def test_cnn_variant_grads_match_finite_differences(C, A, norm_type, norm_input):
+    rng = np.random.default_rng(3 + C)
+    B = 6
     p = R.random_params(N.cnn_param_shapes(C, A, norm_type), seed=1, dtype=F64)
     stats = N.cnn_batch_stats(C, norm_type, F64)
     obs = (rng.random((B, 10, 10, C)) < 0.2).astype(F64)
@@ -106,29 +111,38 @@ def test_batch_norm_tree_names_follow_flax_auto_naming():
 
 
 @pytest.mark.parametrize("norm_input", [False, True])
-def test_cnn_batch_norm_variant_matches_torch_autograd(norm_input):
+@pytest.mark.parametrize("C,A", CNN_SHAPES, ids=["C%dA%d" % s for s in CNN_SHAPES])
+def test_cnn_batch_norm_variant_matches_torch_autograd(C, A, norm_input):
     """Independent pin: the batch_norm network built from torch primitives (batch_norm in training mode normalises
-    with the biased batch variance, like flax) and differentiated by torch autograd, fp64."""
+    with the biased batch variance, like flax) and differentiated by torch autograd, fp64.  The running statistics
+    (new_stats) of all three BatchNorms follow flax: 0.99 of the old ones plus 0.01 of the biased batch statistics of
+    each BatchNorm's input, from non-trivial old ones."""
     import torch
-    rng = np.random.default_rng(12)
-    B, C, A = 7, 4, 3
-    p = R.random_params(N.cnn_param_shapes(C, A, "batch_norm"), seed=13, dtype=F64)
-    stats = N.cnn_batch_stats(C, "batch_norm", F64)
+    rng = np.random.default_rng(12 + C)
+    B = 7
+    p = R.random_params(N.cnn_param_shapes(C, A, "batch_norm"), seed=13 + C, dtype=F64)
+    stats = {k: {"mean": 0.1 * rng.standard_normal(v["mean"].shape), "var": 0.5 + rng.random(v["var"].shape)}
+             for k, v in N.cnn_batch_stats(C, "batch_norm", F64).items()}
     obs = (rng.random((B, 10, 10, C)) < 0.25).astype(F64)
     act, tgt = rng.integers(0, A, B), rng.standard_normal(B)
-    loss, _, g, _ = N.cnn_loss_and_grads(p, stats, obs, act, tgt, "batch_norm", norm_input)
+    loss, _, g, new_stats = N.cnn_loss_and_grads(p, stats, obs, act, tgt, "batch_norm", norm_input)
     tp = {k: torch.tensor(v, dtype=torch.float64, requires_grad=True) for k, v in p.items()}
     bn = lambda x, name: torch.nn.functional.batch_norm(x, None, None, tp[name + "/scale"], tp[name + "/bias"],
                                                         training=True, eps=1e-5)
-    x = torch.tensor(obs).permute(0, 3, 1, 2)                         # NCHW: batch_norm reduces over N, H, W
-    x = bn(x, "BatchNorm_0") if norm_input else x / 255.0
-    z = torch.nn.functional.conv2d(x, tp["CNN_0/Conv_0/kernel"].permute(3, 2, 0, 1), tp["CNN_0/Conv_0/bias"])
-    h = torch.relu(bn(z, "CNN_0/BatchNorm_0")).permute(0, 2, 3, 1).reshape(B, -1)
-    z = bn(h @ tp["CNN_0/Dense_0/kernel"] + tp["CNN_0/Dense_0/bias"], "CNN_0/BatchNorm_1")
-    q = torch.relu(z) @ tp["Dense_0/kernel"] + tp["Dense_0/bias"]
+    x0 = torch.tensor(obs).permute(0, 3, 1, 2)                        # NCHW: batch_norm reduces over N, H, W
+    x = bn(x0, "BatchNorm_0") if norm_input else x0 / 255.0
+    z1 = torch.nn.functional.conv2d(x, tp["CNN_0/Conv_0/kernel"].permute(3, 2, 0, 1), tp["CNN_0/Conv_0/bias"])
+    h = torch.relu(bn(z1, "CNN_0/BatchNorm_0")).permute(0, 2, 3, 1).reshape(B, -1)
+    z2 = h @ tp["CNN_0/Dense_0/kernel"] + tp["CNN_0/Dense_0/bias"]
+    q = torch.relu(bn(z2, "CNN_0/BatchNorm_1")) @ tp["Dense_0/kernel"] + tp["Dense_0/bias"]
     tl = 0.5 * ((q[torch.arange(B), torch.tensor(act)] - torch.tensor(tgt)) ** 2).mean()
     tl.backward()
     assert abs(float(tl.detach()) - loss) < 1e-12
     for k in p:
         ref = tp[k].grad.numpy() if tp[k].grad is not None else np.zeros_like(p[k])
         assert np.allclose(g[k], ref, rtol=1e-8, atol=1e-11), k
+    for name, z in (("BatchNorm_0", x0), ("CNN_0/BatchNorm_0", z1), ("CNN_0/BatchNorm_1", z2)):
+        zr = z.detach().transpose(0, 1).reshape(z.shape[1], -1) if z.dim() == 4 else z.detach().T
+        mean, var = zr.mean(1).numpy(), zr.var(1, unbiased=False).numpy()
+        assert np.allclose(new_stats[name]["mean"], 0.99 * stats[name]["mean"] + 0.01 * mean, rtol=1e-12, atol=1e-14), name
+        assert np.allclose(new_stats[name]["var"], 0.99 * stats[name]["var"] + 0.01 * var, rtol=1e-10, atol=1e-14), name
