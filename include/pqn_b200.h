@@ -77,7 +77,10 @@ int pqn_version(void);
  * pqn_launch_count: kernels launched by this library since load.
  * pqn_profile_enable(1): bracket every kernel launch with CUDA events on the
  * launching stream; pqn_profile_read sums elapsed ms / launch counts per kernel
- * id (arrays of pqn_num_kernels() entries on the host) and optionally resets. */
+ * id (arrays of pqn_num_kernels() entries on the host) and optionally resets.
+ * The spans are per launch, so they are only meaningful while one stream runs:
+ * under concurrent streams (a list of envs, env_list.py) a span also times
+ * whatever other streams ran beside the kernel. */
 long long pqn_launch_count(void);
 int pqn_num_kernels(void);
 const char* pqn_kernel_name(int id);

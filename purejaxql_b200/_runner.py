@@ -83,14 +83,19 @@ def single_run(config, make_train, alg_file_name="pqn", env_sharding=True):
     print(config)
     alg_name = config.get("ALG_NAME", "pqn")
     env_name = config["ENV_NAME"]
+    env_names = sweep.env_names(config)                               # a list of envs: one run trains them all
     use_wandb = config.get("WANDB_MODE", "disabled") != "disabled"
+    d_rank, d_world = init_distributed()
+    if env_names is not None:                                         # refused before a wandb run is started
+        from . import env_list
+        env_list.refuse(config, d_world, env_sharding)
     if use_wandb:
         import wandb
+        label = "+".join(env_names) if env_names is not None else env_name
         wandb.init(entity=config["ENTITY"], project=config["PROJECT"],
-                   tags=[alg_name.upper(), env_name.upper(), "b200_native"],
-                   name=f'{config["ALG_NAME"]}_{config["ENV_NAME"]}', config=config, mode=config["WANDB_MODE"])
+                   tags=[alg_name.upper(), *(n.upper() for n in env_names or [env_name]), "b200_native"],
+                   name=f'{config["ALG_NAME"]}_{label}', config=config, mode=config["WANDB_MODE"])
     grid = sweep.Grid(config)                                         # lists of LR, GAMMA, ...: one batched sweep
-    d_rank, d_world = init_distributed()
     env_sharded = pick_data_parallel(config, d_world, env_sharding) == "envs"
     rng = jr.PRNGKey(config["SEED"])                                  # :456
     t0 = time.time()
@@ -107,38 +112,53 @@ def single_run(config, make_train, alg_file_name="pqn", env_sharding=True):
         print(f"rank {rank}: no seeds assigned ({grid.total_seeds} seeds < world size {world})")
         return None
     train = make_train(config)
-    train.engine.seed_lo = seed_lo
-    if env_sharded:
-        train.engine.env_shard = (d_rank, d_world)
+    engines = getattr(train, "engines", None) or {env_name: train.engine}
+    for engine in engines.values():
+        engine.seed_lo = seed_lo
+        if env_sharded:
+            engine.env_shard = (d_rank, d_world)
     outs = train(local_rngs)                                          # :460-461 (seed axis is native)
     torch.cuda.synchronize()
     print(f"Took {time.time() - t0} seconds to complete.")
     if config.get("SAVE_PATH", None) is not None and not (env_sharded and d_rank != 0):   # :464-483
-        from .utils.save_load import save_params
-        model_state = outs["runner_state"][0]
-        save_dir = os.path.join(config["SAVE_PATH"], env_name)
-        os.makedirs(save_dir, exist_ok=True)
-        prefix = f'{alg_name}_{env_name}_seed{config["SEED"]}'
-        if rank == 0:
-            config_loader.save_yaml({k: v for k, v in config.items() if k != "alg"},
-                                    os.path.join(save_dir, f'{prefix}_config.yaml'))
-            if grid.G > 1:                                            # the values every checkpoint trained with
-                config_loader.save_yaml({"axes": {k: v for k, v in grid.axes}, "num_seeds": grid.num_seeds,
-                                         "seeds": grid.table(0, grid.total_seeds)},
-                                        os.path.join(save_dir, f'{prefix}_sweep.yaml'))
-        for i in range(local_rngs.shape[0]):
-            def pick(d):
-                return {k: (pick(v) if isinstance(v, dict) else v[i]) for k, v in d.items()}
-            gi = seed_lo + i
-            name = f"vmap{gi}" if grid.G == 1 else f"g{gi // grid.num_seeds}_vmap{gi % grid.num_seeds}"
-            save_params(pick(model_state.params), os.path.join(save_dir, f'{prefix}_{name}.safetensors'))
+        if env_names is None:
+            _save(config, grid, outs, alg_name, rank, seed_lo, local_rngs.shape[0])
+        else:                                     # every env where and as its standalone run saves it
+            for name, engine in engines.items():
+                _save(engine.cfg, grid, outs[name], alg_name, rank, seed_lo, local_rngs.shape[0])
     return outs
+
+
+def _save(config, grid, outs, alg_name, rank, seed_lo, num_local):
+    """The run's config (and sweep table) yaml and one checkpoint per local seed under <SAVE_PATH>/<ENV_NAME>."""
+    from .utils.save_load import save_params
+    env_name = config["ENV_NAME"]
+    model_state = outs["runner_state"][0]
+    save_dir = os.path.join(config["SAVE_PATH"], env_name)
+    os.makedirs(save_dir, exist_ok=True)
+    prefix = f'{alg_name}_{env_name}_seed{config["SEED"]}'
+    if rank == 0:
+        config_loader.save_yaml({k: v for k, v in config.items() if k != "alg"},
+                                os.path.join(save_dir, f'{prefix}_config.yaml'))
+        if grid.G > 1:                                                # the values every checkpoint trained with
+            config_loader.save_yaml({"axes": {k: v for k, v in grid.axes}, "num_seeds": grid.num_seeds,
+                                     "seeds": grid.table(0, grid.total_seeds)},
+                                    os.path.join(save_dir, f'{prefix}_sweep.yaml'))
+    for i in range(num_local):
+        def pick(d):
+            return {k: (pick(v) if isinstance(v, dict) else v[i]) for k, v in d.items()}
+        gi = seed_lo + i
+        name = f"vmap{gi}" if grid.G == 1 else f"g{gi // grid.num_seeds}_vmap{gi % grid.num_seeds}"
+        save_params(pick(model_state.params), os.path.join(save_dir, f'{prefix}_{name}.safetensors'))
 
 
 def tune(default_config, make_train):
     """wandb Bayesian sweep over LR (pqn_minatar.py:486-531)."""
-    import wandb
     default_config = {**default_config, **default_config["alg"]}
+    if sweep.env_names(default_config) is not None:
+        from . import env_list
+        env_list.refuse({**default_config, "HYP_TUNE": True}, 1)
+    import wandb
     print(default_config)
     alg_name = default_config.get("ALG_NAME", "pqn")
     env_name = default_config["ENV_NAME"]

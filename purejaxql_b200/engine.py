@@ -28,6 +28,7 @@ import torch
 from . import _lib, envs, jaxrandom as jr, state as runstate, sweep
 from .networks import NET_CNN, NET_MLP, NET_MLP_BITS, NET_RNN, QNetworkSpec
 
+CNN_NEEDS_MINATAR = "the MinAtar CNN needs a (10,10,C) binary-observation env"
 INFO_KEYS = ("returned_episode_returns", "returned_episode_lengths", "timestep", "returned_episode", "discount")
 
 
@@ -120,7 +121,7 @@ def network_spec(env, network: str, c: dict):
     norm_type, norm_input = c.get("NORM_TYPE", "layer_norm"), bool(c.get("NORM_INPUT", False))
     if network == "cnn":
         if not env.binary_obs:
-            raise ValueError("the MinAtar CNN needs a (10,10,C) binary-observation env")
+            raise ValueError(CNN_NEEDS_MINATAR)
         spec = QNetworkSpec(NET_CNN, env.info.obs_shape[2], env.num_actions, norm_type=norm_type, norm_input=norm_input)
         return spec, env.packed_obs_words, torch.int32
     kind = NET_MLP_BITS if env.binary_obs else NET_MLP
@@ -159,6 +160,7 @@ class EngineBase:
         # on_update_begin(n) before update n, on_update_end(n, payload) with the engine's static buffers after it
         self.on_update_begin = None
         self.on_update_end = None
+        self.log_prefix = ""        # prepended to every wandb key (an env list logs each env under "<env>/")
         self.graph_captured = False
         self.graph_replays = 0
         self.graph_launches_per_replay = 0
@@ -227,11 +229,22 @@ class EngineBase:
         return {kk: torch.where(cnt > 0, sums[:, j] / cnt.clamp(min=1), torch.full_like(cnt, float("nan")))
                 for j, kk in enumerate(INFO_KEYS)}
 
+    def train(self, rngs):
+        """The whole run: ``train_steps(rngs)`` driven to its end."""
+        steps = self.train_steps(rngs)
+        while True:
+            try:
+                next(steps)
+            except StopIteration as done:
+                return done.value
+
     def _run_updates(self, keys, params, u, update_body, payload, graph_auto, test_metrics, frame_channels=None,
                      live=None):
         """NUM_UPDATES x update_body, with the metrics (pqn_minatar.py:329-338), the evaluation (:340-350) and the
-        wandb log (:353-365) of every update.  The first update this process runs is eager (it warms every code
-        path); when CUDA_GRAPH is true, or "auto" and graph_auto holds, later updates replay a graph captured after it.
+        wandb log (:353-365) of every update.  A generator: it yields the update's index after each update, so that a
+        driver (env_list.py) can interleave the updates of several engines, and returns its result at the end.  The
+        first update this process runs is eager (it warms every code path); when CUDA_GRAPH is true, or "auto" and
+        graph_auto holds, later updates replay a graph captured after it.
         `live` names the engine's buffers that carry a run from one update to the next besides ``u``'s: they are what
         the training state holds.  On resume the state is copied into them and into the metric columns first, and
         the loop starts at the column after the saved update.  Returns (metrics, test_hist, test_metrics): [S, NU]
@@ -302,6 +315,7 @@ class EngineBase:
                 self._wandb_log(metrics, test_hist, col, jr.to_numpy_u32(keys)[:, 0])
             if self.state_every and n_done % self.state_every == 0:
                 self._save_state(keys, live, metrics, test_hist, test_metrics, n_done)
+            yield col
         torch.cuda.synchronize(dev)
         return metrics, test_hist, test_metrics
 
@@ -398,7 +412,7 @@ class EngineBase:
             for s in range(S):
                 for m, v in metrics.items():
                     row[f"rng{int(seed_labels[s])}/{m}"] = v[s, col].item()
-        wandb.log(row, step=int(row["update_steps"]))
+        wandb.log({self.log_prefix + k: v for k, v in row.items()}, step=int(row["update_steps"]))
 
     def _result(self, params, batch_stats, u, metrics, test_hist, runner_tail):
         """train()'s result: {"runner_state": (TrainState, *runner_tail), "metrics", "sweep"}."""
@@ -439,7 +453,9 @@ class PQNEngine(EngineBase):
         return q_out
 
     # ------------------------------------------------------------------ #
-    def train(self, rngs):
+    def train_steps(self, rngs):
+        """train(rngs), one update per ``next``: a generator that yields after every update and returns train's
+        result."""
         dev, L = self.device, _lib.lib()
         T, E, A = self.T, self.E, self.A
         keys = jr.as_key_tensor(rngs, dev)
@@ -582,7 +598,7 @@ class PQNEngine(EngineBase):
         # "auto" captures the update when the run is launch-bound (small S*E)
         payload = dict(obs=obs_buf, action=act_buf, reward=rew_buf, done=done_buf, maxq=maxq_buf, targets=targets,
                        params=params, state=state, rng=u.rng)
-        metrics, test_hist, test_metrics = self._run_updates(
+        metrics, test_hist, test_metrics = yield from self._run_updates(
             keys, params, u, update_body, payload, S * E * T <= (1 << 21) and world == 1, test_metrics,
             frame_channels=self.env.observation_space().shape[-1] if self.network == "cnn" else None,
             live=dict(params=params, batch_stats=batch_stats, env_state=state, last_obs=obs_buf[:, T]))

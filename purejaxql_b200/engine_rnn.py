@@ -25,11 +25,16 @@ from .engine import EngineBase
 from .networks import NET_RNN, QNetworkSpec
 
 
+def refuse_env(name: str):
+    """The recurrent engine's refusal of an env it is not built for (raised before anything is built)."""
+    if name in envs.MINATAR_GAMES + envs.MINATAR_UNREGISTERED:              # its memory buffer stores float observation rows
+        raise NotImplementedError("the recurrent script is built for the float-observation envs "
+                                  "(classic control, MemoryChain-bsuite)")
+
+
 class PQNRnnEngine(EngineBase):
     def __init__(self, config: dict, device=None, env_params: envs.EnvParams | None = None):
-        if config["ENV_NAME"] in envs.MINATAR_GAMES + envs.MINATAR_UNREGISTERED:                 # its memory buffer stores float observation rows
-            raise NotImplementedError("the recurrent script is built for the float-observation envs "
-                                      "(classic control, MemoryChain-bsuite)")
+        refuse_env(config["ENV_NAME"])
         super().__init__(config, True, device, env_params)           # env_params: MemoryChain's memory_length (:134-136)
         c = config
         self.W = int(c["MEMORY_WINDOW"])
@@ -70,7 +75,8 @@ class PQNRnnEngine(EngineBase):
         return obs, state
 
     # ------------------------------------------------------------------ #
-    def train(self, rngs):
+    def train_steps(self, rngs):
+        """train(rngs), one update per ``next`` (EngineBase.train drives it to its end)."""
         dev, L, mode = self.device, _lib.lib(), self.rng_mode
         T, E, A, W, H, D, Bm = self.T, self.E, self.A, self.W, self.H, self.D, self.Bm
         Tm = W + T
@@ -200,7 +206,7 @@ class PQNRnnEngine(EngineBase):
                     last_action=last_action, **{f"mem/{k}": v for k, v in vars(mem).items()})
         if self.with_stats:
             live["batch_stats"] = self.batch_stats
-        metrics, test_hist, test_metrics = self._run_updates(
+        metrics, test_hist, test_metrics = yield from self._run_updates(
             keys, params, u, update_body, dict(mem=mem, params=params, rng=u.rng, batch_stats=self.batch_stats), True,
             test_metrics, live=live)
         bs = self.batch_stats if self.with_stats else spec.init_stats(S, dev)

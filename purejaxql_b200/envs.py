@@ -438,6 +438,12 @@ def reset_into(env_id: int, keys: torch.Tensor, state: torch.Tensor, obs: torch.
                                                rng_mode, _lib.stream_ptr()), "pqn_env_reset_params")
 
 
+def check_name(name: str):
+    """Refuse a name that is not an env of ``ENV_IDS`` (host-side: builds nothing)."""
+    if name not in ENV_IDS:
+        raise KeyError(f"unknown env {name!r}; known: {sorted(ENV_IDS)}")
+
+
 # --------------------------------------------------------------------------- #
 # the batched environment
 # --------------------------------------------------------------------------- #
@@ -446,8 +452,7 @@ class BatchedEnv:
     ``FlattenObservationWrapper``), batched over the leading axis."""
 
     def __init__(self, name: str, flatten_obs: bool = False, rng_mode: int = 0):
-        if name not in ENV_IDS:
-            raise KeyError(f"unknown env {name!r}; known: {sorted(ENV_IDS)}")
+        check_name(name)
         self.name = name
         self.env_id = ENV_IDS[name]
         info = _lib.EnvInfo()

@@ -9,6 +9,7 @@ purejaxql/pqn_gymnax.py.
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=DeepSea-bsuite
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=FourRooms-misc
     python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole alg.ENV_NAME=GaussianBandit-misc
+    python -m purejaxql_b200.pqn_gymnax +alg=pqn_cartpole NUM_SEEDS=4 "alg.ENV_NAME=[CartPole-v1,Acrobot-v1,Catch-bsuite,DeepSea-bsuite]"
 
 Every env of ``envs.ENV_IDS`` runs with its gymnax default ``EnvParams``: CartPole-v1, Acrobot-v1, MountainCar-v0
 (200 steps), MemoryChain-bsuite, Catch-bsuite (its 10 x 5 board flattened to 50 inputs), DeepSea-bsuite (its 8 x 8
@@ -24,15 +25,24 @@ Differences from pqn_minatar (as in the reference, pqn_gymnax.py:29-58,92-97):
 MLP ``QNetwork(HIDDEN_SIZE, NUM_LAYERS)`` without the /255, the observation is
 flattened (``FlattenObservationWrapper``), ``TEST_NUM_STEPS`` may be overridden
 from the config, and there is REW_SCALE.
+
+A list-valued ``ENV_NAME`` trains every env of the list in one run (``env_list.py``): ``train(rngs)`` returns
+``{env_name: <what a standalone train(rngs) of that env returns>}``.
 """
 from __future__ import annotations
 
-from . import _runner, envs, state, sweep
+from . import _runner, env_list, envs, state, sweep
 from .engine import PQNEngine, prepare_config
 
 
 def make_train(config):
     sweep.Grid(config)                       # refuses lists it cannot train before anything is built
+    if sweep.env_names(config) is not None:  # a list of envs: one engine per env on its own stream (env_list.py)
+        return env_list.make_train(config, _make_train_one, envs.check_name)
+    return _make_train_one(config)
+
+
+def _make_train_one(config):
     env, env_params = envs.make(config["ENV_NAME"], flatten_obs=True)      # :92-94
     prepare_config(config, env_params.max_steps_in_episode, allow_test_steps_override=True)    # :80-97
     resume = state.load_for_resume(config, "pqn_gymnax")   # RESUME_FROM, checked before anything is built

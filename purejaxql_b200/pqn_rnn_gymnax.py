@@ -7,6 +7,7 @@
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=UmbrellaChain-bsuite
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=MetaMaze-misc
     python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole alg.ENV_NAME=GaussianBandit-misc
+    python -m purejaxql_b200.pqn_rnn_gymnax +alg=pqn_rnn_cartpole "alg.ENV_NAME=[CartPole-v1,MemoryChain-bsuite,MetaMaze-misc]"
 
 The envs are CartPole-v1, Acrobot-v1, MountainCar-v0, MemoryChain-bsuite, Catch-bsuite (50 inputs: every
 NORM_TYPE / NORM_INPUT runs on it), DeepSea-bsuite (64 inputs), UmbrellaChain-bsuite, DiscountingChain-bsuite,
@@ -18,17 +19,30 @@ are refused: the memory stores float observation rows.
 NUM_UPDATES_DECAY, TEST_NUM_STEPS), ``RNNQNetwork`` (MLP trunk -> one-hot last action -> scanned GRU with done-resets ->
 Q head), a memory of MEMORY_WINDOW + NUM_STEPS transitions warmed up with random actions, minibatches over ENVS (whole
 trajectories) and the Q(lambda) targets computed inside the loss from the window's own q values.  As in the other
-scripts ``train(rngs)`` takes the ``[NUM_SEEDS, 2]`` key array natively.
+scripts ``train(rngs)`` takes the ``[NUM_SEEDS, 2]`` key array natively, and a list-valued ``ENV_NAME`` trains every
+env of the list in one run (``env_list.py``; ``ENV_KWARGS.memory_length`` applies to the MemoryChain-bsuite entry).
 """
 from __future__ import annotations
 
-from . import _runner, envs, state, sweep
+from . import _runner, env_list, envs, state, sweep
 from .engine import prepare_config
-from .engine_rnn import PQNRnnEngine
+from .engine_rnn import PQNRnnEngine, refuse_env
+
+
+def _check_env(name):
+    """The refusal a standalone run of `name` meets, without building the env."""
+    envs.check_name(name)
+    refuse_env(name)
 
 
 def make_train(config):
     sweep.Grid(config)                       # refuses lists it cannot train before anything is built
+    if sweep.env_names(config) is not None:  # a list of envs: one engine per env on its own stream (env_list.py)
+        return env_list.make_train(config, _make_train_one, _check_env, env_sharding=False)
+    return _make_train_one(config)
+
+
+def _make_train_one(config):
     env, env_params = envs.make(config["ENV_NAME"], flatten_obs=True)      # :134-139
     if config["ENV_NAME"] == "MemoryChain-bsuite":
         # :134-136 -- EnvParams(memory_length=ENV_KWARGS.get("memory_length", 10)): the script's default is 10, not

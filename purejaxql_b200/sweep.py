@@ -12,6 +12,9 @@ g * NUM_SEEDS + i is seed i of point g.  Every point uses the same keys ``split(
 random numbers), so the key array of a sweep is those keys tiled G times (``Grid.tile``) and the seeds of point g train
 exactly what a standalone run of point g's config given the same key array trains.
 
+``ENV_NAME`` may be a list too: not a grid axis (different envs cannot share launches) but a list of envs, each trained
+by its own engine as a standalone run of its name would train it (``env_list.py``); every env trains every grid point.
+
 The device reads the hyperparameters from per-seed arrays (``engine.seed_inputs``): the eps table [NU][S], the
 RAdam schedule [S][steps][4] (one shared [steps][4] table when G == 1), and gamma, lambda, max-norm and reward scale
 [S].  A config without lists gives exactly the inputs of a scalar run.
@@ -27,15 +30,32 @@ MAX_SEEDS = 65535          # the seed axis is gridDim.y of the kernels
 _DEFAULTS = {"REW_SCALE": 1}
 
 
+def env_names(config: dict) -> list | None:
+    """The envs of a list-valued ``ENV_NAME`` (None for a single env); refuses an empty list and duplicate names."""
+    v = config.get("ENV_NAME")
+    if not isinstance(v, (list, tuple)):
+        return None
+    if len(v) == 0:
+        raise ValueError("ENV_NAME=[]: an empty list has no env to train")
+    if not all(isinstance(n, str) for n in v):
+        raise ValueError(f"ENV_NAME={v!r}: every entry of the list must be an env name")
+    dup = sorted({n for n in v if list(v).count(n) > 1})
+    if dup:
+        raise ValueError(f"ENV_NAME={v!r}: {', '.join(dup)} appears more than once; each env trains once per run")
+    return list(v)
+
+
 class Grid:
     """The grid of a config (refuses lists it cannot train, before anything is built).  ``points[g]`` maps each
     list-valued key to point g's value; ``config(g)`` is point g's scalar config."""
 
     def __init__(self, config: dict):
+        env_names(config)
         for k, v in config.items():
-            if isinstance(v, (list, tuple)) and k not in SWEEP_KEYS:
+            if isinstance(v, (list, tuple)) and k not in SWEEP_KEYS and k != "ENV_NAME":
                 raise ValueError(f"{k}={v!r}: only {', '.join(SWEEP_KEYS)} may be a list (a grid of settings trained "
-                                 f"as one batched run); {k} changes the shapes or the kernels of the run")
+                                 f"as one batched run), and ENV_NAME (a list of envs trained side by side); {k} "
+                                 f"changes the shapes or the kernels of the run")
         self.axes = []
         for k in SWEEP_KEYS:
             v = config.get(k)
