@@ -346,6 +346,61 @@ int pqn_radam_clip_step_seeds(float* params, const float* grads, float* mu, floa
                               int64_t sched_seed_stride, int32_t* step_counter, float* gnorm_scratch /*[S][64]*/,
                               int32_t S, int64_t P, const float* max_norm, float b1, float b2, float eps, void* stream);
 
+/* pqn_radam_clip_step_seeds for population-based training: seed s reads row t of the table of seed sched_src[s]
+ * (int32[S]; any value when sched_seed_stride is 0) at sched + sched_src[s] * sched_seed_stride + 4 * t and steps with
+ * lr_t * lr_mult[s] (float32[S], the product rounded once).  With sched_src[s] = s (or a shared table) and
+ * lr_mult[s] = 1: bit-identical to pqn_radam_clip_step_seeds. */
+int pqn_radam_clip_step_pbt(float* params, const float* grads, float* mu, float* nu, const float* sched,
+                            int64_t sched_seed_stride, const int32_t* sched_src, const float* lr_mult,
+                            int32_t* step_counter, float* gnorm_scratch /*[S][64]*/, int32_t S, int64_t P,
+                            const float* max_norm, float b1, float b2, float eps, void* stream);
+
+/* ---- population-based training (truncation selection over the seed axis; DESIGN.md section 3.10) ---------------
+ * One exploit/explore event, all on the device (no host synchronisation):
+ *   fitness[s] = (sum over c < fit_cols of fit[s * fit_stride + c]) / fit_cols, in float64, in column order
+ *   order      = seeds by descending fitness; ties by the lower index; NaN last (also by index)
+ *   key        : kp, ke = split(kp) (key is advanced in place); ka, kf = split(ke)
+ *   a = randint(ka, (m,), 0, m); b = randint(kf, (m, n_perturb), 0, 2)
+ *   child order[S - m + j] takes the rows of parent order[a[j]] (parent[child] = that parent, parent[s] = s for every
+ *   other seed): params, mu, nu [S][P], batch_stats [S][stats_floats] (NULL: none), eps rows [eps_from, eps_rows) of
+ *   eps [eps_rows][S], sched_src, lr_mult, gamma, lambda_, max_norm, rew_scale [S]
+ *   then for each i < n_perturb, phi = factors[b[j][i]] (fp32): PQN_PBT_LR, _MAX_GRAD_NORM, _REW_SCALE multiply the
+ *   child's lr_mult / max_norm / rew_scale by phi; PQN_PBT_GAMMA, _LAMBDA set x = clamp(1 - (1 - x) * phi, 0, 1).
+ * 2 <= S <= 65535 and 1 <= m <= S / 2 (parents and children are disjoint).  Outputs fitness float64[S], order
+ * int32[S], parent int32[S].  workspace: pqn_pbt_workspace_bytes(S, m) bytes. */
+enum { PQN_PBT_LR = 0, PQN_PBT_MAX_GRAD_NORM = 1, PQN_PBT_REW_SCALE = 2, PQN_PBT_GAMMA = 3, PQN_PBT_LAMBDA = 4 };
+typedef struct {
+  int32_t S, m;
+  const double* fit;
+  int64_t fit_stride;
+  int32_t fit_cols;
+  int32_t rng_mode;               /* JAX_THREEFRY_PARTITIONABLE */
+  int32_t* key;                   /* [2] the event chain's key kp */
+  int32_t n_perturb;
+  int32_t perturb[5];             /* PQN_PBT_* of column i of b */
+  float factors[2];
+  float* params;
+  float* mu;
+  float* nu;
+  int64_t P;
+  float* batch_stats;
+  int64_t stats_floats;
+  float* eps;
+  int32_t eps_rows, eps_from;
+  int32_t* sched_src;
+  float* lr_mult;
+  float* gamma;
+  float* lambda_;
+  float* max_norm;
+  float* rew_scale;
+  double* fitness;
+  int32_t* order;
+  int32_t* parent;
+  void* workspace;
+} pqn_pbt_event_t;
+int64_t pqn_pbt_workspace_bytes(int32_t S, int32_t m);
+int pqn_pbt_event(const pqn_pbt_event_t* args_host, void* stream);
+
 /* dummy input BatchNorm running statistics (flax nn.BatchNorm momentum 0.99;
  * pqn_minatar.py:65,293-296): batch_stats float32[S][2][F] (mean, var),
  * bn_sums float32[S][2][F] (sum x, sum x^2 over `count` elements per feature);

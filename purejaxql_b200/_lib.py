@@ -29,6 +29,17 @@ class NetDesc(Structure):
                 ("num_actions", c_int32), ("norm_type", c_int32), ("norm_input", c_int32)]
 
 
+class PbtEvent(Structure):
+    """pqn_pbt_event_t: the arguments of one population-based training event."""
+    _fields_ = [("S", c_int32), ("m", c_int32), ("fit", c_void_p), ("fit_stride", c_int64), ("fit_cols", c_int32),
+                ("rng_mode", c_int32), ("key", c_void_p), ("n_perturb", c_int32), ("perturb", c_int32 * 5),
+                ("factors", c_float * 2), ("params", c_void_p), ("mu", c_void_p), ("nu", c_void_p), ("P", c_int64),
+                ("batch_stats", c_void_p), ("stats_floats", c_int64), ("eps", c_void_p), ("eps_rows", c_int32),
+                ("eps_from", c_int32), ("sched_src", c_void_p), ("lr_mult", c_void_p), ("gamma", c_void_p),
+                ("lambda_", c_void_p), ("max_norm", c_void_p), ("rew_scale", c_void_p), ("fitness", c_void_p),
+                ("order", c_void_p), ("parent", c_void_p), ("workspace", c_void_p)]
+
+
 NORM_TYPES = {"layer_norm": 0, "batch_norm": 1}          # any other string: no normalisation (pqn_minatar.py:35-36)
 
 
@@ -106,6 +117,11 @@ _SIGS = {
                                     c_int64, c_float, c_float, c_float, c_float, c_void_p]),
     "pqn_radam_clip_step_seeds": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                           c_void_p, c_int32, c_int64, c_void_p, c_float, c_float, c_float, c_void_p]),
+    "pqn_radam_clip_step_pbt": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_int32, c_int64, c_void_p, c_float, c_float, c_float,
+                                        c_void_p]),
+    "pqn_pbt_workspace_bytes": (c_int64, [c_int32, c_int32]),
+    "pqn_pbt_event": (c_int, [POINTER(PbtEvent), c_void_p]),
     "pqn_bn_stats_update": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int64, c_float, c_float, c_void_p]),
     "pqn_set_tensor_core_path": (c_int, [c_int]),
     "pqn_set_conv_mma_path": (c_int, [c_int]),

@@ -9,7 +9,7 @@ import time
 
 import torch
 
-from . import config_loader, jaxrandom as jr, sweep
+from . import config_loader, jaxrandom as jr, pbt, sweep
 
 
 def init_distributed():
@@ -97,6 +97,7 @@ def single_run(config, make_train, alg_file_name="pqn", env_sharding=True):
                    name=f'{config["ALG_NAME"]}_{label}', config=config, mode=config["WANDB_MODE"])
     grid = sweep.Grid(config)                                         # lists of LR, GAMMA, ...: one batched sweep
     env_sharded = pick_data_parallel(config, d_world, env_sharding) == "envs"
+    pbt.settings(config, d_world, env_sharded)                        # a population must live in one process
     rng = jr.PRNGKey(config["SEED"])                                  # :456
     t0 = time.time()
     rngs = jr.split(rng, config["NUM_SEEDS"], int(config.get("JAX_THREEFRY_PARTITIONABLE", 0)))   # :459
@@ -144,6 +145,9 @@ def _save(config, grid, outs, alg_name, rank, seed_lo, num_local):
             config_loader.save_yaml({"axes": {k: v for k, v in grid.axes}, "num_seeds": grid.num_seeds,
                                      "seeds": grid.table(0, grid.total_seeds)},
                                     os.path.join(save_dir, f'{prefix}_sweep.yaml'))
+        if "pbt" in outs:                                             # the population's lineage
+            config_loader.save_yaml(pbt.lineage_yaml(outs["pbt"], pbt.settings(config)),
+                                    os.path.join(save_dir, f'{prefix}_pbt.yaml'))
     for i in range(num_local):
         def pick(d):
             return {k: (pick(v) if isinstance(v, dict) else v[i]) for k, v in d.items()}
@@ -155,6 +159,7 @@ def _save(config, grid, outs, alg_name, rank, seed_lo, num_local):
 def tune(default_config, make_train):
     """wandb Bayesian sweep over LR (pqn_minatar.py:486-531)."""
     default_config = {**default_config, **default_config["alg"]}
+    pbt.settings({**default_config, "HYP_TUNE": True})
     if sweep.env_names(default_config) is not None:
         from . import env_list
         env_list.refuse({**default_config, "HYP_TUNE": True}, 1)

@@ -25,6 +25,7 @@ UNITS = [
     ("pqn_net.cu", []),
     ("pqn_optim.cu", []),
     ("pqn_perm.cu", []),
+    ("pqn_pbt.cu", []),
     ("pqn_tc.cu", []),
 ]
 

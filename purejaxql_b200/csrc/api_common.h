@@ -19,7 +19,8 @@ enum KernelId : int {
   K_RNN_SCAN, K_RNN_MISC /* GRU network (pqn_rnn.cuh) */,
   K_GRAD_FINAL /* fixed-order second stage of the deterministic gradient reductions */,
   K_PERM /* jax.random.permutation bucket + rank sort (pqn_perm.cu) */,
-  K_BITS_FWD, K_BITS_WGRAD /* Dense_0 of the MLP on packed MinAtar bits (pqn_bits.cuh) */, K_COUNT
+  K_BITS_FWD, K_BITS_WGRAD /* Dense_0 of the MLP on packed MinAtar bits (pqn_bits.cuh) */,
+  K_PBT /* population-based training event (pqn_pbt.cu) */, K_COUNT
 };
 
 // A hyperparameter that may differ between seeds: v[seed] when v is given (the *_seeds entry points), else the value c

@@ -41,7 +41,7 @@ static const char* const kNames[K_COUNT] = {
     "conv_fwd", "dense_fwd", "row_bwd", "wgrad", "dgrad", "conv_bwd", "gather_rows", "sqnorm", "radam", "advance",
     "bn_update", "tc_gemm", "tc_split", "tc_dense_fwd", "tc_wgrad", "tc_dgrad", "net_init",
     "conv_fwd_infer", "tc_dense_fwd_head", "norm_fwd", "norm_bwd", "norm_reduce", "rnn_scan", "rnn_misc",
-    "grad_finalize", "permutation", "bits_dense_fwd", "bits_wgrad"};
+    "grad_finalize", "permutation", "bits_dense_fwd", "bits_wgrad", "pbt"};
 
 struct Span { int id; cudaEvent_t a, b; };
 static long long g_launches = 0;

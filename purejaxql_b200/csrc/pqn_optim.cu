@@ -47,17 +47,22 @@ __global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ g
   }
 }
 
+// PBT (population-based training): seed s reads the table of seed sched_src[s] and scales its lr_t by lr_mult[s]
+template <bool PBT>
 __global__ void __launch_bounds__(256) radam_kernel(float* __restrict__ params, const float* __restrict__ grads,
                                                     float* __restrict__ mu, float* __restrict__ nu,
                                                     const float* __restrict__ sched, int64_t sched_stride,
+                                                    const int32_t* __restrict__ sched_src,
+                                                    const float* __restrict__ lr_mult,
                                                     const int32_t* __restrict__ step_counter,
                                                     const float* __restrict__ gn, int64_t P, SeedScalar max_norm_s,
                                                     float b1, float b2, float eps) {
   const int seed = blockIdx.y;
   const int64_t i4 = (int64_t)blockIdx.x * 256 + threadIdx.x;
   const int t = step_counter[0];
-  const float* __restrict__ row = sched + seed * sched_stride + 4 * t;   // this seed's table (stride 0: shared)
-  const float lr = __ldg(row + 0);
+  const int64_t table = PBT ? (int64_t)__ldg(sched_src + seed) : (int64_t)seed;
+  const float* __restrict__ row = sched + table * sched_stride + 4 * t;   // this seed's table (stride 0: shared)
+  const float lr = PBT ? __fmul_rn(__ldg(row + 0), __ldg(lr_mult + seed)) : __ldg(row + 0);
   const float bc1 = __ldg(row + 1);
   const float bc2 = __ldg(row + 2);
   const float rect = __ldg(row + 3);
@@ -172,7 +177,8 @@ __global__ void net_init_kernel(const uint32_t* __restrict__ keys, float* __rest
 using namespace pqn;
 
 static int radam_clip_step(float* params, const float* grads, float* mu, float* nu, const float* sched,
-                           int64_t sched_stride, int32_t* step_counter, float* gnorm_scratch, int32_t S, int64_t P,
+                           int64_t sched_stride, const int32_t* sched_src, const float* lr_mult,
+                           int32_t* step_counter, float* gnorm_scratch, int32_t S, int64_t P,
                            SeedScalar max_norm, float b1, float b2, float eps, void* stream, const char* who) {
   if (!params || !grads || !mu || !nu || !sched || sched_stride < 0 || !step_counter || !gnorm_scratch || S <= 0 ||
       P <= 0 || (P & 3) || S > 65535)
@@ -180,9 +186,15 @@ static int radam_clip_step(float* params, const float* grads, float* mu, float* 
   cudaStream_t st = (cudaStream_t)stream;
   { LaunchScope _ls(K_SQNORM, st); sqnorm_kernel<<<dim3(NORM_BLOCKS, S), 256, 0, st>>>(grads, P, gnorm_scratch); }
   const unsigned nb = (unsigned)((P / 4 + 255) / 256);
-  { LaunchScope _ls(K_RADAM, st); radam_kernel<<<dim3(nb, S), 256, 0, st>>>(params, grads, mu, nu, sched, sched_stride,
-                                                                           step_counter, gnorm_scratch, P, max_norm, b1,
-                                                                           b2, eps); }
+  if (sched_src) {
+    LaunchScope _ls(K_RADAM, st);
+    radam_kernel<true><<<dim3(nb, S), 256, 0, st>>>(params, grads, mu, nu, sched, sched_stride, sched_src, lr_mult,
+                                                    step_counter, gnorm_scratch, P, max_norm, b1, b2, eps);
+  } else {
+    LaunchScope _ls(K_RADAM, st);
+    radam_kernel<false><<<dim3(nb, S), 256, 0, st>>>(params, grads, mu, nu, sched, sched_stride, nullptr, nullptr,
+                                                     step_counter, gnorm_scratch, P, max_norm, b1, b2, eps);
+  }
   { LaunchScope _ls(K_ADVANCE, st); advance_kernel<<<1, 1, 0, st>>>(step_counter); }
   return check_launch(who);
 }
@@ -192,7 +204,8 @@ extern "C" {
 int pqn_radam_clip_step(float* params, const float* grads, float* mu, float* nu, const float* sched,
                         int32_t* step_counter, float* gnorm_scratch, int32_t S, int64_t P, float max_norm, float b1,
                         float b2, float eps, void* stream) {
-  return radam_clip_step(params, grads, mu, nu, sched, 0, step_counter, gnorm_scratch, S, P, SeedScalar{nullptr, max_norm},
+  return radam_clip_step(params, grads, mu, nu, sched, 0, nullptr, nullptr, step_counter, gnorm_scratch, S, P,
+                         SeedScalar{nullptr, max_norm},
                          b1, b2, eps, stream, "pqn_radam_clip_step");
 }
 
@@ -200,8 +213,18 @@ int pqn_radam_clip_step_seeds(float* params, const float* grads, float* mu, floa
                               int64_t sched_seed_stride, int32_t* step_counter, float* gnorm_scratch, int32_t S,
                               int64_t P, const float* max_norm, float b1, float b2, float eps, void* stream) {
   if (!max_norm) return set_error(PQN_E_INVALID, "pqn_radam_clip_step_seeds: max_norm is NULL");
-  return radam_clip_step(params, grads, mu, nu, sched, sched_seed_stride, step_counter, gnorm_scratch, S, P,
-                         SeedScalar{max_norm, 0.f}, b1, b2, eps, stream, "pqn_radam_clip_step_seeds");
+  return radam_clip_step(params, grads, mu, nu, sched, sched_seed_stride, nullptr, nullptr, step_counter, gnorm_scratch,
+                         S, P, SeedScalar{max_norm, 0.f}, b1, b2, eps, stream, "pqn_radam_clip_step_seeds");
+}
+
+int pqn_radam_clip_step_pbt(float* params, const float* grads, float* mu, float* nu, const float* sched,
+                            int64_t sched_seed_stride, const int32_t* sched_src, const float* lr_mult,
+                            int32_t* step_counter, float* gnorm_scratch, int32_t S, int64_t P, const float* max_norm,
+                            float b1, float b2, float eps, void* stream) {
+  if (!max_norm || !sched_src || !lr_mult)
+    return set_error(PQN_E_INVALID, "pqn_radam_clip_step_pbt: max_norm, sched_src and lr_mult are required");
+  return radam_clip_step(params, grads, mu, nu, sched, sched_seed_stride, sched_src, lr_mult, step_counter,
+                         gnorm_scratch, S, P, SeedScalar{max_norm, 0.f}, b1, b2, eps, stream, "pqn_radam_clip_step_pbt");
 }
 
 int pqn_net_init(const pqn_net_desc_t* d, const uint32_t* keys, float* params, int32_t S, void* stream) {

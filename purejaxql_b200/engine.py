@@ -25,7 +25,7 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
-from . import _lib, envs, jaxrandom as jr, state as runstate, sweep
+from . import _lib, envs, jaxrandom as jr, pbt, state as runstate, sweep
 from .networks import NET_CNN, NET_MLP, NET_MLP_BITS, NET_RNN, QNetworkSpec
 
 CNN_NEEDS_MINATAR = "the MinAtar CNN needs a (10,10,C) binary-observation env"
@@ -141,6 +141,8 @@ class EngineBase:
     def __init__(self, config: dict, flatten_obs: bool, device=None, env_params: envs.EnvParams | None = None):
         self.cfg = c = config
         self.grid = sweep.Grid(config)       # per-seed hyperparameters: a grid of G points x NUM_SEEDS
+        self.pbt = pbt.settings(config)      # population-based training (None: off); train() builds the population
+        self.population = None
         self.seed_lo = 0            # global index of this run's first seed (a seed-sharded rank trains a slice)
         self.env_shard = None       # (rank, world): train envs [rank*E/world, (rank+1)*E/world) of every seed
         self.device = torch.device(device or "cuda")
@@ -181,6 +183,34 @@ class EngineBase:
         c = self.cfg
         return seed_tensors(seed_inputs(self.grid, self.seed_lo, S, self.NU, c["NUM_UPDATES_DECAY"],
                                         self.nmb * self.epochs, c.get("LR_LINEAR_DECAY", False)), self.device)
+
+    def _population(self, hp, sched_stride, S):
+        """The run's pbt.Population over its S seeds (None without PBT).  The event edits hp's tables in place."""
+        self.population = None
+        if self.pbt is None:
+            return None
+        dp, _, world = self._placement()
+        if dp == "seeds" and world > 1:
+            raise ValueError(f"PBT_INTERVAL={self.pbt.interval}: a seed-sharded run of {world} processes would split "
+                             f"the population over the processes; run PBT in one process or with DATA_PARALLEL=envs")
+        self.population = pbt.Population(self.pbt, S, self.NU, hp, sched_stride, self.rng_mode, self.device)
+        return self.population
+
+    def _radam_step(self, params, u, hp, sched_stride, S, P):
+        """clip + RAdam of every seed (pqn_minatar.py:292): pqn_radam_clip_step_seeds, or with PBT
+        pqn_radam_clip_step_pbt, which reads each seed's schedule source and LR multiplier."""
+        L, pop, sp = _lib.lib(), self.population, _lib.stream_ptr
+        if pop is None:
+            _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(u.grads), _lib.p(u.mu), _lib.p(u.nu),
+                                                   _lib.p(hp["sched"]), sched_stride, _lib.p(u.step_counter),
+                                                   _lib.p(u.gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999, 1e-8,
+                                                   sp()), "pqn_radam_clip_step_seeds")
+        else:
+            _lib.check(L.pqn_radam_clip_step_pbt(_lib.p(params), _lib.p(u.grads), _lib.p(u.mu), _lib.p(u.nu),
+                                                 _lib.p(hp["sched"]), sched_stride, _lib.p(pop.sched_src),
+                                                 _lib.p(pop.lr_mult), _lib.p(u.step_counter), _lib.p(u.gnorm), S, P,
+                                                 _lib.p(hp["max_norm"]), 0.9, 0.999, 1e-8, sp()),
+                       "pqn_radam_clip_step_pbt")
 
     def _update_buffers(self, params, rng):
         """The optimiser state and the static buffers every update reads and writes (so that it can be replayed
@@ -260,6 +290,9 @@ class EngineBase:
             test_every = int(NU * c["TEST_INTERVAL"])
             test_hist = {kk: torch.zeros((S, max(NU, 1)), dtype=torch.float64, device=dev) for kk in INFO_KEYS}
         live = {**(live or {}), "mu": u.mu, "nu": u.nu, "step_counter": u.step_counter, "rng": u.rng, "idx": u.idx}
+        pop = self.population
+        if pop is not None:
+            live.update(pop.live())
         n0 = 0
         if self.resume is not None:
             n0, test_metrics = self._restore_state(live, metrics, test_hist)
@@ -313,6 +346,12 @@ class EngineBase:
                     test_hist[kk][:, col] = test_metrics[kk]
             if c.get("WANDB_MODE", "disabled") != "disabled":
                 self._wandb_log(metrics, test_hist, col, jr.to_numpy_u32(keys)[:, 0])
+            if pop is not None and pop.due(n_done, NU):         # eager, on the static buffers the graph replays
+                if pop.st.fitness == "test":
+                    fit, c0, cols = test_metrics[pbt.FITNESS_METRIC].contiguous(), 0, 1
+                else:
+                    fit, c0, cols = metrics[pbt.FITNESS_METRIC], n_done - pop.st.interval, pop.st.interval
+                pop.event(n_done, fit, c0, cols, params, u.mu, u.nu, self.batch_stats)
             if self.state_every and n_done % self.state_every == 0:
                 self._save_state(keys, live, metrics, test_hist, test_metrics, n_done)
             yield col
@@ -428,8 +467,11 @@ class EngineBase:
             opt_state=SimpleNamespace(mu=u.mu, nu=u.nu, count=grad_steps),
             timesteps=torch.full((S,), timesteps, dtype=torch.int64), n_updates=torch.full((S,), NU),
             grad_steps=torch.full((S,), grad_steps))
-        return {"runner_state": (train_state, *runner_tail), "metrics": out_metrics,
-                "sweep": self.grid.table(self.seed_lo, S)}
+        out = {"runner_state": (train_state, *runner_tail), "metrics": out_metrics,
+               "sweep": self.grid.table(self.seed_lo, S)}
+        if self.population is not None:
+            out["pbt"] = self.population.result(self.grid, self.seed_lo, NU)
+        return out
 
 
 class PQNEngine(EngineBase):
@@ -486,7 +528,8 @@ class PQNEngine(EngineBase):
 
         # ---- schedules (pqn_minatar.py:134-147) and the other per-seed hyperparameters
         hp, sched_stride = self._seed_tables(S)
-        eps_table, sched = hp["eps"], hp["sched"]
+        eps_table = hp["eps"]
+        self._population(hp, sched_stride, S)
 
         # ---- key chain (SURVEY Appendix B; pqn_minatar.py:172-173,415-423).  A resumed run (RESUME_FROM) skips the
         # initialiser, the first evaluation and the reset: the saved state is copied over the buffers below
@@ -584,10 +627,7 @@ class PQNEngine(EngineBase):
                         _lib.p(u.qsa_sum), _lib.p(bn_sums), S, mb, _lib.p(ws), sp()), "pqn_qnet_loss_grad")
                     allreduce_(u.grads, True)                        # the ONE collective of the data path
                     allreduce_(bn_sums, False)
-                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(u.grads), _lib.p(u.mu), _lib.p(u.nu),
-                                                           _lib.p(sched), sched_stride, _lib.p(u.step_counter),
-                                                           _lib.p(u.gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
-                                                           1e-8, sp()), "pqn_radam_clip_step_seeds")
+                    self._radam_step(params, u, hp, sched_stride, S, P)
                     _lib.check(L.pqn_bn_stats_update(_lib.p(batch_stats), _lib.p(bn_sums), S, F, spec.stats_total,
                                                      bn_count, 0.99, sp()), "pqn_bn_stats_update")
             allreduce_(u.loss_sum, True)

@@ -84,7 +84,8 @@ class PQNRnnEngine(EngineBase):
         S = keys.shape[0]
         spec, P = self.spec, self.spec.total
         hp, sched_stride = self._seed_tables(S)
-        eps_table, sched = hp["eps"], hp["sched"]                   # [NU][S], RAdam rows (sweep layout)
+        eps_table = hp["eps"]                                        # [NU][S]
+        self._population(hp, sched_stride, S)
 
         # ---- key chain (:255-256, :505-543).  A resumed run (RESUME_FROM) skips the initialiser, the first evaluation,
         # the reset and the memory warm-up: the saved state is copied over the buffers below
@@ -194,10 +195,7 @@ class PQNRnnEngine(EngineBase):
                         _lib.p(la), _lib.p(ac), _lib.p(rw), _lib.p(dn), _lib.p(u.grads), _lib.p(u.loss_sum),
                         _lib.p(u.qsa_sum), S, Tm, Bm, _lib.p(hp["gamma"]), _lib.p(hp["lam"]), _lib.p(ws),
                         _lib.stream_ptr()), "pqn_rnn_loss_grad_seeds")
-                    _lib.check(L.pqn_radam_clip_step_seeds(_lib.p(params), _lib.p(u.grads), _lib.p(u.mu), _lib.p(u.nu),
-                                                           _lib.p(sched), sched_stride, _lib.p(u.step_counter),
-                                                           _lib.p(u.gnorm), S, P, _lib.p(hp["max_norm"]), 0.9, 0.999,
-                                                           1e-8, _lib.stream_ptr()), "pqn_radam_clip_step_seeds")
+                    self._radam_step(params, u, hp, sched_stride, S, P)
             self._end_update(u, r, info_sums)                        # :398
 
         # these runs are launch-bound (32 envs x 64 steps: thousands of small launches per update), so "auto" always

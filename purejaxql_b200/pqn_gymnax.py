@@ -31,12 +31,13 @@ A list-valued ``ENV_NAME`` trains every env of the list in one run (``env_list.p
 """
 from __future__ import annotations
 
-from . import _runner, env_list, envs, state, sweep
+from . import _runner, env_list, envs, pbt, state, sweep
 from .engine import PQNEngine, prepare_config
 
 
 def make_train(config):
     sweep.Grid(config)                       # refuses lists it cannot train before anything is built
+    pbt.settings(config)                     # refuses bad PBT_* settings before anything is built
     if sweep.env_names(config) is not None:  # a list of envs: one engine per env on its own stream (env_list.py)
         return env_list.make_train(config, _make_train_one, envs.check_name)
     return _make_train_one(config)

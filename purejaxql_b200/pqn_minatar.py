@@ -20,7 +20,7 @@ test_metrics, rng), "metrics": {name: [S, NUM_UPDATES]}}``.  A list-valued
 """
 from __future__ import annotations
 
-from . import _runner, env_list, envs, state, sweep
+from . import _runner, env_list, envs, pbt, state, sweep
 from .engine import CNN_NEEDS_MINATAR, PQNEngine, prepare_config
 
 
@@ -33,6 +33,7 @@ def _check_env(name):
 
 def make_train(config):
     sweep.Grid(config)                       # refuses lists it cannot train before anything is built
+    pbt.settings(config)                     # refuses bad PBT_* settings before anything is built
     if sweep.env_names(config) is not None:  # a list of envs: one engine per env on its own stream (env_list.py)
         return env_list.make_train(config, _make_train_one, _check_env)
     return _make_train_one(config)

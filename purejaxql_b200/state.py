@@ -14,7 +14,7 @@ from __future__ import annotations
 import json
 import os
 
-from . import sweep
+from . import pbt, sweep
 
 FORMAT_VERSION = 1
 # the config keys that shape a run, with the value an absent key stands for; a resumed run must match each one
@@ -27,6 +27,7 @@ RUN_KEYS = {
     "SEED": 0, "NUM_SEEDS": 1, "JAX_THREEFRY_PARTITIONABLE": 0,
     "TEST_DURING_TRAINING": False, "TEST_INTERVAL": None, "TEST_NUM_ENVS": None, "TEST_NUM_STEPS": None,
     "EPS_TEST": None, "LR_LINEAR_DECAY": False, "DATA_PARALLEL": "auto",
+    **pbt.DEFAULTS,       # a state file written before PBT existed lacks these keys: it resumes a run without PBT
 }
 
 
@@ -76,8 +77,9 @@ def check_meta(meta: dict, config: dict, script: str, rank: int, world: int, pat
                          f"of {world} (world size); under a multi-GPU launch, write {{rank}} in RESUME_FROM")
     want = run_keys(config)
     for k, v in want.items():
-        if meta["config"].get(k) != v:
-            raise ValueError(f"RESUME_FROM: {k}={v!r} differs from the saved run's {k}={meta['config'].get(k)!r} "
+        saved = meta["config"].get(k, _jsonable(RUN_KEYS[k]))      # a key the saving version lacked: its default
+        if saved != v:
+            raise ValueError(f"RESUME_FROM: {k}={v!r} differs from the saved run's {k}={saved!r} "
                              f"({path}); a resumed run must keep every key that shapes it")
     if int(meta["n_done"]) >= int(meta["num_updates"]):
         raise ValueError(f"{path}: the saved run is finished ({meta['n_done']} of {meta['num_updates']} updates)")

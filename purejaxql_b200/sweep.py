@@ -28,6 +28,7 @@ import numpy as np
 SWEEP_KEYS = ("LR", "MAX_GRAD_NORM", "GAMMA", "LAMBDA", "REW_SCALE", "EPS_START", "EPS_FINISH", "EPS_DECAY")
 MAX_SEEDS = 65535          # the seed axis is gridDim.y of the kernels
 _DEFAULTS = {"REW_SCALE": 1}
+LIST_SETTINGS = ("PBT_PERTURB", "PBT_FACTORS")   # list-valued settings of population-based training, not grid axes
 
 
 def env_names(config: dict) -> list | None:
@@ -52,7 +53,7 @@ class Grid:
     def __init__(self, config: dict):
         env_names(config)
         for k, v in config.items():
-            if isinstance(v, (list, tuple)) and k not in SWEEP_KEYS and k != "ENV_NAME":
+            if isinstance(v, (list, tuple)) and k not in SWEEP_KEYS and k != "ENV_NAME" and k not in LIST_SETTINGS:
                 raise ValueError(f"{k}={v!r}: only {', '.join(SWEEP_KEYS)} may be a list (a grid of settings trained "
                                  f"as one batched run), and ENV_NAME (a list of envs trained side by side); {k} "
                                  f"changes the shapes or the kernels of the run")
